@@ -47,7 +47,7 @@ def workload_config(rv, n_prompts, total_bytes, seed, scale):
     measured properties of the batch (tokens, long pieces ...) are reported under `workload_stats` instead"""
     return {"workload": WORKLOAD, "vocab": rv.label, "vocab_stand_in": rv.stand_in, "prompts_per_gpu": int(n_prompts),
             "total_bytes_per_gpu": int(total_bytes), "seed": int(seed), "scale": float(scale),
-            "l2": "inputs (%.0f MB) and per-byte work arrays (> 1 GB) exceed the 126 MB L2; no flush needed" % (total_bytes / 1e6)}
+            "l2": "inputs (%.0f MB) and per-byte work arrays (> 1 GB) exceed the 50 MB L2 of an H100; no flush needed" % (total_bytes / 1e6)}
 
 
 def peaks():
@@ -55,7 +55,28 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth, 700 W card)"
+
+
+def dump_outputs(out_dir, n_tokens, d_ids, d_out_off, d_counts, n, budget=48 << 20):
+    """What the device leg's last timed step returned, as .npy files: token offsets per prompt (float64, exact), token counts per
+    prompt (float32, exact), and the token ids of a fixed seeded sample of whole prompts (float32: ids < 2**24 are exact), taken
+    in sample order until `budget` bytes of ids; the sampled prompt indices go beside them."""
+    os.makedirs(out_dir, exist_ok=True)
+    off = d_out_off.cpu().numpy().astype(np.uint64)
+    ids = d_ids[:n_tokens].cpu().numpy().view(np.uint32)
+    pick, taken = [], 0
+    for i in np.random.default_rng(0).permutation(n):
+        k = int(off[i + 1] - off[i])
+        if taken + k > budget // 4:
+            break
+        pick.append(int(i)); taken += k
+    pick = np.sort(np.asarray(pick, dtype=np.int64))
+    sample = np.concatenate([ids[int(off[i]):int(off[i + 1])] for i in pick]) if len(pick) else np.zeros(0, np.uint32)
+    np.save(os.path.join(out_dir, "offsets.npy"), off.astype(np.float64))
+    np.save(os.path.join(out_dir, "counts.npy"), d_counts[:n].cpu().numpy().view(np.uint32).astype(np.float32))
+    np.save(os.path.join(out_dir, "ids_sample.npy"), sample.astype(np.float32))
+    np.save(os.path.join(out_dir, "ids_sample_prompts.npy"), pick.astype(np.float64))
 
 
 class ClockSampler:
@@ -169,7 +190,7 @@ def cgroup_throttle():
 def pin_to_gpu_numa_node(local_rank):
     """Run this rank -- and allocate its pinned buffers, which follow the allocating thread's node -- on the CPUs next to its GPU.
     With eight ranks the host leg is bound by the box's PCIe roots and memory: a rank whose buffers sit on the other socket pays
-    the inter-socket link on every copy (SCALE_r01: e2e efficiency 0.87 at N = 8 without pinning).  Returns what was done."""
+    the inter-socket link on every copy.  Returns what was done."""
     try:
         import pynvml
         pynvml.nvmlInit()
@@ -269,6 +290,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-config5", action="store_true", help="skip the extra config-5 record")
     ap.add_argument("--sustain-seconds", type=float, default=2.0, help="extra record: the device leg held this long (0 = skip)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step of the device leg computed to DIR/*.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "cfbpe" else args.warmup
     if args.impl == "reference":
@@ -374,6 +396,8 @@ def main():
     e1.record()
     barrier()
     dev_ms = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0:      # before any later leg writes the same buffers again
+        dump_outputs(args.dump_outputs, int(d_out_off[n].item()), d_ids, d_out_off, d_counts, n)
     total_all = sum_over_ranks(float(total))
     tokens_all = sum_over_ranks(float(n_tokens))
     value = total_all * args.steps / (dev_ms * 1e-3)
@@ -585,18 +609,6 @@ def main():
     }
     dom = max(kms, key=lambda k: kms[k])
     achieved = alg[dom] / (kms[dom] * 1e-3) / 1e9 if kms[dom] > 0 else 0.0
-    # dram bytes of that kernel from the committed `ncu --set full` capture -- only if the capture is of THIS build of the kernels
-    traffic, traffic_note = None, "no ncu capture committed for this build"
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath):
-        try:
-            tj = json.load(open(tpath))
-            if tj.get("build_id") == N.load().cfbpe_build_id().decode():
-                traffic, traffic_note = tj.get(dom), "profiles/ncu_traffic.json (build %s)" % tj.get("build_id")
-            else:
-                traffic_note = "profiles/ncu_traffic.json is of build %s, this is %s: stale, not reported" % (tj.get("build_id"), N.load().cfbpe_build_id().decode())
-        except Exception:
-            traffic = None
     path_alg = total + 4 * n_tokens + 21 * n
     kernels_ms = sum(kms.values())
 
@@ -627,7 +639,7 @@ def main():
         "gpu_launches": 13 * args.steps,   # prompt map, split, split fix-up, long-piece scan, big pieces (list), long pieces, piece-rank scan, piece lookup, short-piece merges, flag_count, tile_scan, emit, offsets
         "kernel_ms": kms,   # CUDA-event durations; bpe_long runs on a second stream next to bpe_encode, so they overlap
         "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": hbm_gbs, "unit": "GB/s", "frac": achieved / hbm_gbs,
-                     "traffic": traffic, "traffic_source": traffic_note, "peak_source": peak_src, "algorithmic_bytes_per_launch": alg[dom],
+                     "peak_source": peak_src, "algorithmic_bytes_per_launch": alg[dom],
                      "path_algorithmic_bytes": path_alg,
                      "path_achieved_gbs": path_alg / (kernels_ms * 1e-3) / 1e9 if kernels_ms > 0 else 0.0},
         "strong": strong, "strong_one_context": strong_lib, "host_cpu": host_cpu, "sustained": sustained,

@@ -1,4 +1,4 @@
-"""Build libcfbpe.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libcfbpe.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -33,7 +33,7 @@ def build(force=False, verbose=False, defines=(), out=None):
     """defines/out: build an experimental variant (A/B timing of kernel parameters) next to the product library"""
     if out is None and not force and not needs_build():
         return SO
-    cmd = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "-Xcompiler", "-fPIC,-fvisibility=hidden,-O2", "-shared", "--cudart", "shared",
            "-Xptxas", "-v" if verbose else "-O3", '-DCFBPE_SRC_HASH="%s"' % source_hash(),
            os.path.join(CSRC, "cfbpe.cu"), os.path.join(CSRC, "vocab.cpp"), "-o", out or SO] + ["-D" + d for d in defines]

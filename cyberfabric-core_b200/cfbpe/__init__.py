@@ -1,4 +1,4 @@
-"""cfbpe -- host side of the B200-native batched BPE tokenizer (cyberfabric-core llm-gateway path).
+"""cfbpe -- host side of the H100-native batched BPE tokenizer (cyberfabric-core llm-gateway path).
 
 `_native`   ctypes binding of libcfbpe.so (the C ABI in include/cfbpe.h)
 `plugin`    Python mirror of the ModKit plugin surface (TokenizerPluginClient, usage meter)

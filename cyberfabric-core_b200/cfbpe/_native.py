@@ -1,5 +1,5 @@
 """ctypes binding of libcfbpe.so (include/cfbpe.h).  No fallback: if the CUDA library is not
-built or no sm_100 device is present, loading / creating a context raises."""
+built or no sm_90 device is present, loading / creating a context raises."""
 import ctypes as C
 import os
 
@@ -159,7 +159,7 @@ class Context:
         h = C.c_void_p()
         rc = L.cfbpe_create(C.byref(cfg), C.byref(h))
         if rc != OK:
-            raise NativeError(rc, "cfbpe_create failed (no sm_100 device visible?)" if rc == ENODEV else
+            raise NativeError(rc, "cfbpe_create failed (no sm_90 device visible?)" if rc == ENODEV else
                               ("cfbpe_create failed: " + L.cfbpe_last_error(None).decode("utf-8", "replace")))
         self._h = h
         self.device = device

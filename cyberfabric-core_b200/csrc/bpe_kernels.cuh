@@ -1,4 +1,4 @@
-// bpe_kernels.cuh -- the encode hot path as CUDA kernels for sm_100a.
+// bpe_kernels.cuh -- the encode hot path as CUDA kernels for sm_90a (H100).
 //
 //   K1  pretok_split_kernel (+ pretok_fixup_kernel)   packed prompt bytes -> piece-start bitmask      (SURVEY.md 8 a1)
 //   K2s long_scan_kernel              finds the pieces longer than 32 bytes (work list of K2b / K2c), counts pieces per 2 KiB tile
@@ -183,8 +183,8 @@ __device__ __forceinline__ uint64_t ascii_digit_run_end(const uint8_t* __restric
 // point of its chunk (prompt start or is_sync_point) and runs the table-driven automaton of
 // pretok_fsm.h, ONE CHARACTER PER ITERATION, until it stands on a sync point at or beyond the end
 // of its chunk -- which is where a later thread started.  All lanes execute the same instruction
-// stream whatever match they are in (the first version walked whole matches per thread: 4.3 of 32
-// lanes active, profiles/ncu_lines_pretok_split_r01a.txt).
+// stream whatever match they are in (the first version walked whole matches per thread: few of the 32
+// lanes were active).
 // ---------------------------------------------------------------------------------------
 // A thread that started in S_W_U (pretok_sync.cuh) and meets an upper-case letter needs the automaton's real state.  Finding
 // it is a look-back of unbounded length: inlined -- or even called -- in the hot loop it cost the kernel registers and 17 %
@@ -208,8 +208,8 @@ __device__ __forceinline__ void split_thread(const BatchView& b, const VocabSet&
         const uint32_t v = b.vocab_ids ? b.vocab_ids[p] : 0u;
         return kMode == 2 ? ((pats2 >> (4u * (v & 7u))) & 15u) : vs.v[v].pattern_id;
     };
-    // (a shared-memory text tile with coalesced 16-byte loads was measured slower here: occupancy fell from 67 % to
-    //  29 % and the accessor cost more than the L1 hits it replaced -- profiles/ncu_summary_r01k.json)
+    // (a shared-memory text tile with coalesced 16-byte loads was measured slower here: occupancy fell by more than half
+    //  and the accessor cost more than the L1 hits it replaced)
     const uint8_t* __restrict__ s = b.bytes;
 
     // (a resumed walker has consumed at least one byte of the prompt it is in: fix_pos may be that prompt's END)
@@ -365,7 +365,7 @@ __device__ __forceinline__ void split_thread(const BatchView& b, const VocabSet&
 #endif
                     const uint32_t d = state - S_D1 + 1u;                        // digits in the current piece so far
                     {   // a boundary every md digits from `first` on: one flag word at a time (the pattern repeats: a loop over
-                        // the boundaries took 200 cycles each, 100 000 for a run of 1.4 KiB -- profiles/k1_tiles_r02.txt)
+                        // the boundaries cost hundreds of cycles each)
                         const uint64_t first = pos + (md - d);
                         const uint32_t pat_bits = md == 1u ? 0xFFFFFFFFu : (md == 2u ? 0x55555555u : 0x49249249u);
                         if (first < e) {
@@ -462,7 +462,7 @@ __device__ __forceinline__ uint64_t next_set_bit(const uint32_t* __restrict__ bi
 // ---------------------------------------------------------------------------------------
 // K2 (lane-per-piece form).  The window kernel above spends ~19 warp-instructions per byte because one
 // lane per BYTE executes the whole-piece lookup and every merge round, while only the head lane of each
-// piece does useful work in the lookup, and a round advances one merge per piece (ncu: profiles/).  Here a
+// piece does useful work in the lookup, and a round advances one merge per piece.  Here a
 // lane owns PIECES:
 //   pass 1  each lane walks the pieces that start in its 16 bytes of the warp's 512-byte range and does
 //           CoreBPE's whole-piece lookup (short table: key = the piece's <= 12 bytes; long table: hash + verify).
@@ -492,7 +492,7 @@ __device__ __forceinline__ void load16(const uint8_t* __restrict__ p, uint32_t& 
 __device__ __forceinline__ uint32_t whole_piece_lookup(const TablesView& T, const uint8_t* __restrict__ p, uint32_t len) {
     if (len > T.max_token_len) return kNone;
     // (a separate path for pieces of <= 4 bytes -- two words loaded instead of five, a two-byte piece as a direct index into the
-    //  byte-pair table -- made K2a 13 % SLOWER: the lanes of a warp then run two paths one after the other; profiles/bench_r02w.json)
+    //  byte-pair table -- made K2a SLOWER: the lanes of a warp then run two paths one after the other)
     uint32_t w0, w1, w2, w3;
     load16(p, w0, w1, w2, w3);
     uint64_t k0 = static_cast<uint64_t>(w0) | (static_cast<uint64_t>(w1) << 32);
@@ -653,7 +653,7 @@ long_scan_kernel(BatchView b, const uint32_t* __restrict__ piece_bits, LongPiece
 //        per class.
 //   K2m  bpe_merge_kernel    the misses, one LANE per piece (merge_piece_in_lane), 32 pieces of one length class per
 //        warp ticket -- in the fused version the merge loops ran with 4-5 active lanes, because a warp only had the
-//        ~15 misses of its own 512 bytes to spread over its lanes (profiles/ncu_lines_bpe_encode_r01n.txt).
+//        ~15 misses of its own 512 bytes to spread over its lanes.
 // ---------------------------------------------------------------------------------------
 constexpr uint32_t kLookupWarps = 4;
 static_assert(kLookupWarps == kPieceWarps, "K2a's CTA is the 2 KiB tile K2s counted");
@@ -708,7 +708,7 @@ bpe_lookup_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ piece_b
             }
             const uint32_t tok = (len == 1) ? T.byte2id[text[pos]] : whole_piece_lookup(T, text + pos, len);   // a byte is a token
             // (leaving the pieces of 13..32 bytes -- hash over the whole piece, byte-wise verify, one or two lanes active here -- to
-            //  K2m, where 32 of them fill a warp, took 0.15 ms off this kernel and put 0.35 ms on that one: profiles/ab_variants_r02x.txt)
+            //  K2m, where 32 of them fill a warp, took less time off this kernel than it put on that one)
             if (tok != kNone) {
                 dn.by_piece[rank0 + i] = tok;          // (its token flag is its piece flag: flag_count_kernel ORs the piece flags in)
             } else {
@@ -751,7 +751,7 @@ bpe_merge_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ piece_bi
     TablesView T = vs.v[0];
     uint32_t vid = 0;
     // (a TMA-staged hot slice of the pair table, probed before the L2-resident table, made this kernel 2x slower:
-    //  profiles/ab_variants_r02k.txt, DESIGN.md section 4)
+    //  DESIGN.md section 4)
 #pragma unroll 1
     for (uint32_t c = 0; c < 3; ++c) {     // longest class first
         const uint32_t n = status->miss_n[c];
@@ -1027,7 +1027,7 @@ constexpr uint32_t kNoKey = 0xFFFFFFFFu;
 // dirty != nullptr (one word per thread): a thread keeps its proposal -- chunk minima, neighbours, the two looked-up pairs --
 // from round to round and recomputes only after its merge was taken, after a conflict, or after another thread's merge wrote
 // into its chunk (the writer marks the owner).  Per round ~20 of 512 proposals are taken; without this the other ~490 threads
-// redid the chunk scan and both table probes every round (160 warp instructions per merge, profiles/ncu_lines_bpe_list_r01n.txt).
+// redid the chunk scan and both table probes every round.
 template <uint32_t kWarps, uint32_t kPosBits>
 __device__ __forceinline__ bool list_rounds_par(const TablesView& T, uint32_t* id, uint32_t* kk, uint32_t* link, uint32_t* claim,
                                                 uint32_t m, uint32_t* s_red, uint32_t* dirty = nullptr) {

@@ -1,6 +1,6 @@
 // cfbpe.cu -- libcfbpe.so: device context, vocab upload and the C ABI of include/cfbpe.h.
 //
-// Built for sm_100a only.  There is no CPU path in this library: every entry point that
+// Built for sm_90a (H100) only.  There is no CPU path in this library: every entry point that
 // computes runs the kernels of bpe_kernels.cuh on the device or returns an error.
 #include <cuda_runtime.h>
 
@@ -58,7 +58,7 @@ constexpr int kTracePoints = 8;     // CFBPE_PIPE_TRACE: events per sub-batch
 #define CFBPE_FRONT_STREAMS 6
 #endif
 constexpr int kFrontStreams = CFBPE_FRONT_STREAMS;
-constexpr uint64_t kPipeChunkBytes = 12ull << 20;   // largest sub-batch of a pipelined host call (the sizes ramp up to it and down again); measured: profiles/e2e_subbatch_sizes_r01t.jsonl
+constexpr uint64_t kPipeChunkBytes = 12ull << 20;   // largest sub-batch of a pipelined host call (the sizes ramp up to it and down again); on H100 8, 16 and 24 MB are within the noise of it
 constexpr uint64_t kPipeMinBytes = 4ull << 20;      // smaller calls run as one shot (a 134 MB batch sharded over 8 GPUs is 16.8 MB a rank: it must still pipeline)
 
 // ---------------------------------------------------------------------------------------
@@ -123,7 +123,7 @@ struct DeviceVocab { uint8_t* d_blob = nullptr; };
 struct DeviceCtx {
     int device = 0;
     int index = 0;                        // position in cfbpe_ctx::devs (= NCCL rank)
-    int sm_count = 148;
+    int sm_count = 0;                     // set from the device's properties; 0 until then
     uint8_t* d_uc1 = nullptr;
     uint8_t* d_uc2 = nullptr;
     uint8_t* d_ascii = nullptr;
@@ -370,7 +370,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         // chain that uses little of the machine, so they start as early as possible and the short-piece kernels fill the rest
         cudaStream_t ss = ln->prio_mode ? ln->pool[lv][(3 * k) % kPoolSlots] : ln->side[k % kSideStreams];
         CK(cudaStreamWaitEvent(ss, ln->ev_h2d[k], 0));
-        enqueue_split(b, dv->vs, dv->uc, w, ss, static_cast<ProfEvents*>(nullptr));
+        enqueue_split(b, dv->vs, dv->uc, w, ss, static_cast<ProfEvents*>(nullptr), static_cast<uint32_t>(dv->sm_count));
         CK(cudaEventRecord(ln->ev_scan[k], ss));
         if (trace) CK(cudaEventRecord(ln->trace[k][1], ss));
         CK(cudaStreamWaitEvent(ck, ln->ev_scan[k], 0));
@@ -740,7 +740,7 @@ bool create_lane(Lane* ln, int device, uint64_t mb, uint64_t mp) {
         }
     }
     // the long-piece kernels are latency-bound and small: their CTAs go first, the short-piece kernels fill the rest
-    // (A/B of lower priorities and of CTA caps: no gain, profiles/ab_bench_r02h.txt)
+    // (A/B of lower priorities and of CTA caps: no gain)
     ok = ok && cudaStreamCreateWithPriority(&ln->aux_stream, cudaStreamNonBlocking, prio_hi) == cudaSuccess;
     ok = ok && cudaStreamCreateWithPriority(&ln->aux2_stream, cudaStreamNonBlocking, prio_hi) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&ln->ev_fork, cudaEventDisableTiming) == cudaSuccess && cudaEventCreateWithFlags(&ln->ev_join, cudaEventDisableTiming) == cudaSuccess;
@@ -765,7 +765,7 @@ bool create_lane(Lane* ln, int device, uint64_t mb, uint64_t mp) {
 bool create_device(DeviceCtx* dv, int device, int index, uint32_t n_lanes, uint64_t mb, uint64_t mp) {
     dv->device = device; dv->index = index;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 10) return false;     // sm_100a SASS only
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) return false;     // sm_90a SASS only
     if (cudaSetDevice(device) != cudaSuccess) return false;
     dv->sm_count = prop.multiProcessorCount;
     bool ok = cudaFuncSetAttribute(bpe_list_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kListSmemBytes)) == cudaSuccess;
@@ -866,7 +866,7 @@ int cfbpe_create(const cfbpe_config* cfg, cfbpe_ctx** out) {
     for (size_t i = 0; i < devices.size(); ++i) {
         ctx->devs.emplace_back(new DeviceCtx());
         if (!create_device(ctx->devs.back().get(), devices[i], static_cast<int>(i), ctx->n_workspaces, ctx->max_bytes, ctx->max_prompts)) {
-            const bool nodev = ctx->devs.back()->sm_count == 148 && ctx->devs.back()->lanes.empty() && !ctx->devs.back()->d_uc1;
+            const bool nodev = ctx->devs.back()->sm_count == 0;     // refused before anything was allocated: not an sm_90 device
             cudaGetLastError();
             cfbpe_destroy(ctx);
             return nodev ? CFBPE_ENODEV : CFBPE_ENOMEM;

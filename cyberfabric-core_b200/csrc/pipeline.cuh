@@ -52,7 +52,7 @@ inline uint64_t miss_list_words(uint64_t max_bytes, uint32_t c, uint32_t max_chu
 #endif
 constexpr uint32_t kLongCtasPerSm = CFBPE_LONG_CTAS;
 #ifndef CFBPE_LIST_CTAS
-#define CFBPE_LIST_CTAS 3      // (2 -> 3: the kernel alone 0.72 -> 0.57 ms, the step unchanged: profiles/ab_bench_r02z.txt)
+#define CFBPE_LIST_CTAS 3      // (H100, 3 vs 2: the kernel alone 0.63 vs 0.80 ms, the step unchanged)
 #endif
 constexpr uint32_t kListCtasPerSm = CFBPE_LIST_CTAS;   // K2c CTAs (64 KB of shared memory each) per SM
 
@@ -71,7 +71,7 @@ inline uint32_t n_scan_tiles(uint64_t total_bytes) {
 //   back    flag_count, tile_scan (chained on the previous sub-batch's token total), emit, prompt offsets
 template <typename Stream, typename Prof>
 inline void enqueue_split(const BatchView& b, const VocabSet& vs, const UcTables& uc, const Workspace& w, Stream stream, Prof* prof,
-                          uint32_t split_grid = 0) {
+                          uint32_t sm_count) {
     const uint64_t nw = n_flag_words(b.total_bytes);
     CFBPE_ZERO(w.status, sizeof(DeviceStatus), stream);
     if (!b.total_bytes) return;
@@ -88,13 +88,13 @@ inline void enqueue_split(const BatchView& b, const VocabSet& vs, const UcTables
         const uint64_t n_blocks16 = (b.total_bytes + 15) / 16;
         const uint32_t n_tiles = static_cast<uint32_t>((n_blocks16 + kSplitWarpOwned - 1) / kSplitWarpOwned);
         const uint32_t n_tabs = b.vocab_ids ? kNumPatterns : 1u;
-        const uint32_t cap = split_grid ? split_grid : 148u * CFBPE_SPLIT_CTAS;      // resident CTAs: 148 SMs x CTAs per SM (launch bounds)
+        const uint32_t cap = sm_count * CFBPE_SPLIT_CTAS;      // resident CTAs: SMs x CTAs per SM (launch bounds)
         const uint32_t n_ctas = (n_tiles + kSplitCta / 32 - 1) / (kSplitCta / 32);
         CFBPE_LAUNCH_SMEM(pretok_split16_kernel, n_ctas < cap ? n_ctas : cap, kSplitCta, n_tabs * kProdTableBytes, stream,
                           b, vs, uc, w.pstart_bits, w.block_prompt, w.piece_bits, w.status, w.fix_list, w.fix_cap, n_tabs, n_tiles);
     }
 #endif
-    CFBPE_LAUNCH(pretok_fixup_kernel, 296u, 256, stream, b, vs, uc, w.piece_bits, w.status, w.fix_list, w.fix_cap);   // almost always empty
+    CFBPE_LAUNCH(pretok_fixup_kernel, 2 * sm_count, 256, stream, b, vs, uc, w.piece_bits, w.status, w.fix_list, w.fix_cap);   // almost always empty
     CFBPE_MARK(prof, K_SPLIT, stream, false);
     const uint64_t n_warps = (b.total_bytes + kPieceRange - 1) / kPieceRange;
     CFBPE_MARK(prof, K_LONGSCAN, stream, true);
@@ -185,7 +185,7 @@ inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTable
                            uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
                            uint32_t long_grid, Stream stream, Stream aux, Stream aux2, Ev ev_fork, Ev ev_join, Ev ev_join2, Prof* prof,
                            const uint64_t* token_base = nullptr) {
-    enqueue_split(b, vs, uc, w, stream, prof);
+    enqueue_split(b, vs, uc, w, stream, prof, long_grid / 4);
     CFBPE_FORK(stream, aux2, ev_fork);
     enqueue_list(b, vs, w, long_grid, aux2, prof);
     CFBPE_FORK(stream, aux, ev_fork);

@@ -1,7 +1,7 @@
 // pretok_lanes.cuh -- K1, second form: the pre-tokenizer split with ONE LANE PER 16 BYTES.
 //
 // The first form (split_thread in bpe_kernels.cuh: a thread per 64-byte chunk, byte loads, a ~170-instruction loop body
-// per character, 15.5 of 32 lanes active -- profiles/ncu_summary_r01s.json) was bound by instruction issue at 2 % of the
+// per character, half the lanes idle) was bound by instruction issue at a small fraction of the
 // HBM roofline.  Here a warp reads 512 contiguous bytes with one 16-byte load per lane, every lane classifies its 16
 // bytes in registers (class table in shared memory), and the automaton of pretok_fsm.h runs in LOCK-STEP over byte
 // indices: iteration k of the unrolled loop handles byte k of every lane's window, so all byte extraction is static and
@@ -136,7 +136,7 @@ __device__ __noinline__ uint32_t pattern_at(const uint64_t* __restrict__ offsets
 
 // What the out-of-line paths need, in shared memory: a call then carries a pointer and the walker's few registers instead of
 // a dozen arguments (the marshalling code sat in the hot loop four times and pushed it out of the 6 KB L0 instruction cache:
-// 54 % of the stall samples were instruction fetches -- profiles/ncu_summary_r02e.json).
+// most stall samples were instruction fetches).
 struct SplitEnv {
     const uint8_t* s; const uint32_t* pstart_bits; const uint32_t* block_prompt; const uint64_t* offsets; const uint8_t* vocab_ids;
     DeviceStatus* status; SplitFix* fix_list;
@@ -216,7 +216,7 @@ __device__ __noinline__ uint4 split_prompt_group(const SplitEnv* env, uint32_t w
 // A walker that crossed its whole 32-byte window (every second tile has one: sixteen spaces of indentation, a nine-digit number) and
 // needs, on average, three or four characters more.  It goes on with the product automaton over the next blocks of 16 bytes, loaded
 // here -- ASCII only, no prompt start inside: anything else is left to the per-character walker, whose set-up alone (prompt
-// search, the classes of the last three characters from memory) costs ~10 000 cycles (profiles/k1_tiles_r02.txt).
+// search, the classes of the last three characters from memory) dwarfs the few characters it walks.
 // Marks at window positions >= 32 go to the flag words directly.  Returns {state row, marks at window positions < 32,
 // remembered positions, blocks done}; state row != 0: the per-character walker goes on at base + 32 + 16 * blocks.
 constexpr uint32_t kSplitExtBlocks = 8;      // window positions stay below 160 (the remembered positions are bytes)
@@ -283,10 +283,10 @@ constexpr uint32_t kSplitWarpOwned = 30;            // blocks of 16 bytes a WARP
 #define CFBPE_SPLIT_CTAS 4
 #endif
 #ifndef CFBPE_SPLIT_TICKETS
-#define CFBPE_SPLIT_TICKETS 1      // 1: warps draw tiles from a counter; 0: fixed stride (A/B: profiles/ab_variants_r02u.txt, 0.846 -> 0.787 ms)
+#define CFBPE_SPLIT_TICKETS 1      // 1: warps draw tiles from a counter; 0: fixed stride (A/B: the ticket is faster)
 #endif
 #ifndef CFBPE_SPLIT_UNROLL
-#define CFBPE_SPLIT_UNROLL 1       // copies of the step in the hot loop (1 | 2 | 4); measured: profiles/ab_variants_r02g.txt
+#define CFBPE_SPLIT_UNROLL 1       // copies of the step in the hot loop (1 | 2 | 4); 2 and 4 measured slower (instruction cache)
 #endif
 __global__ void __launch_bounds__(kSplitCta, CFBPE_SPLIT_CTAS)
 pretok_split16_kernel(BatchView b, VocabSet vs, UcTables uc, const uint32_t* __restrict__ pstart_bits,

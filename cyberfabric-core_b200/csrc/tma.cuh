@@ -1,8 +1,8 @@
-// tma.cuh -- TMA bulk copies (cp.async.bulk global -> shared, completion counted on an mbarrier) as inline PTX for sm_100a.
+// tma.cuh -- TMA bulk copies (cp.async.bulk global -> shared, completion counted on an mbarrier) as inline PTX for sm_90a (H100).
 // One thread arms the barrier with the byte count (mbar_expect_tx) and issues the copies (bulk_g2s: 16-byte granularity and
 // alignment on both sides); every thread that reads the data waits on the barrier's phase (mbar_wait).  SASS: UBLKCP / SYNCS.
 // Used by K1 (its automaton tables).  (Round 2 also staged a hot slice of the pair table for bpe_merge_kernel this way: slower,
-// removed -- profiles/ab_variants_r02k.txt.)
+// removed.)
 // The CPU SIMT emulator has no asynchronous proxy: its builds copy with plain loops instead.
 #pragma once
 #include <stdint.h>

@@ -1,5 +1,5 @@
 /*
- * cfbpe.h -- C ABI of the B200-native batched BPE tokenizer (libcfbpe.so).
+ * cfbpe.h -- C ABI of the H100-native batched BPE tokenizer (libcfbpe.so).
  *
  * This is the drop-in boundary for cyberfabric-core's LLM Gateway tokenizer /
  * usage-meter worker.  The reference tree has no tokenizer code to replace
@@ -33,7 +33,7 @@
  * cfbpe_config.n_workspaces independent call lanes per device (calls wait only when all are
  * busy; vocabulary loads exclude running calls), the last error is kept per thread, and every
  * entry point leaves the caller's current CUDA device as it found it.  There is NO CPU fallback: cfbpe_create fails with
- * CFBPE_ENODEV when no sm_100 device is present.
+ * CFBPE_ENODEV when no sm_90 device is present.
  *
  * Results are bit-exact with tiktoken 0.12.0 CoreBPE.encode_ordinary for the same rank
  * file and pattern (see oracle/ and tests/).
@@ -61,7 +61,7 @@ extern "C" {
 #define CFBPE_ENOENT (-2)    /* unknown vocab id */
 #define CFBPE_EIO (-5)       /* CUDA runtime failure; see cfbpe_last_error */
 #define CFBPE_ENOMEM (-12)
-#define CFBPE_ENODEV (-19)   /* no usable sm_100 device */
+#define CFBPE_ENODEV (-19)   /* no usable sm_90 device */
 #define CFBPE_EINVAL (-22)   /* bad argument: null pointer, non-monotonic offsets, oversize batch, bad rank file */
 #define CFBPE_ENOSPC (-28)   /* out_cap too small; required id count is in out_offsets[n_prompts] */
 #define CFBPE_EILSEQ (-84)   /* a prompt holds malformed UTF-8 (tiktoken only accepts valid text) */

@@ -113,7 +113,7 @@ impl Drop for Ctx {
 }
 
 impl Ctx {
-    /// `devices`: CUDA ordinals (one = single-device context).  Fails with `CFBPE_ENODEV` when no sm_100 device is visible:
+    /// `devices`: CUDA ordinals (one = single-device context).  Fails with `CFBPE_ENODEV` when no sm_90 device is visible:
     /// there is no CPU fallback.
     pub fn create(devices: &[i32], max_batch_bytes: u64, max_prompts: u32, n_workspaces: u32) -> Result<Self, NativeError> {
         let mut cfg = cfbpe_config {
@@ -134,7 +134,7 @@ impl Ctx {
         let rc = unsafe { cfbpe_create(&cfg, &mut raw) };
         match NonNull::new(raw) {
             Some(p) if rc == CFBPE_OK => Ok(Self(p)),
-            _ => Err(NativeError { code: rc, message: "cfbpe_create failed (no sm_100 device visible?)".to_owned() }),
+            _ => Err(NativeError { code: rc, message: "cfbpe_create failed (no sm_90 device visible?)".to_owned() }),
         }
     }
 

@@ -1,4 +1,4 @@
-//! GPU BPE tokenizer plugin (NVIDIA B200, `libcfbpe.so`).
+//! GPU BPE tokenizer plugin (NVIDIA H100, `libcfbpe.so`).
 //!
 //! ```yaml
 //! modules:

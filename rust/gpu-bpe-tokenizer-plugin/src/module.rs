@@ -36,7 +36,7 @@ impl Module for GpuBpeTokenizerPlugin {
         let cfg: GpuBpeTokenizerPluginConfig = ctx.config()?;
 
         // Device context + vocabulary tables.  Blocking (file reads, CUDA allocation, table build: ~1 s per vocabulary): off the runtime.
-        // Fails when no sm_100 device is visible -- there is no CPU fallback, the module must not come up half-working.
+        // Fails when no sm_90 device is visible -- there is no CPU fallback, the module must not come up half-working.
         let cfg_for_service = cfg.clone();
         let service = tokio::task::spawn_blocking(move || Service::from_config(&cfg_for_service)).await??;
         let service = Arc::new(service);

@@ -36,7 +36,7 @@ impl Service {
     /// Blocking: called from `spawn_blocking` in `Module::init`.
     pub fn from_config(cfg: &GpuBpeTokenizerPluginConfig) -> anyhow::Result<Self> {
         let native = Ctx::create(&cfg.devices, cfg.max_batch_bytes, cfg.max_prompts, cfg.workspaces)
-            .map_err(|e| anyhow::anyhow!("no B200 device context (there is no CPU fallback): {e}"))?;
+            .map_err(|e| anyhow::anyhow!("no H100 device context (there is no CPU fallback): {e}"))?;
         let mut slots = HashMap::new();
         let mut names = Vec::new();
         for (slot, v) in cfg.vocabs.iter().enumerate() {

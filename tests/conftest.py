@@ -16,7 +16,7 @@ COMBOS = [(0, 100256), (1, 150000), (2, 128000), (3, 130072)]
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a GPU machine)")
 
 
 @pytest.fixture(scope="session")
