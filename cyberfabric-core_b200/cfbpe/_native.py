@@ -9,7 +9,9 @@ os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")   # effective if CUDA
 _DIR = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("CFBPE_SO_VARIANT") or os.path.join(_DIR, "libcfbpe.so")   # CFBPE_SO_VARIANT: A/B builds (tools only)
 
-OK, ENOENT, EIO, ENOMEM, ENODEV, EINVAL, ENOSPC, EILSEQ = 0, -2, -5, -12, -19, -22, -28, -84
+OK, ENOENT, EIO, ENOMEM, ENODEV, EINVAL, ENOSPC, EILSEQ, EBADMSG = 0, -2, -5, -12, -19, -22, -28, -84, -74
+SPECIAL_ORDINARY, SPECIAL_ALLOW, SPECIAL_DISALLOW = 0, 1, 2      # what an occurrence of a special token means in one call
+MAX_SPECIALS, MAX_SPECIAL_LEN = 4096, 64
 FORMAT_TIKTOKEN, FORMAT_TEKKEN_JSON = 0, 1
 PATTERN_CL100K, PATTERN_O200K, PATTERN_LLAMA3, PATTERN_TEKKEN = 0, 1, 2, 3
 PATTERN_IDS = {"cl100k": 0, "o200k": 1, "llama3": 2, "tekken": 3}
@@ -23,6 +25,7 @@ EXPORTS = [
     "cfbpe_vocab_get_info", "cfbpe_vocab_export", "cfbpe_vocab_import", "cfbpe_encode_batch", "cfbpe_count_batch",
     "cfbpe_encode_batch_device", "cfbpe_device_status", "cfbpe_host_alloc", "cfbpe_host_free",
     "cfbpe_profile_enable", "cfbpe_profile_read", "cfbpe_decode_batch",
+    "cfbpe_vocab_set_specials", "cfbpe_encode_batch_special", "cfbpe_encode_batch_special_device",
 ]
 
 
@@ -97,6 +100,13 @@ def load():
     L.cfbpe_encode_batch_device.restype = C.c_int
     L.cfbpe_encode_batch_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp,
                                             C.POINTER(C.c_uint64), vp]
+    L.cfbpe_vocab_set_specials.restype = C.c_int
+    L.cfbpe_vocab_set_specials.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, vp, vp]
+    L.cfbpe_encode_batch_special.restype = C.c_int
+    L.cfbpe_encode_batch_special.argtypes = [vp, C.c_uint32, u8p, vp, u8p, vp, vp, C.c_uint64, vp, vp, vp]
+    L.cfbpe_encode_batch_special_device.restype = C.c_int
+    L.cfbpe_encode_batch_special_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, C.c_uint64, vp, vp,
+                                                    C.POINTER(C.c_uint64), vp, vp]
     L.cfbpe_device_status.restype = C.c_int
     L.cfbpe_device_status.argtypes = [vp, vp]
     L.cfbpe_host_alloc.restype = vp
@@ -276,6 +286,74 @@ class Context:
                                               C.byref(nt) if sync else None, stream)
         self._check(rc)
         return nt.value if sync else None
+
+    # ---- special tokens
+    @staticmethod
+    def pack_specials(specials):
+        """{str: id} (tiktoken's special_tokens; dict order = special index) -> (bytes uint8, offsets uint64 n+1, ids uint32)"""
+        toks = [t.encode("utf-8") for t in specials]
+        offs = np.zeros(len(toks) + 1, dtype=np.uint64)
+        if toks:
+            offs[1:] = np.cumsum([len(t) for t in toks])
+        data = np.frombuffer(b"".join(toks), dtype=np.uint8).copy() if toks else np.zeros(1, np.uint8)
+        ids = np.asarray([int(v) for v in specials.values()], dtype=np.uint32) if toks else np.zeros(1, np.uint32)
+        return data, offs, ids
+
+    def vocab_set_specials(self, vocab_id, specials):
+        """register {token string: id} as the special tokens of vocabulary slot `vocab_id` (replaces the earlier set; {} clears it)"""
+        data, offs, ids = self.pack_specials(specials)
+        self._check(load().cfbpe_vocab_set_specials(self._h, vocab_id, len(specials), data.ctypes.data, offs.ctypes.data, ids.ctypes.data))
+
+    @staticmethod
+    def _modes_arg(modes):
+        """modes: None (every special of every vocabulary DISALLOWED) or a sequence indexed by vocabulary slot of None / uint8 arrays
+        of one SPECIAL_* byte per registered special -> (ctypes array or None, arrays kept alive)"""
+        if modes is None:
+            return None, []
+        if len(modes) > MAX_VOCABS:
+            raise NativeError(EINVAL, "modes names more than %d vocabularies" % MAX_VOCABS)
+        keep = [None if m is None else np.ascontiguousarray(m, dtype=np.uint8) for m in modes]
+        arr = (C.c_void_p * MAX_VOCABS)(*([None if m is None else m.ctypes.data for m in keep] + [None] * (MAX_VOCABS - len(keep))))
+        return arr, keep
+
+    def encode_batch_special(self, data: np.ndarray, offsets: np.ndarray, vocab_ids=None, modes=None, out_ids=None, out_offsets=None,
+                             out_counts=None, counts_only=False):
+        """tiktoken's encode(allowed_special / disallowed_special) for every prompt: (ids, offsets, counts).  modes: see _modes_arg.
+        NativeError EBADMSG (with .bad = (prompt, special index)) when a prompt spells a DISALLOWED special."""
+        n = self._check_inputs(data, offsets, vocab_ids)
+        total = int(offsets[n])
+        if out_ids is None and not counts_only:
+            out_ids = np.empty(max(total, 1), dtype=np.uint32)
+        if out_offsets is None:
+            out_offsets = np.empty(n + 1, dtype=np.uint64)
+        if out_counts is None:
+            out_counts = np.empty(max(n, 1), dtype=np.uint32)
+        marr, _keep = self._modes_arg(modes)
+        bad = (C.c_uint32 * 2)()
+        vid = None if vocab_ids is None else vocab_ids.ctypes.data
+        rc = load().cfbpe_encode_batch_special(self._h, n, data.ctypes.data if data.size else None, offsets.ctypes.data, vid, marr,
+                                               None if counts_only else out_ids.ctypes.data, 0 if counts_only else out_ids.size,
+                                               out_offsets.ctypes.data, out_counts.ctypes.data, bad)
+        self._check_special(rc, bad)
+        return (None if counts_only else out_ids[:int(out_offsets[n])]), out_offsets, out_counts[:n]
+
+    def encode_batch_special_device(self, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, out_cap,
+                                    d_out_offsets, d_out_counts, modes=None, stream=0, sync=True):
+        """cfbpe_encode_batch_special_device on raw device pointers; returns the id count when sync"""
+        nt = C.c_uint64(0)
+        marr, _keep = self._modes_arg(modes)
+        bad = (C.c_uint32 * 2)()
+        rc = load().cfbpe_encode_batch_special_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, marr,
+                                                      d_out_ids, out_cap, d_out_offsets, d_out_counts,
+                                                      C.byref(nt) if sync else None, bad, stream)
+        self._check_special(rc, bad)
+        return nt.value if sync else None
+
+    def _check_special(self, rc, bad):
+        if rc != OK:
+            e = NativeError(rc, load().cfbpe_last_error(self._h).decode("utf-8", "replace"))
+            e.bad = (int(bad[0]), int(bad[1])) if rc == EBADMSG else None
+            raise e
 
     def device_status(self, stream=0):
         self._check(load().cfbpe_device_status(self._h, stream))

@@ -60,7 +60,7 @@ class VocabNotFound(TokenizerError):
 
 
 def _map_native(e: N.NativeError) -> TokenizerError:
-    if e.code in (N.EINVAL, N.EILSEQ, N.ENOSPC):
+    if e.code in (N.EINVAL, N.EILSEQ, N.ENOSPC, N.EBADMSG):     # EBADMSG: the message names the disallowed special token
         return InvalidInput(str(e))
     if e.code == N.ENOENT:
         return VocabNotFound(str(e))
@@ -189,6 +189,55 @@ class TokenizerPluginClient:
     def decode_batch(self, ctx: SecurityContext, req: "DecodeBatchRequest") -> "DecodeBatchResponse":
         raise NotImplementedError
 
+    def encode_batch_special(self, ctx: SecurityContext, req: EncodeBatchRequest, special_tokens: dict, allowed: set,
+                             disallowed: set) -> EncodeBatchResponse:
+        """tiktoken's `Encoding.encode(text, allowed_special=allowed, disallowed_special=disallowed)` for every prompt of `req`.
+        special_tokens: {"<|endoftext|>": 100257, ...}; allowed / disallowed: sets of token strings (allowed ones have an id).
+        A prompt that holds a disallowed token raises InvalidInput.  This default works on any plugin: it cuts the texts on the
+        host at every occurrence of an allowed token (leftmost first, the longest at a position), encodes the stretches between
+        them with encode_batch -- all stretches of all prompts in ONE batch -- and puts the special ids back in."""
+        import re
+        n = len(req.offsets) - 1
+        try:
+            texts = [bytes(req.bytes[int(req.offsets[i]):int(req.offsets[i + 1])]).decode("utf-8") for i in range(n)]
+        except UnicodeDecodeError as e:
+            raise InvalidInput("a prompt holds malformed UTF-8") from e
+        if disallowed:
+            bad = re.compile("|".join(re.escape(t) for t in sorted(disallowed, key=len, reverse=True)))
+            for t in texts:
+                m = bad.search(t)
+                if m:
+                    raise InvalidInput("the text holds the special token %r, which is not allowed here" % m.group())
+        cut = re.compile("|".join(re.escape(t) for t in sorted(allowed, key=len, reverse=True))) if allowed else None
+        plan, stretches, refs = [], [], []    # per text: list of ("s", stretch index) | ("t", special id)
+        per = req.vocabs_per_prompt
+        if per is not None and req.vocab_index is not None:
+            per = [per[int(k)] for k in req.vocab_index]
+        for i, t in enumerate(texts):
+            steps, pos = [], 0
+            for m in (cut.finditer(t) if cut else ()):
+                if m.start() > pos:
+                    steps.append(("s", len(stretches))); stretches.append(t[pos:m.start()]); refs.append(None if per is None else per[i])
+                steps.append(("t", int(special_tokens[m.group()])))
+                pos = m.end()
+            if pos < len(t):
+                steps.append(("s", len(stretches))); stretches.append(t[pos:]); refs.append(None if per is None else per[i])
+            plan.append(steps)
+        enc = []
+        if stretches:
+            data, offs = pack_texts(stretches)
+            r = self.encode_batch(ctx, EncodeBatchRequest(req.vocab, data, offs, None if per is None else refs))
+            enc = [r.ids[int(r.offsets[i]):int(r.offsets[i + 1])] for i in range(len(stretches))]
+        parts = []
+        for steps in plan:
+            p = [enc[i] if kind == "s" else np.array([i], dtype=np.uint32) for kind, i in steps]
+            parts.append(np.concatenate(p).astype(np.uint32) if p else np.zeros(0, dtype=np.uint32))
+        counts = np.array([len(p) for p in parts], dtype=np.uint32)
+        offsets = np.zeros(n + 1, dtype=np.uint64)
+        offsets[1:] = np.cumsum(counts, dtype=np.uint64)
+        ids = np.concatenate(parts).astype(np.uint32) if parts else np.zeros(0, dtype=np.uint32)
+        return EncodeBatchResponse(ids, offsets, counts)
+
 
 GTS_PLUGIN_SCHEMA = "gts.x.core.modkit.plugin.v1~x.llmgw.tokenizer.plugin.v1~"
 
@@ -258,6 +307,7 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
         except N.NativeError as e:
             raise _map_native(e) from e
         self._slot: Dict[str, int] = {}
+        self._specials: Dict[int, dict] = {}      # slot -> the special tokens registered on it ({str: id}, in registration order)
         self.resolved: Dict[str, V.ResolvedVocab] = {}
         self._lock = threading.Lock()
         self.instance = PluginInstance(
@@ -372,6 +422,32 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
             raise _map_native(e) from e
         return DecodeBatchResponse(out, offs)
 
+    def encode_batch_special(self, ctx: SecurityContext, req: EncodeBatchRequest, special_tokens: dict, allowed: set,
+                             disallowed: set) -> EncodeBatchResponse:
+        """the device path (cfbpe_encode_batch_special): the scan, the cut and the splice run as CUDA kernels.  The caller's
+        special_tokens are registered on every slot the request uses when they differ from what the slot holds."""
+        if not set(disallowed) <= set(special_tokens):      # a disallowed string that is no special token: only the host cut knows it
+            return super().encode_batch_special(ctx, req, special_tokens, allowed, disallowed)
+        self._check_arrays(req)
+        vid = self._vocab_ids(req)
+        n = len(req.offsets) - 1
+        slots = [self._resolve_slot(req.vocab)] if vid is None else sorted(set(int(v) for v in vid[:n]))
+        want = {str(k): int(v) for k, v in special_tokens.items()}
+        modes = [None] * N.MAX_VOCABS
+        m = np.array([N.SPECIAL_DISALLOW if t in disallowed else (N.SPECIAL_ALLOW if t in allowed else N.SPECIAL_ORDINARY) for t in want],
+                     dtype=np.uint8)
+        try:
+            with self._lock:
+                for slot in slots:
+                    if list(self._specials.get(slot, {}).items()) != list(want.items()):      # (the order gives the mode indices)
+                        self.ctx.vocab_set_specials(slot, want)
+                        self._specials[slot] = dict(want)
+                    modes[slot] = m
+                ids, offs, counts = self.ctx.encode_batch_special(req.bytes, req.offsets, vid, modes)
+        except N.NativeError as e:
+            raise _map_native(e) from e
+        return EncodeBatchResponse(ids, offs, counts)
+
     def close(self):
         self.ctx.close()
 
@@ -478,37 +554,17 @@ class LlmGatewayTokenizerService:
         through encode_ordinary -- all stretches of all texts in ONE plugin batch -- and the special ids are put back in.
         special_tokens: {"<|endoftext|>": 100257, ...}; allowed / disallowed: "all" or a set of token strings; a text
         that holds a disallowed special token raises InvalidInput (tiktoken raises ValueError).  Defaults as tiktoken's:
-        nothing allowed, everything disallowed -- user text that spells a control token is refused, not turned into one."""
-        import re
+        nothing allowed, everything disallowed -- user text that spells a control token is refused, not turned into one.
+        The work is the plugin's encode_batch_special: on the GPU plugin the scan, cut and splice run on the device; the trait's
+        default cuts on the host."""
         allowed = set(special_tokens) if allowed_special == "all" else set(allowed_special)
         disallowed = (set(special_tokens) - allowed) if disallowed_special == "all" else set(disallowed_special)
         unknown = allowed - set(special_tokens)
         if unknown:
             raise InvalidInput("allowed special tokens without an id: %s" % sorted(unknown))
-        if disallowed:
-            bad = re.compile("|".join(re.escape(t) for t in sorted(disallowed, key=len, reverse=True)))
-            for t in texts:
-                m = bad.search(t)
-                if m:
-                    raise InvalidInput("the text holds the special token %r, which is not allowed here" % m.group())
-        cut = re.compile("|".join(re.escape(t) for t in sorted(allowed, key=len, reverse=True))) if allowed else None
-        plan, stretches = [], []          # per text: list of ("s", stretch index) | ("t", special id)
-        for t in texts:
-            steps, pos = [], 0
-            for m in (cut.finditer(t) if cut else ()):
-                if m.start() > pos:
-                    steps.append(("s", len(stretches))); stretches.append(t[pos:m.start()])
-                steps.append(("t", int(special_tokens[m.group()])))
-                pos = m.end()
-            if pos < len(t):
-                steps.append(("s", len(stretches))); stretches.append(t[pos:])
-            plan.append(steps)
-        enc = self.encode(ctx, model, stretches) if stretches else []
-        out = []
-        for steps in plan:
-            parts = [enc[i] if kind == "s" else np.array([i], dtype=np.uint32) for kind, i in steps]
-            out.append(np.concatenate(parts).astype(np.uint32) if parts else np.zeros(0, dtype=np.uint32))
-        return out
+        data, offs = pack_texts(texts)
+        r = self._plugin().encode_batch_special(ctx, EncodeBatchRequest(VocabRef(model), data, offs), special_tokens, allowed, disallowed)
+        return [r.ids[int(r.offsets[i]):int(r.offsets[i + 1])] for i in range(len(texts))]
 
     def check_budget(self, ctx: SecurityContext, model: str, messages: Sequence[dict], remaining_tokens: int) -> bool:
         """pre-call estimate used by check_budget (modules/llm-gateway/docs/DESIGN.md:833-855)"""

@@ -21,6 +21,7 @@
 #include "pretok.cuh"
 #include "pretok_fsm.h"
 #include "pretok_sync.cuh"
+#include "specials.h"
 #include "tables.h"
 #include "tma.cuh"
 
@@ -1687,7 +1688,8 @@ struct DecodeView {
 };
 
 __global__ void __launch_bounds__(256)
-decode_len_kernel(DecodeView d, VocabSet vs, uint32_t* __restrict__ lens, uint32_t* __restrict__ tile_sums, DeviceStatus* status) {
+decode_len_kernel(DecodeView d, VocabSet vs, uint32_t* __restrict__ lens, uint32_t* __restrict__ tile_sums, DeviceStatus* status,
+                  SpecialSet sp = SpecialSet{}) {
     __shared__ uint32_t s_tmp[8];
     const uint64_t base = static_cast<uint64_t>(blockIdx.x) * kDecodeTile;
     uint32_t sum = 0;
@@ -1700,7 +1702,11 @@ decode_len_kernel(DecodeView d, VocabSet vs, uint32_t* __restrict__ lens, uint32
         const uint32_t id = d.ids[i];
         uint32_t len = 0;
         if (id < T.n_ranks) len = T.tokoff[id + 1] - T.tokoff[id];
-        else atomicOr(&status->bad_utf8, 1u);          // reported as "unknown token id" by the decode entry point
+        else {                                          // not an ordinary token: a special token of the vocabulary, or unknown
+            const int k = sp_by_id(sp.v[vid], id);
+            if (k >= 0) len = sp_len(sp.v[vid], static_cast<uint32_t>(k));
+            else atomicOr(&status->bad_utf8, 1u);      // reported as "unknown token id" by the decode entry point
+        }
         lens[i] = len;
         sum += len;
     }
@@ -1710,7 +1716,7 @@ decode_len_kernel(DecodeView d, VocabSet vs, uint32_t* __restrict__ lens, uint32
 
 __global__ void __launch_bounds__(256)
 decode_copy_kernel(DecodeView d, VocabSet vs, const uint32_t* __restrict__ lens, const uint64_t* __restrict__ tile_base,
-                   uint8_t* __restrict__ out, uint64_t out_cap) {
+                   uint8_t* __restrict__ out, uint64_t out_cap, SpecialSet sp = SpecialSet{}) {
     __shared__ uint32_t s_warp[8];
     const uint64_t base = static_cast<uint64_t>(blockIdx.x) * kDecodeTile + 4ull * threadIdx.x;   // my four consecutive tokens
     uint32_t l[4], mine = 0;
@@ -1731,7 +1737,9 @@ decode_copy_kernel(DecodeView d, VocabSet vs, const uint32_t* __restrict__ lens,
         uint32_t vid = 0;
         if (d.vocab_ids) vid = d.vocab_ids[find_prompt(d.id_offsets, d.n_seqs, base + t)];
         const TablesView& T = vs.v[vid];
-        const uint8_t* src = T.blob + T.tokoff[d.ids[base + t]];
+        const uint32_t id = d.ids[base + t];
+        const uint8_t* src = id < T.n_ranks ? T.blob + T.tokoff[id]
+                                            : sp_bytes(sp.v[vid]) + sp.v[vid].w[sp.v[vid].o_offs + sp_by_id(sp.v[vid], id)];   // a special token
         for (uint32_t k = 0; k < l[t]; ++k) if (o + k < out_cap) out[o + k] = src[k];
         o += l[t];
     }

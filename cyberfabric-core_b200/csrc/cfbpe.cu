@@ -26,6 +26,7 @@ static inline void prof_mark(ProfEvents* p, int idx, cudaStream_t s, bool begin)
 
 #include "pipeline.cuh"
 #include "pretok_ctx.h"
+#include "specials.cuh"
 #include "subbatch.h"
 #include "unicode_tables.h"
 #include "vocab.h"
@@ -73,6 +74,23 @@ constexpr uint64_t kPipeMinBytes = 4ull << 20;      // smaller calls run as one 
 // libnccl.so.2: the library links no NCCL symbol) broadcasts the packed tables at vocab load and all-gathers the per-shard
 // token totals of every batch, from which each device rebases its offsets (SURVEY.md section 8(e)).
 // ---------------------------------------------------------------------------------------
+// the buffers of special-token calls (cfbpe_encode_batch_special*), allocated on the lane's first such call: a context that
+// never uses special tokens keeps the footprint it had
+struct LaneSpecial {
+    bool ready = false;
+    uint32_t* kept_n = nullptr;           // [max_prompts] kept matches per prompt ...
+    uint64_t* kept_base = nullptr;        // ... and their exclusive scan
+    uint64_t* st_off = nullptr;           // [max_prompts + 1] stretch byte offsets
+    uint8_t* st_vocab = nullptr;          // [max_prompts] stretch vocabularies
+    uint32_t* st_id = nullptr;            // [max_prompts] special id of a stretch, or kSpText
+    uint64_t* st_base = nullptr;          // [max_prompts] first output id of a stretch
+    uint64_t* fin_offsets = nullptr;      // host calls: the prompts' offsets [max_prompts + 1] ...
+    uint32_t* fin_counts = nullptr;       // ... and counts [max_prompts]
+    uint8_t* modes = nullptr;             // [CFBPE_MAX_VOCABS][kMaxSpecials] the call's mode bytes
+    SpecialStatus* status = nullptr;
+    SpecialStatus* h_status = nullptr;    // pinned
+};
+
 struct Lane {
     std::mutex mu;                        // held for the duration of a call
     int device = 0;
@@ -116,6 +134,7 @@ struct Lane {
     Workspace ws{};
     DeviceStatus* h_status = nullptr;  // pinned
     ProfEvents prof{};
+    LaneSpecial sp;
 };
 
 struct DeviceVocab { uint8_t* d_blob = nullptr; };
@@ -132,6 +151,8 @@ struct DeviceCtx {
     UcTables uc{};
     DeviceVocab vocabs[CFBPE_MAX_VOCABS];
     VocabSet vs{};
+    uint32_t* d_specials[CFBPE_MAX_VOCABS] = {};   // each vocabulary's special-token table (specials.h), or nullptr
+    SpecialSet specials{};                          // their views (modes NULL): what decode reads
     std::vector<std::unique_ptr<Lane>> lanes;
     std::atomic<uint32_t> next_lane{0};
     void* comm = nullptr;                 // ncclComm_t of this device in the context's communicator
@@ -156,6 +177,7 @@ struct cfbpe_ctx {
     std::vector<std::unique_ptr<DeviceCtx>> devs;
     std::shared_mutex vocab_mu;           // calls: shared; vocabulary load / import: exclusive
     HostVocab vocabs[CFBPE_MAX_VOCABS];
+    std::vector<uint32_t> specials[CFBPE_MAX_VOCABS];   // the special-token tables (host copies; empty = none registered)
     uint32_t loaded_mask = 0;
     uint64_t max_bytes = 0;
     uint32_t max_prompts = 0;
@@ -220,6 +242,21 @@ int validate_batch(cfbpe_ctx* ctx, uint32_t n, const uint64_t* offsets, const ui
     return CFBPE_OK;
 }
 
+// Drop the special-token table of a vocabulary on every device (caller holds vocab_mu exclusively)
+void clear_specials(cfbpe_ctx* ctx, uint32_t vocab_id) {
+    ctx->specials[vocab_id].clear();
+    for (auto& dvp : ctx->devs) {
+        DeviceCtx* dv = dvp.get();
+        dv->specials.v[vocab_id] = SpecialView{};
+        if (dv->d_specials[vocab_id]) {
+            cudaSetDevice(dv->device);
+            cudaDeviceSynchronize();          // a device-path call may still read the table
+            cudaFree(dv->d_specials[vocab_id]);
+            dv->d_specials[vocab_id] = nullptr;
+        }
+    }
+}
+
 // Install a packed table blob as vocabulary vocab_id on EVERY device of the context (caller holds vocab_mu exclusively).
 // Device 0 gets it from the host; with several devices the others get it from device 0 by ncclBroadcast over NVLink -- the rank
 // file was parsed once, the tables crossed PCIe once.
@@ -250,6 +287,7 @@ int install_blob(cfbpe_ctx* ctx, uint32_t vocab_id, std::vector<uint8_t>&& blob)
         for (size_t d = 0; d < G; ++d) { cudaSetDevice(ctx->devs[d]->device); if (cudaStreamSynchronize(ctx->devs[d]->lanes[0]->stream) != cudaSuccess && rc == 0) rc = -1; }
         if (rc != 0) { cleanup(); return fail(ctx, CFBPE_EIO, std::string("ncclBroadcast of the vocabulary tables: ") + (rc > 0 ? nc.GetErrorString(rc) : "stream error")); }
     }
+    clear_specials(ctx, vocab_id);           // a new vocabulary starts without special tokens
     HostVocab& hv = ctx->vocabs[vocab_id];
     hv.h_blob = std::move(blob);
     std::memcpy(&hv.hdr, hv.h_blob.data(), sizeof(TablesHeader));
@@ -497,6 +535,83 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     return CFBPE_OK;
 }
 
+// ---------------------------------------------------------------------------------------
+// special tokens (specials.h, specials.cuh)
+// ---------------------------------------------------------------------------------------
+int fail_disallowed(cfbpe_ctx* ctx, uint32_t prompt, uint32_t vid, uint32_t k, uint32_t* out_bad) {
+    if (out_bad) { out_bad[0] = prompt; out_bad[1] = k; }
+    std::string tok;
+    const std::vector<uint32_t>& w = ctx->specials[vid < CFBPE_MAX_VOCABS ? vid : 0];
+    if (!w.empty() && k < w[0]) {
+        const uint8_t* sb = reinterpret_cast<const uint8_t*>(w.data() + w[11]);
+        tok.assign(reinterpret_cast<const char*>(sb + w[w[8] + k]), w[w[8] + k + 1] - w[w[8] + k]);
+    }
+    return fail(ctx, CFBPE_EBADMSG, "prompt " + std::to_string(prompt) + " holds the special token " + tok + " (index " + std::to_string(k) +
+                                    "), which this call disallows");
+}
+
+int ensure_special_lane(cfbpe_ctx* ctx, Lane* ln) {
+    LaneSpecial& sp = ln->sp;
+    if (sp.ready) return CFBPE_OK;
+    const uint64_t mp = ctx->max_prompts;
+    bool ok = dmalloc(&sp.kept_n, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(&sp.kept_base, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(&sp.st_off, mp + 2) == cudaSuccess;
+    ok = ok && dmalloc(&sp.st_vocab, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(&sp.st_id, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(&sp.st_base, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(&sp.fin_offsets, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(&sp.fin_counts, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(&sp.modes, static_cast<uint64_t>(CFBPE_MAX_VOCABS) * kMaxSpecials) == cudaSuccess;
+    ok = ok && dmalloc(&sp.status, 1) == cudaSuccess;
+    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&sp.h_status), sizeof(SpecialStatus)) == cudaSuccess;
+    if (!ok) { cudaGetLastError(); return fail(ctx, CFBPE_ENOMEM, "no device memory for the special-token buffers"); }
+    sp.ready = true;
+    return CFBPE_OK;
+}
+
+void free_special_lane(Lane* ln) {
+    LaneSpecial& sp = ln->sp;
+    cudaFree(sp.kept_n); cudaFree(sp.kept_base); cudaFree(sp.st_off); cudaFree(sp.st_vocab); cudaFree(sp.st_id); cudaFree(sp.st_base);
+    cudaFree(sp.fin_offsets); cudaFree(sp.fin_counts); cudaFree(sp.modes); cudaFree(sp.status);
+    if (sp.h_status) cudaFreeHost(sp.h_status);
+    sp = LaneSpecial{};
+}
+
+SpecialWork special_work(Lane* ln) {
+    const LaneSpecial& sp = ln->sp;
+    return SpecialWork{sp.kept_n, sp.kept_base, sp.st_off, sp.st_vocab, sp.st_id, sp.st_base, sp.status};
+}
+
+// The special set of one call on device dv: the tables of the vocabularies that look for some special in it (every registered
+// special is DISALLOWED when modes[v] is NULL), the call's mode bytes uploaded into the lane.  *scan = false: no vocabulary looks
+// for any special, the call is the ordinary path.
+int special_set(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const uint8_t* const* modes, SpecialSet* out, bool* scan, cudaStream_t s) {
+    *out = SpecialSet{};
+    *scan = false;
+    for (uint32_t v = 0; v < CFBPE_MAX_VOCABS; ++v) {
+        const std::vector<uint32_t>& w = ctx->specials[v];
+        if (w.empty()) continue;
+        const uint32_t n = w[0];
+        const uint8_t* m = modes ? modes[v] : nullptr;
+        if (m) {
+            bool looks = false;
+            for (uint32_t k = 0; k < n; ++k) {
+                if (m[k] > CFBPE_SPECIAL_DISALLOW) return fail(ctx, CFBPE_EINVAL, "modes[" + std::to_string(v) + "][" + std::to_string(k) + "] is not a CFBPE_SPECIAL_* value");
+                looks = looks || m[k] != CFBPE_SPECIAL_ORDINARY;
+            }
+            if (!looks) continue;
+            uint8_t* dm = ln->sp.modes + static_cast<uint64_t>(v) * kMaxSpecials;
+            CK(cudaMemcpyAsync(dm, m, n, cudaMemcpyHostToDevice, s));
+            out->modes[v] = dm;
+        }
+        out->v[v] = dv->specials.v[v];
+        for (uint32_t j = 0; j < 8; ++j) out->first_bytes[j] |= w[kSpHeaderWords + j];
+        *scan = true;
+    }
+    return CFBPE_OK;
+}
+
 // offsets of a shard are ranks inside the shard: add the tokens of the shards before it (the all-gathered totals)
 __global__ void rebase_offsets_kernel(uint64_t* __restrict__ offsets, uint64_t n, const uint64_t* __restrict__ totals, uint32_t shard) {
     uint64_t base = 0;
@@ -509,8 +624,16 @@ __global__ void rebase_offsets_kernel(uint64_t* __restrict__ offsets, uint64_t n
 // bytes; every device runs its shard on its own host thread and lane (uploads, kernels), the per-shard token totals are
 // all-gathered with NCCL (8 bytes a device: the path's only exchange), every device rebases its offsets by the totals of the
 // shards before it and downloads ids, offsets and counts straight to their final places in the caller's buffers.
+int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                     const uint8_t* const* modes, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
+                     uint64_t total, uint32_t* out_bad, uint64_t* defer);
+
+// special != nullptr: a special-token call (cfbpe_encode_batch_special): every shard runs its own special pass; special->modes
+// are the call's modes, special->bad gets the prompt and special index of a CFBPE_EBADMSG
+struct SpecialArgs { const uint8_t* const* modes; uint32_t* bad; };
 int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
-                     uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total) {
+                     uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
+                     const SpecialArgs* special = nullptr) {
     const uint32_t G = static_cast<uint32_t>(ctx->devs.size());
     std::vector<uint32_t> lo(G + 1, 0);
     for (uint32_t d = 1; d < G; ++d) {      // first prompt whose start is >= d * total / G
@@ -522,7 +645,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     lo[G] = n;
     for (uint32_t d = 0; d < G; ++d)
         if (offsets[lo[d + 1]] - offsets[lo[d]] > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "a device's shard exceeds max_batch_bytes (one prompt is too large to balance)");
-    struct Shard { int rc = CFBPE_OK; std::string err; uint64_t tokens = 0; std::vector<uint64_t> local_offs; uint32_t cut[kMaxPipeChunks + 1]; int nc = 0; };
+    struct Shard { int rc = CFBPE_OK; std::string err; uint64_t tokens = 0; std::vector<uint64_t> local_offs; uint32_t cut[kMaxPipeChunks + 1]; int nc = 0; uint32_t bad[2] = {}; };
     std::vector<Shard> sh(G);
     std::vector<std::unique_ptr<LaneLock>> locks(G);
     for (uint32_t d = 0; d < G; ++d) locks[d].reset(new LaneLock(ctx->devs[d].get()));
@@ -535,12 +658,23 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             const uint64_t o0 = offsets[p0];
             s.local_offs.resize(static_cast<size_t>(nd) + 1);
             for (uint32_t i = 0; i <= nd; ++i) s.local_offs[i] = offsets[p0 + i] - o0;
-            s.rc = run_lane(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
-                            nullptr, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc);
+            if (special) {
+                s.rc = run_lane_special(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
+                                        special->modes, nullptr, 0, nullptr, nullptr, want_ids, s.local_offs[nd], s.bad, &s.tokens);
+                s.cut[0] = 0; s.cut[1] = nd; s.nc = 1;
+            } else {
+                s.rc = run_lane(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
+                                nullptr, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc);
+            }
             if (s.rc) s.err = tl_err;
         });
         for (auto& t : th) t.join();
     }
+    for (uint32_t d = 0; d < G && special; ++d)        // a disallowed special wins over every other error, the lowest prompt first
+        if (sh[d].rc == CFBPE_EBADMSG) {
+            const uint32_t p = sh[d].bad[0] + lo[d];
+            return fail_disallowed(ctx, p, vocab_ids ? vocab_ids[p] : 0u, sh[d].bad[1], special->bad);
+        }
     for (uint32_t d = 0; d < G; ++d) if (sh[d].rc) return fail(ctx, sh[d].rc, sh[d].err);
     // ---- phase 2: all-gather of the token totals (NCCL, 8 bytes a device), rebase, download to the final places
     const NcclApi& nc = ctx->nccl;
@@ -629,12 +763,115 @@ int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* o
     return run_lane(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total);
 }
 
+
+// A special-token host call on one lane (the whole call on a single-device context, one shard of a multi-device one), as one pass:
+// upload, scan (when some vocabulary looks for a special), then the ordinary path on the prompts as they are (no kept match) or
+// on the stretches followed by the splice, download.  defer: see run_lane (the results are left in the lane's d_out_* buffers).
+int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                     const uint8_t* const* modes, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
+                     uint64_t total, uint32_t* out_bad, uint64_t* defer) {
+    CK(cudaSetDevice(dv->device));
+    if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }
+    int rc = ensure_special_lane(ctx, ln);
+    if (rc) return rc;
+    cudaStream_t s = ln->stream;
+    SpecialSet sp;
+    bool scan = false;
+    rc = special_set(ctx, dv, ln, modes, &sp, &scan, s);
+    if (rc) return rc;
+    if (total) CK(cudaMemcpyAsync(ln->d_bytes, bytes, total, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ln->d_offsets, offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    if (vocab_ids && n) CK(cudaMemcpyAsync(ln->d_vocab_ids, vocab_ids, n, cudaMemcpyHostToDevice, s));
+    const BatchView b{ln->d_bytes, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n, total};
+    const SpecialWork sw = special_work(ln);
+    uint64_t n_str = n;
+    if (scan) {
+        enqueue_special_scan(b, sp, ln->ws, sw, s);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        const SpecialStatus ss = *ln->sp.h_status;
+        if (ss.bad_inv) {
+            const unsigned long long key = ~ss.bad_inv;
+            return fail_disallowed(ctx, ss.bad_prompt, static_cast<uint32_t>((key >> 12) & 7u), static_cast<uint32_t>(key & 0xFFFu), out_bad);
+        }
+        n_str = n + 2 * ss.kept.n_tokens;
+        if (n_str > ctx->max_prompts)
+            return fail(ctx, CFBPE_EINVAL, "n_prompts + 2 x special-token matches (" + std::to_string(n_str) + ") exceeds max_prompts of this context");
+    }
+    const bool spliced = n_str != n;
+    const uint32_t grid = static_cast<uint32_t>(dv->sm_count * 4);
+    if (!spliced) {
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets, ln->d_out_counts, grid,
+                       s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+    } else {
+        enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets,
+                               ln->d_out_counts, want_ids ? ln->ws.lscratch.rank : nullptr, ctx->max_bytes, ln->sp.fin_offsets, ln->sp.fin_counts,
+                               grid, s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    const DeviceStatus st = *ln->h_status;
+    if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
+    if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
+    if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
+    const uint64_t n_tokens = spliced ? ln->sp.h_status->fin.n_tokens : st.n_tokens;
+    // where the call's ids, offsets and counts are on the device
+    const uint32_t* ids_src = spliced ? ln->ws.lscratch.rank : ln->d_out_ids;
+    const uint64_t* offs_src = spliced ? ln->sp.fin_offsets : ln->d_out_offsets;
+    const uint32_t* counts_src = spliced ? ln->sp.fin_counts : ln->d_out_counts;
+    if (defer) {       // a shard of a multi-device call: its results go where run_multi_device downloads them from
+        if (spliced) {
+            if (want_ids && n_tokens) CK(cudaMemcpyAsync(ln->d_out_ids, ids_src, n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+            CK(cudaMemcpyAsync(ln->d_out_offsets, offs_src, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+            if (n) CK(cudaMemcpyAsync(ln->d_out_counts, counts_src, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+            CK(cudaStreamSynchronize(s));
+        }
+        *defer = n_tokens;
+        return CFBPE_OK;
+    }
+    if (out_offsets) CK(cudaMemcpyAsync(out_offsets, offs_src, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+    if (out_counts && n) CK(cudaMemcpyAsync(out_counts, counts_src, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    if (want_ids && n_tokens > out_cap) {
+        CK(cudaStreamSynchronize(s));
+        if (out_offsets) out_offsets[n] = n_tokens;
+        return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(n_tokens) + " ids");
+    }
+    if (want_ids && n_tokens) CK(cudaMemcpyAsync(out_ids, ids_src, n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return CFBPE_OK;
+}
+
+// shared body of the special-token host calls
+int run_host_special(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids, const uint8_t* const* modes,
+                     uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, uint32_t* out_bad) {
+    tl_err.clear();
+    std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
+    uint64_t total = 0;
+    int rc = validate_batch(ctx, n, offsets, vocab_ids, &total);
+    if (rc) return rc;
+    const bool want_ids = out_ids != nullptr;
+    if (total && !bytes) return fail(ctx, CFBPE_EINVAL, "bytes is NULL");
+    if (!out_offsets) return fail(ctx, CFBPE_EINVAL, "out_offsets is NULL");
+    if (ctx->devs.size() > 1 && n >= ctx->devs.size()) {    // one contiguous shard a device, each with its own special pass
+        const SpecialArgs sa{modes, out_bad};
+        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total, &sa);
+    }
+    if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds max_batch_bytes of this context");
+    DeviceCtx* dv = ctx->devs[0].get();
+    LaneLock lk(dv);
+    return run_lane_special(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, modes, out_ids, out_cap, out_offsets, out_counts, want_ids, total, out_bad, nullptr);
+}
+
 // ---------------------------------------------------------------------------------------
 // construction / destruction
 // ---------------------------------------------------------------------------------------
 void destroy_lane(Lane* ln) {
     if (!ln) return;
     cudaSetDevice(ln->device);
+    free_special_lane(ln);
     cudaFree(ln->d_bytes); cudaFree(ln->d_offsets); cudaFree(ln->d_vocab_ids);
     cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts);
     cudaFree(ln->ws.piece_bits); cudaFree(ln->ws.tok_bits); cudaFree(ln->ws.ids_by_pos);
@@ -910,6 +1147,7 @@ void cfbpe_destroy(cfbpe_ctx* ctx) {
         cudaSetDevice(dv->device);
         cudaFree(dv->d_uc1); cudaFree(dv->d_uc2); cudaFree(dv->d_ascii); cudaFree(dv->d_fsm); cudaFree(dv->d_split_tables);
         for (auto& v : dv->vocabs) { if (v.d_blob) cudaFree(v.d_blob); }
+        for (auto* t : dv->d_specials) cudaFree(t);
     }
     delete ctx;
 }
@@ -1017,9 +1255,9 @@ int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, con
     CK(cudaMemsetAsync(ln->ws.status, 0, sizeof(DeviceStatus), s));
     DecodeView d{ln->d_out_ids, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n_seqs, n_ids};
     const uint32_t n_tiles = static_cast<uint32_t>((n_ids + kDecodeTile - 1) / kDecodeTile);
-    if (n_tiles) decode_len_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_sums, ln->ws.status);
+    if (n_tiles) decode_len_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_sums, ln->ws.status, dv->specials);
     tile_scan_kernel<<<1, n_tiles ? 1024 : 32, 0, s>>>(ln->d_dec_sums, n_tiles, ln->d_dec_base, ln->ws.status, nullptr);
-    if (n_tiles) decode_copy_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_base, ln->d_bytes, ctx->max_bytes);
+    if (n_tiles) decode_copy_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_base, ln->d_bytes, ctx->max_bytes, dv->specials);
     decode_offsets_kernel<<<static_cast<unsigned>((static_cast<uint64_t>(n_seqs) + 1 + 255) / 256), 256, 0, s>>>(d, ln->ws.ids_by_pos, ln->d_dec_base, ln->d_out_offsets, ln->ws.status);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
@@ -1081,6 +1319,121 @@ int cfbpe_encode_batch_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t*
         if (prof) fill_profile(ln, total_bytes);
         const DeviceStatus st = *ln->h_status;
         if (n_tokens) *n_tokens = st.n_tokens;
+        if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
+        if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
+        if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
+        if (d_out_ids && st.n_tokens > out_cap) return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(st.n_tokens) + " ids");
+    }
+    return CFBPE_OK;
+}
+
+int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* ids) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (vocab_id >= CFBPE_MAX_VOCABS) return fail(ctx, CFBPE_EINVAL, "vocab_id out of range");
+    std::vector<uint32_t> words;
+    std::string e;
+    const int rc = build_special_table(n, bytes, offsets, ids, words, e);
+    if (rc) return fail(ctx, rc, e);
+    std::unique_lock<std::shared_mutex> lock(ctx->vocab_mu);
+    if (!ctx->vocabs[vocab_id].loaded) return fail(ctx, CFBPE_ENOENT, "vocab " + std::to_string(vocab_id) + " is not loaded");
+    const size_t G = ctx->devs.size();
+    std::vector<uint32_t*> nt(G, nullptr);
+    if (!words.empty()) {
+        for (size_t d = 0; d < G; ++d) {      // a plain copy to every device: the table is a few KB
+            cudaSetDevice(ctx->devs[d]->device);
+            cudaError_t ce = dmalloc(&nt[d], words.size());
+            if (ce == cudaSuccess) ce = cudaMemcpy(nt[d], words.data(), words.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
+            if (ce != cudaSuccess) {
+                for (size_t k = 0; k <= d; ++k) { cudaSetDevice(ctx->devs[k]->device); cudaFree(nt[k]); }
+                cudaGetLastError();
+                return fail(ctx, CFBPE_ENOMEM, std::string("special-token table upload: ") + cudaGetErrorString(ce));
+            }
+        }
+    }
+    clear_specials(ctx, vocab_id);
+    ctx->specials[vocab_id] = std::move(words);
+    for (size_t d = 0; d < G; ++d) {
+        DeviceCtx* dv = ctx->devs[d].get();
+        dv->d_specials[vocab_id] = nt[d];
+        dv->specials.v[vocab_id] = make_special_view(nt[d], ctx->specials[vocab_id]);
+    }
+    return CFBPE_OK;
+}
+
+int cfbpe_encode_batch_special(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                               const uint8_t* const* modes, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
+                               uint32_t* out_bad) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    return run_host_special(ctx, n_prompts, bytes, offsets, vocab_ids, modes, out_ids, out_cap, out_offsets, out_counts, out_bad);
+}
+
+int cfbpe_encode_batch_special_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                                      const uint8_t* d_vocab_ids, const uint8_t* const* modes, uint32_t* d_out_ids, uint64_t out_cap,
+                                      uint64_t* d_out_offsets, uint32_t* d_out_counts, uint64_t* n_tokens, uint32_t* out_bad, void* stream) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
+    if (n_prompts > ctx->max_prompts || total_bytes > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds the limits of this context");
+    if (!d_offsets || !d_out_offsets || (total_bytes && !d_bytes)) return fail(ctx, CFBPE_EINVAL, "device pointer is NULL");
+    if (!ctx->vocabs[0].loaded && !d_vocab_ids) return fail(ctx, CFBPE_ENOENT, "vocab 0 is not loaded");
+    if (!ctx->loaded_mask) return fail(ctx, CFBPE_ENOENT, "no vocabulary is loaded");
+    DeviceCtx* dv = ctx->devs[0].get();
+    { int cur = -1; if (cudaGetDevice(&cur) == cudaSuccess) for (auto& d : ctx->devs) if (d->device == cur) dv = d.get(); }
+    LaneLock lk(dv);
+    Lane* ln = lk.ln;
+    CK(cudaSetDevice(dv->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws, 0));
+    int rc = ensure_special_lane(ctx, ln);
+    if (rc) return rc;
+    SpecialSet sp;
+    bool scan = false;
+    rc = special_set(ctx, dv, ln, modes, &sp, &scan, s);
+    if (rc) return rc;
+    const BatchView b{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes};
+    const SpecialWork sw = special_work(ln);
+    uint64_t n_str = n_prompts;
+    if (scan) {       // the one synchronisation of the call: the host needs the number of stretches for the launch geometry
+        enqueue_special_scan(b, sp, ln->ws, sw, s);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        ln->ws_pending = false;
+        const SpecialStatus ss = *ln->sp.h_status;
+        if (ss.bad_inv) {
+            const unsigned long long key = ~ss.bad_inv;
+            return fail_disallowed(ctx, ss.bad_prompt, static_cast<uint32_t>((key >> 12) & 7u), static_cast<uint32_t>(key & 0xFFFu), out_bad);
+        }
+        n_str = n_prompts + 2 * ss.kept.n_tokens;
+        if (n_str > ctx->max_prompts)
+            return fail(ctx, CFBPE_EINVAL, "n_prompts + 2 x special-token matches (" + std::to_string(n_str) + ") exceeds max_prompts of this context");
+    }
+    const uint32_t grid = static_cast<uint32_t>(dv->sm_count * 4);
+    if (n_str == n_prompts) {
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts, grid, s, ln->aux_stream, ln->aux2_stream,
+                       ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+    } else {
+        enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets,
+                               ln->d_out_counts, d_out_ids, out_cap, d_out_offsets, d_out_counts, grid, s, ln->aux_stream, ln->aux2_stream,
+                               ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+        // the lane's status carries the call's id count (cfbpe_device_status checks it against out_cap): n_tokens and tok_end
+        CK(cudaMemcpyAsync(&ln->ws.status->n_tokens, &ln->sp.status->fin.n_tokens, 2 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+    }
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ln->ev_ws, s));
+    ln->ws_pending = true;
+    ln->dev_out_cap = out_cap;
+    ln->dev_want_ids = d_out_ids != nullptr;
+    tl_device_lane = ln;
+    if (n_tokens) {
+        CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        const DeviceStatus st = *ln->h_status;
+        *n_tokens = st.n_tokens;
         if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
         if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
         if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");

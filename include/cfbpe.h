@@ -65,6 +65,14 @@ extern "C" {
 #define CFBPE_EINVAL (-22)   /* bad argument: null pointer, non-monotonic offsets, oversize batch, bad rank file */
 #define CFBPE_ENOSPC (-28)   /* out_cap too small; required id count is in out_offsets[n_prompts] */
 #define CFBPE_EILSEQ (-84)   /* a prompt holds malformed UTF-8 (tiktoken only accepts valid text) */
+#define CFBPE_EBADMSG (-74)  /* a prompt spells a special token this call disallows */
+
+/* what an occurrence of a registered special token means in one call (cfbpe_encode_batch_special) */
+#define CFBPE_SPECIAL_ORDINARY 0u   /* its text is ordinary text */
+#define CFBPE_SPECIAL_ALLOW 1u      /* an occurrence becomes its id */
+#define CFBPE_SPECIAL_DISALLOW 2u   /* an occurrence anywhere fails the call */
+#define CFBPE_MAX_SPECIALS 4096u    /* special tokens per vocabulary */
+#define CFBPE_MAX_SPECIAL_LEN 64u   /* bytes per special token */
 
 /* rank-file formats */
 #define CFBPE_FORMAT_TIKTOKEN 0u     /* "<base64 token> <rank>\n" lines */
@@ -157,10 +165,46 @@ CFBPE_API int cfbpe_count_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_
  * ids: the packed token ids of n_seqs sequences, id_offsets[n_seqs + 1] their boundaries (in ids), vocab_ids[n_seqs] or NULL.
  * out_offsets[n_seqs + 1]: byte boundaries of the decoded sequences in out_bytes.  CFBPE_ENOSPC if out_cap is too small
  * (out_offsets[n_seqs] = bytes needed), CFBPE_EINVAL for an id outside its vocabulary or a batch beyond the context's limits
- * (at most max_batch_bytes ids and max_batch_bytes decoded bytes).  Host buffers; no reference interface exists for it
+ * (at most max_batch_bytes ids and max_batch_bytes decoded bytes).  An id past the vocabulary's ranks that is one of its
+ * registered special tokens (cfbpe_vocab_set_specials) decodes to that token's bytes.  Host buffers; no reference interface exists for it
  * (the reference ships no tokenizer: SURVEY.md F1). */
 CFBPE_API int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, const uint64_t* id_offsets,
                                  const uint8_t* vocab_ids, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets);
+
+/* Register the special tokens of a vocabulary (tiktoken's special_tokens): token k = bytes[offsets[k] .. offsets[k+1]), id ids[k];
+ * offsets has n + 1 entries.  Replaces the vocabulary's earlier set; n = 0 clears it, and so do cfbpe_vocab_load and
+ * cfbpe_vocab_import.  Tokens must be valid UTF-8 of 1 .. CFBPE_MAX_SPECIAL_LEN bytes, distinct, with distinct ids (not
+ * 0xFFFFFFFF), at most CFBPE_MAX_SPECIALS of them: else CFBPE_EINVAL.  CFBPE_ENOENT for a slot that is not loaded.  The table
+ * is copied to every device of the context; it is not part of the exported blob (a multi-process deployment registers the
+ * specials on each rank).  Waits for running calls, as a vocabulary load does.  Decode then turns these ids into their bytes
+ * (an id below the vocabulary's n_ranks is always the ordinary token). */
+CFBPE_API int cfbpe_vocab_set_specials(cfbpe_ctx *ctx, uint32_t vocab_id, uint32_t n, const uint8_t *bytes, const uint64_t *offsets,
+                                       const uint32_t *ids);
+
+/* Encode as tiktoken's Encoding.encode(text, allowed_special=..., disallowed_special=...) does, per prompt:
+ *  1. if a DISALLOWED special occurs anywhere in the prompt's bytes (inside or across an allowed one too), the call fails with
+ *     CFBPE_EBADMSG; out_bad[0] = the lowest such prompt, out_bad[1] = the index of the special at its leftmost occurrence
+ *     (the longest one there).  This is checked before anything else: it wins over CFBPE_EILSEQ.
+ *  2. from the start, the leftmost position where an ALLOWED special occurs, the longest one there: the text before it is
+ *     encoded as ordinary text (as a text of its own: its end is the end of the text for the pre-tokenizer), then the special's
+ *     id; repeat after it; the rest is ordinary text.  A match never crosses a prompt boundary.
+ *  3. an ORDINARY special is plain text.
+ * modes[v]: one CFBPE_SPECIAL_* byte per registered special of vocabulary v, or NULL = all DISALLOWED (tiktoken's default);
+ * modes == NULL: NULL for every vocabulary.  out_ids == NULL: counts and offsets only.  out_bad (2 entries) may be NULL.
+ * Other arguments and errors as cfbpe_encode_batch.  n_prompts + 2 x (allowed matches) must not exceed the context's
+ * max_prompts (CFBPE_EINVAL).  A host call runs as one pass on its lane (not pipelined like cfbpe_encode_batch); a call whose
+ * prompts hold no allowed and no disallowed special costs one scan over the bytes beside the ordinary path, and a call for which
+ * no vocabulary has a special to look for is the ordinary path. */
+CFBPE_API int cfbpe_encode_batch_special(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
+                                         const uint8_t *vocab_ids, const uint8_t *const *modes, uint32_t *out_ids, uint64_t out_cap,
+                                         uint64_t *out_offsets, uint32_t *out_counts, uint32_t *out_bad);
+/* The same on device-resident buffers (as cfbpe_encode_batch_device; modes and out_bad are HOST memory).  When some vocabulary
+ * has a special to look for, the call synchronises `stream` once, after the scan, to learn the number of stretches (and whether
+ * a disallowed special occurs); the rest is enqueued asynchronously as in cfbpe_encode_batch_device. */
+CFBPE_API int cfbpe_encode_batch_special_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
+                                                const uint64_t *d_offsets, const uint8_t *d_vocab_ids, const uint8_t *const *modes,
+                                                uint32_t *d_out_ids, uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
+                                                uint64_t *n_tokens, uint32_t *out_bad, void *stream);
 
 /* Same path on device-resident buffers, enqueued on `stream` (a cudaStream_t; NULL = the legacy
  * default stream).  d_bytes must be readable for 32 bytes past total_bytes (the kernels read whole 16-byte

@@ -17,6 +17,13 @@ pub const CFBPE_ENODEV: c_int = -19;
 pub const CFBPE_EINVAL: c_int = -22;
 pub const CFBPE_ENOSPC: c_int = -28;
 pub const CFBPE_EILSEQ: c_int = -84;
+/// a prompt spells a special token the call disallows (`cfbpe_encode_batch_special`)
+pub const CFBPE_EBADMSG: c_int = -74;
+
+pub const CFBPE_SPECIAL_ORDINARY: u8 = 0;
+pub const CFBPE_SPECIAL_ALLOW: u8 = 1;
+pub const CFBPE_SPECIAL_DISALLOW: u8 = 2;
+pub const CFBPE_MAX_SPECIALS: usize = 4096;
 
 pub const CFBPE_FORMAT_TIKTOKEN: u32 = 0;
 pub const CFBPE_FORMAT_TEKKEN_JSON: u32 = 1;
@@ -76,6 +83,14 @@ extern "C" {
                                      d_offsets: *const u64, d_vocab_ids: *const u8, d_out_ids: *mut u32, out_cap: u64,
                                      d_out_offsets: *mut u64, d_out_counts: *mut u32, n_tokens: *mut u64,
                                      stream: *mut c_void) -> c_int;
+    pub fn cfbpe_vocab_set_specials(ctx: *mut cfbpe_ctx, vocab_id: u32, n: u32, bytes: *const u8, offsets: *const u64, ids: *const u32) -> c_int;
+    pub fn cfbpe_encode_batch_special(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64, vocab_ids: *const u8,
+                                      modes: *const *const u8, out_ids: *mut u32, out_cap: u64, out_offsets: *mut u64, out_counts: *mut u32,
+                                      out_bad: *mut u32) -> c_int;
+    pub fn cfbpe_encode_batch_special_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64, d_offsets: *const u64,
+                                             d_vocab_ids: *const u8, modes: *const *const u8, d_out_ids: *mut u32, out_cap: u64,
+                                             d_out_offsets: *mut u64, d_out_counts: *mut u32, n_tokens: *mut u64, out_bad: *mut u32,
+                                             stream: *mut c_void) -> c_int;
     pub fn cfbpe_device_status(ctx: *mut cfbpe_ctx, stream: *mut c_void) -> c_int;
     pub fn cfbpe_host_alloc(ctx: *mut cfbpe_ctx, size: usize) -> *mut c_void;
     pub fn cfbpe_host_free(ctx: *mut cfbpe_ctx, ptr: *mut c_void);
@@ -182,6 +197,49 @@ impl Ctx {
         let rc = unsafe {
             cfbpe_encode_batch(self.0.as_ptr(), n, bytes.as_ptr(), offsets.as_ptr(), vocab_ids.map_or(std::ptr::null(), <[u8]>::as_ptr),
                                out.ids.as_mut_ptr(), out.ids.len() as u64, out.offsets.as_mut_ptr(), out.counts.as_mut_ptr())
+        };
+        self.check(rc)?;
+        out.ids.truncate(out.offsets[n as usize] as usize);
+        out.counts.truncate(n as usize);
+        Ok(out)
+    }
+
+    /// Register `(token, id)` pairs as the special tokens of a vocabulary slot (the pair order is the special index the
+    /// per-call modes refer to); an empty slice clears them.
+    pub fn vocab_set_specials(&self, vocab_id: u32, specials: &[(String, u32)]) -> Result<(), NativeError> {
+        let mut bytes = Vec::new();
+        let mut offsets = vec![0u64];
+        for (t, _) in specials {
+            bytes.extend_from_slice(t.as_bytes());
+            offsets.push(bytes.len() as u64);
+        }
+        let ids: Vec<u32> = specials.iter().map(|(_, id)| *id).collect();
+        let n = u32::try_from(specials.len()).map_err(|_| NativeError { code: CFBPE_EINVAL, message: "too many special tokens".to_owned() })?;
+        // SAFETY: the three buffers hold n tokens / n + 1 offsets / n ids and are not retained.
+        self.check(unsafe { cfbpe_vocab_set_specials(self.0.as_ptr(), vocab_id, n, bytes.as_ptr(), offsets.as_ptr(), ids.as_ptr()) })
+    }
+
+    /// tiktoken's `encode(allowed_special = …, disallowed_special = …)` for every prompt: `modes[v]` holds one
+    /// `CFBPE_SPECIAL_*` byte per registered special of vocabulary `v` (`None`: every special disallowed).  A prompt that spells a
+    /// disallowed special fails with `CFBPE_EBADMSG`; the message names the prompt and the token.
+    pub fn encode_batch_special(&self, bytes: &[u8], offsets: &[u64], vocab_ids: Option<&[u8]>, modes: &[Option<&[u8]>])
+        -> Result<Encoded, NativeError> {
+        let n = Self::check_inputs(bytes.len(), offsets, vocab_ids)?;
+        if modes.len() > CFBPE_MAX_VOCABS as usize {
+            return Err(NativeError { code: CFBPE_EINVAL, message: "modes names more vocabularies than a context holds".to_owned() });
+        }
+        let mut mp = [std::ptr::null::<u8>(); CFBPE_MAX_VOCABS as usize];
+        for (v, m) in modes.iter().enumerate() {
+            mp[v] = m.map_or(std::ptr::null(), <[u8]>::as_ptr);
+        }
+        let total = offsets[n as usize] as usize;
+        let mut out = Encoded { ids: vec![0; total.max(1)], offsets: vec![0; n as usize + 1], counts: vec![0; (n as usize).max(1)] };
+        let mut bad = [0u32; 2];
+        // SAFETY: as encode_batch; every modes entry is null or holds one byte per registered special (the library checks the values).
+        let rc = unsafe {
+            cfbpe_encode_batch_special(self.0.as_ptr(), n, bytes.as_ptr(), offsets.as_ptr(), vocab_ids.map_or(std::ptr::null(), <[u8]>::as_ptr),
+                                       mp.as_ptr(), out.ids.as_mut_ptr(), out.ids.len() as u64, out.offsets.as_mut_ptr(), out.counts.as_mut_ptr(),
+                                       bad.as_mut_ptr())
         };
         self.check(rc)?;
         out.ids.truncate(out.offsets[n as usize] as usize);

@@ -6,7 +6,7 @@ use std::sync::Arc;
 use async_trait::async_trait;
 use cfbpe_sys::{Ctx, NativeError};
 use llm_gateway_sdk::{
-    CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, TokenizerError,
+    CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens, TokenizerError,
     TokenizerPluginClient, VocabRef,
 };
 use modkit_security::SecurityContext;
@@ -21,11 +21,14 @@ pub struct Service {
     slots: HashMap<String, u8>,
     names: Vec<String>,
     batcher: CountBatcher,
+    /// slot -> the special tokens registered on it, in registration order (= the special index of the per-call modes)
+    specials: Arc<std::sync::Mutex<HashMap<u8, Vec<(String, u32)>>>>,
 }
 
 fn map_native(e: NativeError) -> TokenizerError {
     match e.code {
-        cfbpe_sys::CFBPE_EINVAL | cfbpe_sys::CFBPE_EILSEQ | cfbpe_sys::CFBPE_ENOSPC => TokenizerError::InvalidInput(e.message),
+        // (EBADMSG: the message names the disallowed special token)
+        cfbpe_sys::CFBPE_EINVAL | cfbpe_sys::CFBPE_EILSEQ | cfbpe_sys::CFBPE_ENOSPC | cfbpe_sys::CFBPE_EBADMSG => TokenizerError::InvalidInput(e.message),
         cfbpe_sys::CFBPE_ENOENT => TokenizerError::VocabNotFound { vocab: e.message },
         cfbpe_sys::CFBPE_ENODEV | cfbpe_sys::CFBPE_ENOMEM => TokenizerError::ServiceUnavailable(e.message),
         _ => TokenizerError::Internal(e.message),
@@ -63,7 +66,7 @@ impl Service {
         }
         let native = Arc::new(native);
         let batcher = CountBatcher::start(native.clone(), cfg.batch_bytes.min(cfg.max_batch_bytes), cfg.max_prompts, cfg.batch_wait_us);
-        Ok(Self { native, slots, names, batcher })
+        Ok(Self { native, slots, names, batcher, specials: Arc::default() })
     }
 
     pub fn vocab_names(&self) -> &[String] {
@@ -136,6 +139,40 @@ impl TokenizerPluginClient for Service {
             .map_err(|e| TokenizerError::Internal(e.to_string()))?
             .map_err(map_native)?;
         Ok(DecodeBatchResponse { bytes, offsets })
+    }
+
+    /// The device path: scan, cut and splice run as CUDA kernels (`cfbpe_encode_batch_special`).  The caller's special tokens
+    /// are registered on every slot the request uses when they differ from what the slot holds.
+    async fn encode_batch_special(&self, _ctx: &SecurityContext, req: EncodeBatchRequest, special: &SpecialTokens)
+        -> Result<EncodeBatchResponse, TokenizerError> {
+        let n = req.offsets.len().saturating_sub(1);
+        let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
+        let mut used: Vec<u8> = match &vid { Some(v) => v[..n].to_vec(), None => vec![self.slot(&req.vocab)?] };
+        used.sort_unstable();
+        used.dedup();
+        let want: Vec<(String, u32)> = special.ids.iter().map(|(t, id)| (t.clone(), *id)).collect();
+        let modes: Vec<u8> = want.iter().map(|(t, _)| {
+            if special.allowed.contains(t) { cfbpe_sys::CFBPE_SPECIAL_ALLOW }
+            else if special.disallow_all_others { cfbpe_sys::CFBPE_SPECIAL_DISALLOW }
+            else { cfbpe_sys::CFBPE_SPECIAL_ORDINARY }
+        }).collect();
+        let (native, specials) = (self.native.clone(), self.specials.clone());
+        let out = tokio::task::spawn_blocking(move || {
+            let mut held = specials.lock().unwrap_or_else(std::sync::PoisonError::into_inner);
+            let mut per_vocab: Vec<Option<&[u8]>> = vec![None; cfbpe_sys::CFBPE_MAX_VOCABS as usize];
+            for &slot in &used {
+                if held.get(&slot) != Some(&want) {
+                    native.vocab_set_specials(u32::from(slot), &want)?;
+                    held.insert(slot, want.clone());
+                }
+                per_vocab[slot as usize] = Some(&modes);
+            }
+            native.encode_batch_special(&req.bytes, &req.offsets, vid.as_deref(), &per_vocab)
+        })
+        .await
+        .map_err(|e| TokenizerError::Internal(e.to_string()))?
+        .map_err(map_native)?;
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts })
     }
 }
 

@@ -4,7 +4,7 @@ use async_trait::async_trait;
 use modkit_security::SecurityContext;
 
 use crate::error::TokenizerError;
-use crate::models::{CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse};
+use crate::models::{CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens, VocabRef};
 
 /// Each plugin registers this trait with a scoped `ClientHub` entry using its GTS instance id as the scope.  Clients are
 /// `Arc<dyn … + Send + Sync>` shared by all tokio tasks (`libs/modkit/src/client_hub.rs:142-165`): calls are concurrent and
@@ -22,4 +22,69 @@ pub trait TokenizerPluginClient: Send + Sync {
 
     /// ids -> bytes; `InvalidInput` for an id outside its vocabulary.
     async fn decode_batch(&self, ctx: &SecurityContext, req: DecodeBatchRequest) -> Result<DecodeBatchResponse, TokenizerError>;
+
+    /// tiktoken's `encode(text, allowed_special = …, disallowed_special = …)` for every prompt of the batch; `InvalidInput` when
+    /// a prompt spells a special token that is not allowed.  The default works on any plugin: it cuts every text at the
+    /// allowed special tokens on the host (leftmost, then the longest there), sends all stretches of all texts through ONE
+    /// `encode_batch`, and puts the special ids back.  `gpu-bpe-tokenizer-plugin` overrides it with the device path.
+    async fn encode_batch_special(&self, ctx: &SecurityContext, req: EncodeBatchRequest, special: &SpecialTokens)
+        -> Result<EncodeBatchResponse, TokenizerError> {
+        let n = req.offsets.len().saturating_sub(1);
+        let mut texts = Vec::with_capacity(n);
+        for i in 0..n {
+            let b = &req.bytes[req.offsets[i] as usize..req.offsets[i + 1] as usize];
+            texts.push(std::str::from_utf8(b).map_err(|_| TokenizerError::InvalidInput("a prompt holds malformed UTF-8".to_owned()))?);
+        }
+        let mut allowed: Vec<&String> = special.allowed.iter().collect();
+        allowed.sort_by_key(|t| std::cmp::Reverse(t.len()));
+        if special.disallow_all_others {
+            for t in &texts {
+                if let Some(bad) = special.ids.keys().find(|k| !special.allowed.contains(*k) && t.contains(k.as_str())) {
+                    return Err(TokenizerError::InvalidInput(format!("the text holds the special token {bad:?}, which is not allowed here")));
+                }
+            }
+        }
+        enum Step { Stretch(usize), Special(u32) }
+        let (mut plan, mut stretches): (Vec<Vec<Step>>, Vec<&str>) = (Vec::new(), Vec::new());
+        let mut per: Option<Vec<VocabRef>> = req.vocabs_per_prompt.as_ref().map(|_| Vec::new());
+        for (p, t) in texts.iter().enumerate() {
+            let (mut steps, mut pos) = (Vec::new(), 0usize);
+            let vocab_of = |p: usize| req.vocabs_per_prompt.as_ref().map(|v| match &req.vocab_index { Some(ix) => v[ix[p] as usize].clone(), None => v[p].clone() });
+            while pos < t.len() {
+                let next = allowed.iter().filter_map(|tok| t[pos..].find(tok.as_str()).map(|i| (pos + i, *tok))).min_by_key(|(i, tok)| (*i, std::cmp::Reverse(tok.len())));
+                let end = next.map_or(t.len(), |(i, _)| i);
+                if end > pos {
+                    steps.push(Step::Stretch(stretches.len()));
+                    stretches.push(&t[pos..end]);
+                    if let (Some(per), Some(v)) = (per.as_mut(), vocab_of(p)) { per.push(v); }
+                }
+                match next {
+                    Some((i, tok)) => { steps.push(Step::Special(special.ids[tok])); pos = i + tok.len(); }
+                    None => pos = t.len(),
+                }
+            }
+            plan.push(steps);
+        }
+        let enc = if stretches.is_empty() {
+            EncodeBatchResponse { ids: Vec::new(), offsets: vec![0], counts: Vec::new() }
+        } else {
+            let mut bytes = Vec::new();
+            let mut offsets = vec![0u64];
+            for s in &stretches { bytes.extend_from_slice(s.as_bytes()); offsets.push(bytes.len() as u64); }
+            self.encode_batch(ctx, EncodeBatchRequest { vocab: req.vocab.clone(), bytes: bytes.into(), offsets, vocabs_per_prompt: per.take(), vocab_index: None }).await?
+        };
+        let mut out = EncodeBatchResponse { ids: Vec::new(), offsets: vec![0u64], counts: Vec::with_capacity(n) };
+        for steps in plan {
+            let start = out.ids.len();
+            for s in steps {
+                match s {
+                    Step::Stretch(i) => out.ids.extend_from_slice(&enc.ids[enc.offsets[i] as usize..enc.offsets[i + 1] as usize]),
+                    Step::Special(id) => out.ids.push(id),
+                }
+            }
+            out.counts.push((out.ids.len() - start) as u32);
+            out.offsets.push(out.ids.len() as u64);
+        }
+        Ok(out)
+    }
 }

@@ -80,39 +80,14 @@ impl TokenizerClient for TokenizerService {
 
     async fn encode_with_special(&self, ctx: &SecurityContext, model: &str, texts: &[String], special: &SpecialTokens)
         -> Result<Vec<Vec<u32>>, TokenizerError> {
-        // cut every text at the allowed special tokens (leftmost, longest first), send all stretches of all texts through ONE
-        // plugin batch, put the special ids back; a text that spells a token that is not allowed is refused
-        let mut allowed: Vec<&String> = special.allowed.iter().collect();
-        allowed.sort_by_key(|t| std::cmp::Reverse(t.len()));
-        if let Some(unknown) = allowed.iter().find(|t| !special.ids.contains_key(**t)) {
+        // the plugin does the work: the trait's default cuts on the host, the GPU plugin scans, cuts and splices on the device
+        if let Some(unknown) = special.allowed.iter().find(|t| !special.ids.contains_key(*t)) {
             return Err(TokenizerError::InvalidInput(format!("allowed special token without an id: {unknown}")));
         }
-        if special.disallow_all_others {
-            for t in texts {
-                if let Some(bad) = special.ids.keys().find(|k| !special.allowed.contains(*k) && t.contains(k.as_str())) {
-                    return Err(TokenizerError::InvalidInput(format!("the text holds the special token {bad:?}, which is not allowed here")));
-                }
-            }
-        }
-        enum Step { Stretch(usize), Special(u32) }
-        let (mut plan, mut stretches): (Vec<Vec<Step>>, Vec<String>) = (Vec::new(), Vec::new());
-        for t in texts {
-            let (mut steps, mut pos) = (Vec::new(), 0usize);
-            while pos < t.len() {
-                let next = allowed.iter().filter_map(|tok| t[pos..].find(tok.as_str()).map(|i| (pos + i, *tok))).min_by_key(|(i, tok)| (*i, std::cmp::Reverse(tok.len())));
-                match next {
-                    Some((i, tok)) => {
-                        if i > pos { steps.push(Step::Stretch(stretches.len())); stretches.push(t[pos..i].to_owned()); }
-                        steps.push(Step::Special(special.ids[tok]));
-                        pos = i + tok.len();
-                    }
-                    None => { steps.push(Step::Stretch(stretches.len())); stretches.push(t[pos..].to_owned()); pos = t.len(); }
-                }
-            }
-            plan.push(steps);
-        }
-        let enc = if stretches.is_empty() { Vec::new() } else { self.encode(ctx, model, &stretches).await? };
-        Ok(plan.into_iter().map(|steps| steps.into_iter().flat_map(|s| match s { Step::Stretch(i) => enc[i].clone(), Step::Special(id) => vec![id] }).collect()).collect())
+        let (bytes, offsets) = pack_texts(texts);
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None };
+        let r = self.plugin().await?.encode_batch_special(ctx, req, special).await?;
+        Ok((0..texts.len()).map(|i| r.ids[r.offsets[i] as usize..r.offsets[i + 1] as usize].to_vec()).collect())
     }
 
     async fn count_tokens(&self, ctx: &SecurityContext, model: &str, messages: &[Value]) -> Result<Usage, TokenizerError> {
