@@ -26,6 +26,7 @@ EXPORTS = [
     "cfbpe_encode_batch_device", "cfbpe_device_status", "cfbpe_host_alloc", "cfbpe_host_free",
     "cfbpe_profile_enable", "cfbpe_profile_read", "cfbpe_decode_batch",
     "cfbpe_vocab_set_specials", "cfbpe_encode_batch_special", "cfbpe_encode_batch_special_device",
+    "cfbpe_encode_batch_starts", "cfbpe_encode_batch_starts_device",
 ]
 
 
@@ -100,6 +101,11 @@ def load():
     L.cfbpe_encode_batch_device.restype = C.c_int
     L.cfbpe_encode_batch_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp,
                                             C.POINTER(C.c_uint64), vp]
+    L.cfbpe_encode_batch_starts.restype = C.c_int
+    L.cfbpe_encode_batch_starts.argtypes = [vp, C.c_uint32, u8p, vp, u8p, vp, vp, C.c_uint64, vp, vp]
+    L.cfbpe_encode_batch_starts_device.restype = C.c_int
+    L.cfbpe_encode_batch_starts_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, C.c_uint64, vp, vp,
+                                                   C.POINTER(C.c_uint64), vp]
     L.cfbpe_vocab_set_specials.restype = C.c_int
     L.cfbpe_vocab_set_specials.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, vp, vp]
     L.cfbpe_encode_batch_special.restype = C.c_int
@@ -246,6 +252,30 @@ class Context:
         self._check(rc)
         return out_ids[:int(out_offsets[n])], out_offsets, out_counts[:n]
 
+    def encode_batch_starts(self, data: np.ndarray, offsets: np.ndarray, vocab_ids=None, out_ids=None, out_starts=None,
+                            out_offsets=None, out_counts=None):
+        """encode_batch plus each token's byte offset within its prompt: (ids, starts uint32, offsets, counts).  Token k of prompt i
+        covers bytes[offsets_in[i] + starts[k] .. offsets_in[i] + end), end = starts[k + 1] or the prompt's length for its last token."""
+        n = self._check_inputs(data, offsets, vocab_ids)
+        total = int(offsets[n])
+        if out_ids is None:
+            out_ids = np.empty(max(total, 1), dtype=np.uint32)
+        if out_starts is None:
+            out_starts = np.empty(out_ids.size, dtype=np.uint32)
+        if out_starts.dtype != np.uint32 or out_starts.size < out_ids.size or not out_starts.flags.c_contiguous:
+            raise NativeError(EINVAL, "out_starts must be a C-contiguous uint32 array with room for as many entries as out_ids")
+        if out_offsets is None:
+            out_offsets = np.empty(n + 1, dtype=np.uint64)
+        if out_counts is None:
+            out_counts = np.empty(max(n, 1), dtype=np.uint32)
+        vid = None if vocab_ids is None else vocab_ids.ctypes.data
+        rc = load().cfbpe_encode_batch_starts(self._h, n, data.ctypes.data if data.size else None, offsets.ctypes.data, vid,
+                                              out_ids.ctypes.data, out_starts.ctypes.data, out_ids.size, out_offsets.ctypes.data,
+                                              out_counts.ctypes.data)
+        self._check(rc)
+        nt = int(out_offsets[n])
+        return out_ids[:nt], out_starts[:nt], out_offsets, out_counts[:n]
+
     def count_batch(self, data: np.ndarray, offsets: np.ndarray, vocab_ids=None, out_counts=None):
         n = self._check_inputs(data, offsets, vocab_ids)
         if out_counts is None:
@@ -284,6 +314,16 @@ class Context:
         rc = load().cfbpe_encode_batch_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids,
                                               d_out_ids, out_cap, d_out_offsets, d_out_counts,
                                               C.byref(nt) if sync else None, stream)
+        self._check(rc)
+        return nt.value if sync else None
+
+    def encode_batch_starts_device(self, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, d_out_starts, out_cap,
+                                   d_out_offsets, d_out_counts, stream=0, sync=True):
+        """cfbpe_encode_batch_starts_device on raw device pointers (d_out_starts: room for out_cap uint32); the id count when sync"""
+        nt = C.c_uint64(0)
+        rc = load().cfbpe_encode_batch_starts_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids,
+                                                     d_out_starts, out_cap, d_out_offsets, d_out_counts,
+                                                     C.byref(nt) if sync else None, stream)
         self._check(rc)
         return nt.value if sync else None
 

@@ -98,6 +98,7 @@ class EncodeBatchRequest:
     vocabs_per_prompt: Optional[Sequence[VocabRef]] = None   # multi-tenant batches: one vocab per prompt
     vocab_index: Optional[np.ndarray] = None   # uint8, n: with it, vocabs_per_prompt lists the DISTINCT vocabularies and
                                                # vocab_index[i] picks prompt i's (large batches: no per-prompt objects)
+    with_starts: bool = False    # also return every token's byte offset within its prompt (EncodeBatchResponse.starts)
 
 
 @dataclass
@@ -105,6 +106,7 @@ class EncodeBatchResponse:
     ids: np.ndarray              # uint32 dense id stream
     offsets: np.ndarray          # uint64, n+1
     counts: np.ndarray           # uint32, n
+    starts: Optional[np.ndarray] = None   # uint32, one per id: byte offset of the token within its prompt (with_starts)
 
 
 @dataclass
@@ -394,6 +396,12 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
         self._check_arrays(req)
         vid = self._vocab_ids(req)
         try:
+            if req.with_starts:
+                ids, starts, offs, counts = self.ctx.encode_batch_starts(
+                    req.bytes, req.offsets, vid,
+                    None if out is None else out.ids, None if out is None else out.starts,
+                    None if out is None else out.offsets, None if out is None else out.counts)
+                return EncodeBatchResponse(ids, offs, counts, starts)
             ids, offs, counts = self.ctx.encode_batch(
                 req.bytes, req.offsets, vid,
                 None if out is None else out.ids, None if out is None else out.offsets,
@@ -485,6 +493,26 @@ class LlmGatewayTokenizerService:
         data, offs = pack_texts(texts)
         r = self._plugin().encode_batch(ctx, EncodeBatchRequest(VocabRef(model), data, offs))
         return [r.ids[int(r.offsets[i]):int(r.offsets[i + 1])] for i in range(len(texts))]
+
+    def encode_with_offsets(self, ctx: SecurityContext, model: str, texts: Sequence[str]) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """per text: (ids, spans), spans an (n, 2) uint64 array of each token's [start, end) byte range in text.encode("utf-8")
+        (tiktoken's decode_with_offsets gives the starts in characters; Hugging Face tokenizers' `offsets` are such spans).
+        Cutting a text to a context window or into chunks of at most N tokens is a cut at a span boundary."""
+        data, offs = pack_texts(texts)
+        r = self._plugin().encode_batch(ctx, EncodeBatchRequest(VocabRef(model), data, offs, with_starts=True))
+        if r.starts is None:
+            raise ServiceUnavailable("the tokenizer plugin does not return token starts")
+        out = []
+        for i in range(len(texts)):
+            a, b = int(r.offsets[i]), int(r.offsets[i + 1])
+            st = r.starts[a:b].astype(np.uint64)
+            spans = np.empty((b - a, 2), dtype=np.uint64)
+            spans[:, 0] = st
+            spans[:-1, 1] = st[1:]
+            if b > a:
+                spans[-1, 1] = int(offs[i + 1]) - int(offs[i])
+            out.append((r.ids[a:b], spans))
+        return out
 
     def count_tokens(self, ctx: SecurityContext, model: str, messages: Sequence[dict]) -> Usage:
         """Usage.input_tokens of one chat request = sum of len(encode_ordinary(text)) over its

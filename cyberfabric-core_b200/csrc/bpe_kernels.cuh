@@ -1670,6 +1670,71 @@ prompt_offsets_kernel(BatchView b, const uint32_t* __restrict__ tok_bits, const 
     }
 }
 
+// Token starts (pipeline.cuh, enqueue_emit): starts[r] = byte offset of token r within its prompt.  The tokens of the (sub-)batch
+// are ranks [tok_end - n_tokens, tok_end) of the id stream (status, from tile_scan) and tile its bytes in order, so a token's byte
+// position is the sum of the lengths of the tokens before it.  A CTA takes kStartsTile tokens, a thread 8 consecutive ones (it
+// finds their prompt once, by rank in out_offsets, and steps on); the grid covers one token a byte.  Ranks at or past out_cap
+// have no id and get no start.
+//   starts_len:  starts[r] = byte length of id r (the vocabulary of its prompt); tile_sums[tile] = their sum
+//   tile_scan:   exclusive scan of the tile sums
+//   starts_emit: scan of the lengths inside the tile + the tile's base - offsets[prompt]
+constexpr uint32_t kStartsTile = 2048;
+__device__ __forceinline__ uint32_t starts_prompt(const uint64_t* __restrict__ out_offsets, uint32_t p, uint64_t r) {
+    while (out_offsets[p + 1] <= r) ++p;         // (p + 1 <= n_prompts: r is below out_offsets[n_prompts])
+    return p;
+}
+
+__global__ void __launch_bounds__(256)
+starts_len_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ ids, const uint64_t* __restrict__ out_offsets, uint64_t out_cap,
+                  const DeviceStatus* status, uint32_t* __restrict__ starts, uint32_t* __restrict__ tile_sums) {
+    __shared__ uint32_t s_tmp[8];
+    const uint64_t n = status->n_tokens, r0 = status->tok_end - n;
+    const uint64_t lim = r0 + n < out_cap ? r0 + n : out_cap;
+    const uint64_t r = r0 + static_cast<uint64_t>(blockIdx.x) * kStartsTile + 8u * threadIdx.x;
+    uint32_t sum = 0;
+    if (r < lim) {
+        uint32_t p = find_prompt(out_offsets, b.n_prompts, r);
+        for (uint32_t k = 0; k < 8 && r + k < lim; ++k) {
+            p = starts_prompt(out_offsets, p, r + k);
+            const TablesView& T = vs.v[b.vocab_ids ? b.vocab_ids[p] : 0u];
+            const uint32_t id = ids[r + k];
+            const uint32_t len = T.tokoff[id + 1] - T.tokoff[id];
+            starts[r + k] = len;
+            sum += len;
+        }
+    }
+    const uint32_t t = block_reduce_add_256(sum, s_tmp);
+    if (threadIdx.x == 0) tile_sums[blockIdx.x] = t;
+}
+
+__global__ void __launch_bounds__(256)
+starts_emit_kernel(BatchView b, const uint64_t* __restrict__ out_offsets, uint64_t out_cap, const DeviceStatus* status,
+                   const uint64_t* __restrict__ tile_base, uint32_t* __restrict__ starts) {
+    __shared__ uint32_t s_warp[8];
+    const uint64_t n = status->n_tokens, r0 = status->tok_end - n;
+    const uint64_t lim = r0 + n < out_cap ? r0 + n : out_cap;
+    const uint64_t r = r0 + static_cast<uint64_t>(blockIdx.x) * kStartsTile + 8u * threadIdx.x;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint32_t len[8], sum = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < 8; ++k) { len[k] = (r + k < lim) ? starts[r + k] : 0u; sum += len[k]; }
+    uint32_t x = sum;                             // block exclusive scan of the threads' sums
+#pragma unroll
+    for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(kFull, x, d); if (lane >= d) x += o; }
+    if (lane == 31) s_warp[wid] = x;
+    __syncthreads();
+    uint32_t before = 0;
+    for (uint32_t k = 0; k < wid; ++k) before += s_warp[k];
+    if (r >= lim) return;
+    uint64_t pos = tile_base[blockIdx.x] + before + x - sum;        // byte position of token r in the (sub-)batch
+    uint32_t p = find_prompt(out_offsets, b.n_prompts, r);
+    for (uint32_t k = 0; k < 8 && r + k < lim; ++k) {
+        p = starts_prompt(out_offsets, p, r + k);
+        starts[r + k] = static_cast<uint32_t>(pos - b.offsets[p]);
+        pos += len[k];
+    }
+}
+
 // ---------------------------------------------------------------------------------------
 // Decode (SURVEY.md section 8(f) item 2): ids -> bytes.  tiktoken's decode_bytes: the concatenation of the tokens' bytes.
 //   decode_len:    length of every token (0xFFFFFFFF + status->bad_utf8-style flag for an id outside the vocabulary),

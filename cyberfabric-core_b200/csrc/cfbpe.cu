@@ -131,6 +131,7 @@ struct Lane {
     uint32_t* d_out_ids = nullptr;
     uint64_t* d_out_offsets = nullptr;
     uint32_t* d_out_counts = nullptr;
+    uint32_t* d_out_starts = nullptr;    // host calls with token starts: [max_bytes + 1], allocated on the lane's first such call
     Workspace ws{};
     DeviceStatus* h_status = nullptr;  // pinned
     ProfEvents prof{};
@@ -333,6 +334,17 @@ void fill_profile(Lane* ln, uint64_t n_bytes) {
     tl_profile_ready = true;
 }
 
+// the lane's buffer of token starts (host calls of cfbpe_encode_batch_starts), allocated on its first such call: a context that never
+// asks for starts keeps the footprint it had.  The caller has selected the lane's device.
+int ensure_starts_lane(cfbpe_ctx* ctx, Lane* ln) {
+    if (ln->d_out_starts) return CFBPE_OK;
+    if (dmalloc(&ln->d_out_starts, ln->max_bytes + 1) != cudaSuccess) {
+        cudaGetLastError(); ln->d_out_starts = nullptr;
+        return fail(ctx, CFBPE_ENOMEM, "no device memory for the token starts");
+    }
+    return CFBPE_OK;
+}
+
 // Pipelined host call: the batch is cut into sub-batches of ~kPipeChunkBytes on prompt boundaries; each is an
 // independent encode pass on its own slice of the workspace.  Uploads (h2d_stream) run ahead of the kernels
 // (stream), downloads (d2h_stream) trail them; token ranks are chained on the device (DeviceStatus::tok_end), so
@@ -341,8 +353,8 @@ void fill_profile(Lane* ln, uint64_t n_bytes) {
 // defer != nullptr (a shard of a multi-device call): nothing is downloaded here -- ids, offsets and counts stay in the lane's device
 // buffers (dense, shard-local ranks: sub-batch k's offsets at d_out_offsets + p_k + k) and *defer gets the shard's token total.
 int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, int G, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
-                       const uint8_t* vocab_ids, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
-                       uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out) {
+                       const uint8_t* vocab_ids, uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
+                       bool want_ids, uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out) {
     // ---- cut
     uint32_t cut[kMaxPipeChunks + 1];
     const int nc = plan_sub_batches(offsets, n, total, ctx->pipe_chunk, kMaxPipeChunks, cut);
@@ -430,7 +442,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         enqueue_scan(b, w, ss, static_cast<ProfEvents*>(nullptr), k ? &prev->d_status_arr[k - 1].tok_end : nullptr);   // (G > 1: a peer pointer)
         CK(cudaEventRecord(ln->ev_chain[k], ss));
         enqueue_emit(b, w, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets + p0 + k, ln->d_out_counts + p0,
-                     ss, static_cast<ProfEvents*>(nullptr));
+                     ss, static_cast<ProfEvents*>(nullptr), out_starts ? ln->d_out_starts : nullptr, &dv->vs);
         CK(cudaGetLastError());
         status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr + k, ln->h_status_arr + k);
         CK(cudaEventRecord(ln->ev_done[k], ss));
@@ -455,6 +467,8 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (no_copy) continue;
         if (want_ids && st.tok_end <= out_cap && st.n_tokens)
             CK(cudaMemcpyAsync(out_ids + base, ln->d_out_ids + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
+        if (out_starts && st.tok_end <= out_cap && st.n_tokens)      // (prompt-relative: the same ranks and base as the ids)
+            CK(cudaMemcpyAsync(out_starts + base, ln->d_out_starts + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (out_offsets) CK(cudaMemcpyAsync(out_offsets + p0, ln->d_out_offsets + p0 + k, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
         if (out_counts && nk) CK(cudaMemcpyAsync(out_counts + p0, ln->d_out_counts + p0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (trace) { CK(cudaEventRecord(ln->trace[k][5], ds)); host_dl[k] = host_ms(); }
@@ -489,14 +503,17 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
 
 // One device's share of a host call (the whole call on a single-device context): validation is done, the lane is locked.
 // defer / cut_out / nc_out: see run_host_pipelined; the one-shot path under `defer` leaves everything on the device as ONE sub-batch.
+// out_starts != nullptr: the tokens' starts too (in ln->d_out_starts, beside the ids; under `defer` it is only a flag).
 int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
-             uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
+             uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
              uint64_t* defer = nullptr, uint32_t* cut_out = nullptr, int* nc_out = nullptr) {
     CK(cudaSetDevice(dv->device));
     if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }   // an asynchronous device-path call still owns the workspace
+    if (out_starts) { const int rc = ensure_starts_lane(ctx, ln); if (rc) return rc; }
     const bool profiling = ctx->profiling.load();
     if (!profiling && total >= ctx->pipe_min && n >= 2)
-        return run_host_pipelined(ctx, &dv, &ln, 1, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total, defer, cut_out, nc_out);
+        return run_host_pipelined(ctx, &dv, &ln, 1, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
+                                  defer, cut_out, nc_out);
     cudaStream_t s = ln->stream;
     ProfEvents* prof = profiling ? &ln->prof : nullptr;
     if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); }
@@ -508,7 +525,7 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     BatchView b{ln->d_bytes, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n, total};
     enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets,
                    ln->d_out_counts, static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof);
+                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, out_starts ? ln->d_out_starts : nullptr);
     CK(cudaGetLastError());
     if (prof) cudaEventRecord(prof->d2h[0], s);
     CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
@@ -528,6 +545,7 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
             return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(st.n_tokens) + " ids");
         }
         if (st.n_tokens) CK(cudaMemcpyAsync(out_ids, ln->d_out_ids, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        if (out_starts && st.n_tokens) CK(cudaMemcpyAsync(out_starts, ln->d_out_starts, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     }
     if (prof) { cudaEventRecord(prof->d2h[1], s); cudaEventRecord(prof->total[1], s); }
     CK(cudaStreamSynchronize(s));
@@ -632,7 +650,7 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
 // are the call's modes, special->bad gets the prompt and special index of a CFBPE_EBADMSG
 struct SpecialArgs { const uint8_t* const* modes; uint32_t* bad; };
 int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
-                     uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
+                     uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
                      const SpecialArgs* special = nullptr) {
     const uint32_t G = static_cast<uint32_t>(ctx->devs.size());
     std::vector<uint32_t> lo(G + 1, 0);
@@ -664,7 +682,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
                 s.cut[0] = 0; s.cut[1] = nd; s.nc = 1;
             } else {
                 s.rc = run_lane(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
-                                nullptr, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc);
+                                nullptr, out_starts, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc);
             }
             if (s.rc) s.err = tl_err;
         });
@@ -717,6 +735,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             uint64_t base = 0;
             for (uint32_t e = 0; e < d; ++e) base += ln->h_totals[e];
             if (want_ids && fits && s.tokens) ck(cudaMemcpyAsync(out_ids + base, ln->d_out_ids, s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "ids download");
+            if (out_starts && fits && s.tokens) ck(cudaMemcpyAsync(out_starts + base, ln->d_out_starts, s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "starts download");
             ck(cudaStreamSynchronize(st), "stream sync");
         });
         for (auto& t : th) t.join();
@@ -729,9 +748,9 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     return CFBPE_OK;
 }
 
-// shared body of encode_batch / count_batch (host buffers)
+// shared body of encode_batch / encode_batch_starts / count_batch (host buffers); out_starts: NULL but for encode_batch_starts
 int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
-             uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids) {
+             uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids) {
     tl_err.clear();
     std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
     uint64_t total = 0;
@@ -752,15 +771,17 @@ int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* o
                 locks[g].reset(new LaneLock(dvs[g]));
                 lns[g] = locks[g]->ln;
                 if (lns[g]->ws_pending) { CK(cudaSetDevice(dvs[g]->device)); CK(cudaEventSynchronize(lns[g]->ev_ws)); lns[g]->ws_pending = false; }
+                if (out_starts) { CK(cudaSetDevice(dvs[g]->device)); rc = ensure_starts_lane(ctx, lns[g]); if (rc) return rc; }
             }
-            return run_host_pipelined(ctx, dvs, lns, G, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total, nullptr, nullptr, nullptr);
+            return run_host_pipelined(ctx, dvs, lns, G, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
+                                      nullptr, nullptr, nullptr);
         }
-        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total);
+        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total);
     }
     if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds max_batch_bytes of this context");
     DeviceCtx* dv = ctx->devs[0].get();
     LaneLock lk(dv);
-    return run_lane(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total);
+    return run_lane(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total);
 }
 
 
@@ -857,7 +878,7 @@ int run_host_special(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     if (!out_offsets) return fail(ctx, CFBPE_EINVAL, "out_offsets is NULL");
     if (ctx->devs.size() > 1 && n >= ctx->devs.size()) {    // one contiguous shard a device, each with its own special pass
         const SpecialArgs sa{modes, out_bad};
-        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total, &sa);
+        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, nullptr, out_cap, out_offsets, out_counts, want_ids, total, &sa);
     }
     if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds max_batch_bytes of this context");
     DeviceCtx* dv = ctx->devs[0].get();
@@ -873,7 +894,7 @@ void destroy_lane(Lane* ln) {
     cudaSetDevice(ln->device);
     free_special_lane(ln);
     cudaFree(ln->d_bytes); cudaFree(ln->d_offsets); cudaFree(ln->d_vocab_ids);
-    cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts);
+    cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts); cudaFree(ln->d_out_starts);
     cudaFree(ln->ws.piece_bits); cudaFree(ln->ws.tok_bits); cudaFree(ln->ws.ids_by_pos);
     cudaFree(ln->ws.lscratch.rank); cudaFree(ln->ws.lscratch.aux0); cudaFree(ln->ws.lscratch.aux1);
     for (uint32_t c = 0; c < 3; ++c) cudaFree(ln->ws.miss.list[c]);
@@ -1055,6 +1076,53 @@ bool load_nccl(NcclApi* n) {
     return n->CommInitAll && n->CommDestroy && n->GroupStart && n->GroupEnd && n->Broadcast && n->AllGather && n->GetErrorString;
 }
 
+// shared body of encode_batch_device / encode_batch_starts_device: d_out_starts (nullable) gets the starts, beside d_out_ids
+int run_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+               const uint8_t* d_vocab_ids, uint32_t* d_out_ids, uint32_t* d_out_starts, uint64_t out_cap, uint64_t* d_out_offsets,
+               uint32_t* d_out_counts, uint64_t* n_tokens, void* stream) {
+    std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
+    if (n_prompts > ctx->max_prompts || total_bytes > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds the limits of this context");
+    if (!d_offsets || !d_out_offsets || (total_bytes && !d_bytes)) return fail(ctx, CFBPE_EINVAL, "device pointer is NULL");
+    if (!ctx->vocabs[0].loaded && !d_vocab_ids) return fail(ctx, CFBPE_ENOENT, "vocab 0 is not loaded");
+    if (!ctx->loaded_mask) return fail(ctx, CFBPE_ENOENT, "no vocabulary is loaded");
+    // the buffers live on ONE device: the first of the context whose ordinal is current, else the first
+    DeviceCtx* dv = ctx->devs[0].get();
+    { int cur = -1; if (cudaGetDevice(&cur) == cudaSuccess) for (auto& d : ctx->devs) if (d->device == cur) dv = d.get(); }
+    LaneLock lk(dv);
+    Lane* ln = lk.ln;
+    CK(cudaSetDevice(dv->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    // a lane is one workspace: a call on another stream waits (on the device) for the lane's previous device-path call;
+    // consecutive calls take different lanes when the context has several (n_workspaces) and then overlap
+    if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws, 0));
+    const bool profiling = ctx->profiling.load();
+    ProfEvents* prof = profiling ? &ln->prof : nullptr;
+    if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); cudaEventRecord(prof->h2d[1], s); }
+    BatchView b{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes};
+    enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts,
+                   static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
+                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, d_out_starts);   // profiling: one stream, so that the per-kernel times do not overlap
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ln->ev_ws, s));
+    ln->ws_pending = true;
+    ln->dev_out_cap = out_cap;
+    ln->dev_want_ids = d_out_ids != nullptr;
+    tl_device_lane = ln;
+    if (prof) { cudaEventRecord(prof->d2h[0], s); cudaEventRecord(prof->d2h[1], s); cudaEventRecord(prof->total[1], s); }
+    if (n_tokens || prof) {
+        CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        if (prof) fill_profile(ln, total_bytes);
+        const DeviceStatus st = *ln->h_status;
+        if (n_tokens) *n_tokens = st.n_tokens;
+        if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
+        if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
+        if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
+        if (d_out_ids && st.n_tokens > out_cap) return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(st.n_tokens) + " ids");
+    }
+    return CFBPE_OK;
+}
+
 }  // namespace
 
 // Every entry point that selects a device puts the caller's current device back on return: the library is a guest in the host
@@ -1216,7 +1284,16 @@ int cfbpe_encode_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes,
                        uint32_t* out_counts) {
     DeviceGuard restore_device;
     if (!ctx) return CFBPE_EINVAL;
-    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, true);
+    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, out_ids, nullptr, out_cap, out_offsets, out_counts, true);
+}
+
+int cfbpe_encode_batch_starts(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                              uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (!out_ids || !out_starts) return fail(ctx, CFBPE_EINVAL, "out_ids and out_starts are required");
+    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, true);
 }
 
 int cfbpe_count_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets,
@@ -1224,7 +1301,7 @@ int cfbpe_count_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, 
     DeviceGuard restore_device;
     if (!ctx) return CFBPE_EINVAL;
     if (!out_counts && n_prompts) return fail(ctx, CFBPE_EINVAL, "out_counts is NULL");
-    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, nullptr, 0, nullptr, out_counts, false);
+    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, nullptr, nullptr, 0, nullptr, out_counts, false);
 }
 
 int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, const uint64_t* id_offsets,
@@ -1284,47 +1361,19 @@ int cfbpe_encode_batch_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t*
     DeviceGuard restore_device;
     if (!ctx) return CFBPE_EINVAL;
     tl_err.clear();
-    std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
-    if (n_prompts > ctx->max_prompts || total_bytes > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds the limits of this context");
-    if (!d_offsets || !d_out_offsets || (total_bytes && !d_bytes)) return fail(ctx, CFBPE_EINVAL, "device pointer is NULL");
-    if (!ctx->vocabs[0].loaded && !d_vocab_ids) return fail(ctx, CFBPE_ENOENT, "vocab 0 is not loaded");
-    if (!ctx->loaded_mask) return fail(ctx, CFBPE_ENOENT, "no vocabulary is loaded");
-    // the buffers live on ONE device: the first of the context whose ordinal is current, else the first
-    DeviceCtx* dv = ctx->devs[0].get();
-    { int cur = -1; if (cudaGetDevice(&cur) == cudaSuccess) for (auto& d : ctx->devs) if (d->device == cur) dv = d.get(); }
-    LaneLock lk(dv);
-    Lane* ln = lk.ln;
-    CK(cudaSetDevice(dv->device));
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    // a lane is one workspace: a call on another stream waits (on the device) for the lane's previous device-path call;
-    // consecutive calls take different lanes when the context has several (n_workspaces) and then overlap
-    if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws, 0));
-    const bool profiling = ctx->profiling.load();
-    ProfEvents* prof = profiling ? &ln->prof : nullptr;
-    if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); cudaEventRecord(prof->h2d[1], s); }
-    BatchView b{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes};
-    enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts,
-                   static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof);   // profiling: one stream, so that the per-kernel times do not overlap
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ln->ev_ws, s));
-    ln->ws_pending = true;
-    ln->dev_out_cap = out_cap;
-    ln->dev_want_ids = d_out_ids != nullptr;
-    tl_device_lane = ln;
-    if (prof) { cudaEventRecord(prof->d2h[0], s); cudaEventRecord(prof->d2h[1], s); cudaEventRecord(prof->total[1], s); }
-    if (n_tokens || prof) {
-        CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        if (prof) fill_profile(ln, total_bytes);
-        const DeviceStatus st = *ln->h_status;
-        if (n_tokens) *n_tokens = st.n_tokens;
-        if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
-        if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
-        if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
-        if (d_out_ids && st.n_tokens > out_cap) return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(st.n_tokens) + " ids");
-    }
-    return CFBPE_OK;
+    return run_device(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, nullptr, out_cap, d_out_offsets, d_out_counts,
+                      n_tokens, stream);
+}
+
+int cfbpe_encode_batch_starts_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                                     const uint8_t* d_vocab_ids, uint32_t* d_out_ids, uint32_t* d_out_starts, uint64_t out_cap,
+                                     uint64_t* d_out_offsets, uint32_t* d_out_counts, uint64_t* n_tokens, void* stream) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (!d_out_ids || !d_out_starts) return fail(ctx, CFBPE_EINVAL, "d_out_ids and d_out_starts are required");
+    return run_device(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, d_out_starts, out_cap, d_out_offsets, d_out_counts,
+                      n_tokens, stream);
 }
 
 int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* ids) {

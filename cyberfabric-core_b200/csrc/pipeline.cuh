@@ -158,9 +158,14 @@ inline void enqueue_scan(const BatchView& b, const Workspace& w, Stream stream, 
         CFBPE_LAUNCH(tile_scan_kernel, 1u, 32, stream, w.tile_counts, 0u, w.tile_base, w.status, token_base);   // tok_end = base
     }
 }
+// out_starts (nullable; only with out_ids, and then vs too): each token's byte offset within its prompt, at the token's rank.  The
+// token flags inside a multi-token piece are not at the tokens' first bytes (the long-piece kernels flag compacted slots), so the
+// starts come from the ids: the tokens tile the text, so a token's byte position is the sum of the byte lengths of the tokens
+// before it.  Lengths and their per-tile sums, a scan of the tile sums, then the scan inside every tile minus the prompt's offset.
+// The dense-id tile arrays are free once the ids are out (the tiles of 2048 tokens are no more than the 2 KiB piece tiles).
 template <typename Stream, typename Prof>
 inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
-                         uint32_t* out_counts, Stream stream, Prof* prof) {
+                         uint32_t* out_counts, Stream stream, Prof* prof, uint32_t* out_starts = nullptr, const VocabSet* vs = nullptr) {
     CFBPE_MARK(prof, K_EMIT, stream, true);
     if (b.total_bytes && out_ids) {
         CFBPE_LAUNCH(emit_compact_kernel, n_scan_tiles(b.total_bytes), 256, stream, w.tok_bits, w.piece_bits, n_flag_words(b.total_bytes), w.tile_base,
@@ -169,22 +174,31 @@ inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_i
     CFBPE_LAUNCH(prompt_offsets_kernel, static_cast<unsigned>((static_cast<uint64_t>(b.n_prompts) + 1 + 7) / 8), 256, stream,      // a warp per prompt boundary
                  b, w.tok_bits, w.tile_base, out_offsets, out_counts, w.status);
     CFBPE_MARK(prof, K_EMIT, stream, false);
+    if (b.total_bytes && out_ids && out_starts) {
+        const uint32_t n_tiles = static_cast<uint32_t>((b.total_bytes + kStartsTile - 1) / kStartsTile);   // (at most one token a byte)
+        CFBPE_LAUNCH(starts_len_kernel, n_tiles, 256, stream, b, *vs, out_ids, out_offsets, out_cap, w.status, out_starts, w.dense.tile_pieces);
+        CFBPE_LAUNCH(tile_scan_kernel, 1u, 1024, stream, w.dense.tile_pieces, n_tiles, w.dense.piece_base, static_cast<DeviceStatus*>(nullptr),
+                     static_cast<const uint64_t*>(nullptr));
+        CFBPE_LAUNCH(starts_emit_kernel, n_tiles, 256, stream, b, out_offsets, out_cap, w.status, w.dense.piece_base, out_starts);
+    }
 }
 template <typename Stream, typename Prof>
 inline void enqueue_back(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
-                         uint32_t* out_counts, Stream stream, Prof* prof, const uint64_t* token_base) {
+                         uint32_t* out_counts, Stream stream, Prof* prof, const uint64_t* token_base, uint32_t* out_starts = nullptr,
+                         const VocabSet* vs = nullptr) {
     enqueue_count(b, w, stream, prof);
     enqueue_scan(b, w, stream, prof, token_base);
-    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof);
+    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs);
 }
 
 // The whole path.  `aux` / `aux2` are streams of their own for the two long-piece kernels (pass the main stream to run everything
-// in order); CFBPE_FORK / CFBPE_JOIN order them.  out_ids may be nullptr (count only).  Everything is asynchronous.
+// in order); CFBPE_FORK / CFBPE_JOIN order them.  out_ids may be nullptr (count only); out_starts (nullable, with out_ids): the
+// tokens' byte offsets within their prompts.  Everything is asynchronous.
 template <typename Stream, typename Prof, typename Ev>
 inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTables& uc, const Workspace& w,
                            uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
                            uint32_t long_grid, Stream stream, Stream aux, Stream aux2, Ev ev_fork, Ev ev_join, Ev ev_join2, Prof* prof,
-                           const uint64_t* token_base = nullptr) {
+                           const uint64_t* token_base = nullptr, uint32_t* out_starts = nullptr) {
     enqueue_split(b, vs, uc, w, stream, prof, long_grid / 4);
     CFBPE_FORK(stream, aux2, ev_fork);
     enqueue_list(b, vs, w, long_grid, aux2, prof);
@@ -193,7 +207,7 @@ inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTable
     enqueue_short(b, vs, w, long_grid, stream, prof);
     CFBPE_JOIN(stream, aux, ev_join);
     CFBPE_JOIN(stream, aux2, ev_join2);
-    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base);
+    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base, out_starts, &vs);
 }
 
 }  // namespace cfbpe

@@ -157,6 +157,17 @@ CFBPE_API int cfbpe_vocab_import(cfbpe_ctx *ctx, uint32_t vocab_id, const uint8_
 CFBPE_API int cfbpe_encode_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
                        const uint8_t *vocab_ids, uint32_t *out_ids, uint64_t out_cap, uint64_t *out_offsets,
                        uint32_t *out_counts);
+/* cfbpe_encode_batch plus the byte offset of every token within its prompt: out_starts[k] (room for out_cap entries, as out_ids)
+ * is where the k-th id of the stream starts in its prompt, so token k of prompt i covers
+ * bytes[offsets[i] + out_starts[k] .. offsets[i] + end), end = out_starts[k + 1], or the prompt's length for its last token.
+ * A prompt's first token starts at 0 and the starts strictly increase within a prompt.  Ids, offsets and counts are those of
+ * cfbpe_encode_batch on the same inputs.  out_ids and out_starts are required (NULL: CFBPE_EINVAL); other arguments and errors
+ * as cfbpe_encode_batch (CFBPE_ENOSPC: out_offsets[n_prompts] = ids needed).  Costs: 4 bytes of device memory per byte of
+ * max_batch_bytes on each lane that runs such a call, allocated on its first one (CFBPE_ENOMEM if that fails), and three small
+ * kernels after the ids (the byte lengths of the ids, scanned). */
+CFBPE_API int cfbpe_encode_batch_starts(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
+                                        const uint8_t *vocab_ids, uint32_t *out_ids, uint32_t *out_starts, uint64_t out_cap,
+                                        uint64_t *out_offsets, uint32_t *out_counts);
 /* Token counts only (no id stream leaves the device). */
 CFBPE_API int cfbpe_count_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
                       const uint8_t *vocab_ids, uint32_t *out_counts);
@@ -216,6 +227,12 @@ CFBPE_API int cfbpe_encode_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, cons
                               const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t *d_out_ids,
                               uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
                               uint64_t *n_tokens, void *stream);
+/* cfbpe_encode_batch_starts on device-resident buffers, as cfbpe_encode_batch_device: the starts go straight to d_out_starts
+ * (room for out_cap entries).  d_out_ids and d_out_starts are required (NULL: CFBPE_EINVAL). */
+CFBPE_API int cfbpe_encode_batch_starts_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
+                                               const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t *d_out_ids,
+                                               uint32_t *d_out_starts, uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
+                                               uint64_t *n_tokens, void *stream);
 /* Synchronise `stream` and return the status word of the last device call (0, CFBPE_EILSEQ, CFBPE_ENOSPC). */
 CFBPE_API int cfbpe_device_status(cfbpe_ctx *ctx, void *stream);
 

@@ -109,11 +109,17 @@ impl TokenizerPluginClient for Service {
         let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
         let native = self.native.clone();
         // never block a tokio worker on a CUDA synchronisation (precedent: modules/file-parser/src/infra/parsers/html_parser.rs:47)
-        let out = tokio::task::spawn_blocking(move || native.encode_batch(&req.bytes, &req.offsets, vid.as_deref()))
+        let (out, starts) = tokio::task::spawn_blocking(move || {
+            if req.with_starts {
+                native.encode_batch_starts(&req.bytes, &req.offsets, vid.as_deref()).map(|(e, s)| (e, Some(s)))
+            } else {
+                native.encode_batch(&req.bytes, &req.offsets, vid.as_deref()).map(|e| (e, None))
+            }
+        })
             .await
             .map_err(|e| TokenizerError::Internal(e.to_string()))?
             .map_err(map_native)?;
-        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts })
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts })
     }
 
     async fn count_tokens(&self, _ctx: &SecurityContext, req: CountTokensRequest) -> Result<Vec<u32>, TokenizerError> {
@@ -172,7 +178,7 @@ impl TokenizerPluginClient for Service {
         .await
         .map_err(|e| TokenizerError::Internal(e.to_string()))?
         .map_err(map_native)?;
-        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts })
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts: None })
     }
 }
 

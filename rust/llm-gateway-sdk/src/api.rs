@@ -12,6 +12,10 @@ pub trait TokenizerClient: Send + Sync {
     /// `encode_ordinary` of every text under the vocabulary of `model` (canonical id or vocabulary name).
     async fn encode(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<Vec<u32>>, TokenizerError>;
 
+    /// Per text: the ids and each token's `[start, end)` byte span in the text's UTF-8 (cut to a context window or into chunks
+    /// at a span boundary).
+    async fn encode_with_offsets(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError>;
+
     /// tiktoken's `encode(text, allowed_special = …, disallowed_special = …)`.
     async fn encode_with_special(&self, ctx: &SecurityContext, model: &str, texts: &[String], special: &SpecialTokens)
         -> Result<Vec<Vec<u32>>, TokenizerError>;

@@ -25,15 +25,21 @@ pub struct EncodeBatchRequest {
     /// with it, `vocabs_per_prompt` lists the DISTINCT vocabularies and `vocab_index[i]` picks prompt i's
     /// (a 65 536-prompt batch carries three names and 64 KiB of indices, not 65 536 strings)
     pub vocab_index: Option<Vec<u8>>,
+    /// also return every token's byte offset within its prompt (`EncodeBatchResponse::starts`); `false` for a plain encode
+    pub with_starts: bool,
 }
 
-#[derive(Debug, Clone, Default)]
+#[derive(Debug, Clone, Default, Serialize, Deserialize)]
 pub struct EncodeBatchResponse {
     /// dense id stream of all prompts (tiktoken `encode_ordinary` semantics, bit-exact)
     pub ids: Vec<u32>,
     /// `n + 1` offsets into `ids`
     pub offsets: Vec<u64>,
     pub counts: Vec<u32>,
+    /// with `with_starts`: one entry per id, the byte offset of the token within its prompt (token k of prompt i covers
+    /// `bytes[offsets_in[i] + starts[k] .. offsets_in[i] + end)`, `end` the next start or the prompt's length)
+    #[serde(default, skip_serializing_if = "Option::is_none")]
+    pub starts: Option<Vec<u32>>,
 }
 
 #[derive(Debug, Clone)]

@@ -66,14 +66,14 @@ pub trait TokenizerPluginClient: Send + Sync {
             plan.push(steps);
         }
         let enc = if stretches.is_empty() {
-            EncodeBatchResponse { ids: Vec::new(), offsets: vec![0], counts: Vec::new() }
+            EncodeBatchResponse { ids: Vec::new(), offsets: vec![0], counts: Vec::new(), starts: None }
         } else {
             let mut bytes = Vec::new();
             let mut offsets = vec![0u64];
             for s in &stretches { bytes.extend_from_slice(s.as_bytes()); offsets.push(bytes.len() as u64); }
-            self.encode_batch(ctx, EncodeBatchRequest { vocab: req.vocab.clone(), bytes: bytes.into(), offsets, vocabs_per_prompt: per.take(), vocab_index: None }).await?
+            self.encode_batch(ctx, EncodeBatchRequest { vocab: req.vocab.clone(), bytes: bytes.into(), offsets, vocabs_per_prompt: per.take(), vocab_index: None, with_starts: false }).await?
         };
-        let mut out = EncodeBatchResponse { ids: Vec::new(), offsets: vec![0u64], counts: Vec::with_capacity(n) };
+        let mut out = EncodeBatchResponse { ids: Vec::new(), offsets: vec![0u64], counts: Vec::with_capacity(n), starts: None };
         for steps in plan {
             let start = out.ids.len();
             for s in steps {

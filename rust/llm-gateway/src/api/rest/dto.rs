@@ -13,6 +13,9 @@ pub struct TokenizeRequest {
     /// return the ids as well as the counts
     #[serde(default)]
     pub return_ids: bool,
+    /// return each token's `[start, end)` byte span in its text's UTF-8 as well
+    #[serde(default)]
+    pub return_offsets: bool,
 }
 
 #[derive(Debug, Serialize, JsonSchema)]
@@ -23,6 +26,9 @@ pub struct TokenizeResponse {
     /// token ids of every text, when asked for
     #[serde(skip_serializing_if = "Option::is_none")]
     pub ids: Option<Vec<Vec<u32>>>,
+    /// byte span of every token of every text, when asked for
+    #[serde(skip_serializing_if = "Option::is_none")]
+    pub offsets: Option<Vec<Vec<[u64; 2]>>>,
 }
 
 /// How the provider frames the messages (`llm_gateway_sdk::ChatTemplate`); absent: content only.

@@ -27,10 +27,16 @@ pub async fn tokenize(
 ) -> Result<Json<TokenizeResponse>, Problem> {
     // only sizes are logged, never the text (docs/DESIGN.md:120-124)
     tracing::debug!(model = %req.model, texts = req.texts.len(), bytes = req.texts.iter().map(String::len).sum::<usize>(), "tokenize");
-    let ids = service.encode(&ctx, &req.model, &req.texts).await.map_err(problem)?;
+    let (ids, offsets) = if req.return_offsets {
+        let r = service.encode_with_offsets(&ctx, &req.model, &req.texts).await.map_err(problem)?;
+        let (ids, spans): (Vec<_>, Vec<_>) = r.into_iter().unzip();
+        (ids, Some(spans))
+    } else {
+        (service.encode(&ctx, &req.model, &req.texts).await.map_err(problem)?, None)
+    };
     let counts: Vec<u32> = ids.iter().map(|v| v.len() as u32).collect();
     let input_tokens = counts.iter().map(|c| u64::from(*c)).sum();
-    Ok(Json(TokenizeResponse { counts, input_tokens, ids: req.return_ids.then_some(ids) }))
+    Ok(Json(TokenizeResponse { counts, input_tokens, ids: req.return_ids.then_some(ids), offsets }))
 }
 
 pub async fn count_tokens(

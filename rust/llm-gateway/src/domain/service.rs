@@ -74,8 +74,22 @@ impl TokenizerService {
 impl TokenizerClient for TokenizerService {
     async fn encode(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<Vec<u32>>, TokenizerError> {
         let (bytes, offsets) = pack_texts(texts);
-        let r = self.plugin().await?.encode_batch(ctx, EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None }).await?;
+        let r = self.plugin().await?.encode_batch(ctx, EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false }).await?;
         Ok((0..texts.len()).map(|i| r.ids[r.offsets[i] as usize..r.offsets[i + 1] as usize].to_vec()).collect())
+    }
+
+    async fn encode_with_offsets(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError> {
+        let (bytes, offsets) = pack_texts(texts);
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets: offsets.clone(), vocabs_per_prompt: None, vocab_index: None,
+                                       with_starts: true };
+        let r = self.plugin().await?.encode_batch(ctx, req).await?;
+        let starts = r.starts.ok_or_else(|| TokenizerError::ServiceUnavailable("the tokenizer plugin does not return token starts".to_owned()))?;
+        Ok((0..texts.len()).map(|i| {
+            let (a, b) = (r.offsets[i] as usize, r.offsets[i + 1] as usize);
+            let len = offsets[i + 1] - offsets[i];
+            let spans = (a..b).map(|k| [u64::from(starts[k]), if k + 1 < b { u64::from(starts[k + 1]) } else { len }]).collect();
+            (r.ids[a..b].to_vec(), spans)
+        }).collect())
     }
 
     async fn encode_with_special(&self, ctx: &SecurityContext, model: &str, texts: &[String], special: &SpecialTokens)
@@ -85,7 +99,7 @@ impl TokenizerClient for TokenizerService {
             return Err(TokenizerError::InvalidInput(format!("allowed special token without an id: {unknown}")));
         }
         let (bytes, offsets) = pack_texts(texts);
-        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None };
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false };
         let r = self.plugin().await?.encode_batch_special(ctx, req, special).await?;
         Ok((0..texts.len()).map(|i| r.ids[r.offsets[i] as usize..r.offsets[i + 1] as usize].to_vec()).collect())
     }
