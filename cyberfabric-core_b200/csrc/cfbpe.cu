@@ -212,6 +212,17 @@ int fail(cfbpe_ctx*, int code, const std::string& msg) {
 template <typename T>
 cudaError_t dmalloc(T** p, uint64_t count) { return cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T)); }
 
+// the error a pass's status reports (status_error), or CFBPE_OK
+int fail_status(cfbpe_ctx* ctx, const DeviceStatus& st) {
+    const StatusError e = status_error(st);
+    return e.code ? fail(ctx, e.code, e.msg) : CFBPE_OK;
+}
+// out_cap is too small for the call's `need` ids; a host call also learns it in out_offsets[n]
+int fail_nospace(cfbpe_ctx* ctx, uint64_t need, uint64_t* out_offsets = nullptr, uint32_t n = 0) {
+    if (out_offsets) out_offsets[n] = need;
+    return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(need) + " ids");
+}
+
 // a free lane of the device, locked: round robin without waiting; when all are busy, wait for the next in turn
 struct LaneLock {
     Lane* ln = nullptr;
@@ -345,13 +356,30 @@ int ensure_starts_lane(cfbpe_ctx* ctx, Lane* ln) {
     return CFBPE_OK;
 }
 
+// an asynchronous device-path call may still own the lane's workspace: wait for it (the caller has selected the lane's device)
+int wait_for_device_call(cfbpe_ctx* ctx, Lane* ln) {
+    if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }
+    return CFBPE_OK;
+}
+
+// the inputs of a one-pass host call into the lane's buffers, on s; *b: the batch as the kernels see it
+int upload_batch(cfbpe_ctx* ctx, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids, uint64_t total,
+                 cudaStream_t s, BatchView* b) {
+    if (total) CK(cudaMemcpyAsync(ln->d_bytes, bytes, total, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ln->d_offsets, offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    if (vocab_ids && n) CK(cudaMemcpyAsync(ln->d_vocab_ids, vocab_ids, n, cudaMemcpyHostToDevice, s));
+    *b = BatchView{ln->d_bytes, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n, total};
+    return CFBPE_OK;
+}
+
 // Pipelined host call: the batch is cut into sub-batches of ~kPipeChunkBytes on prompt boundaries; each is an
 // independent encode pass on its own slice of the workspace.  Uploads (h2d_stream) run ahead of the kernels
 // (stream), downloads (d2h_stream) trail them; token ranks are chained on the device (DeviceStatus::tok_end), so
 // ids and offsets land at their final places.  The host only waits for each sub-batch's status to learn how many
 // ids to fetch.
 // defer != nullptr (a shard of a multi-device call): nothing is downloaded here -- ids, offsets and counts stay in the lane's device
-// buffers (dense, shard-local ranks: sub-batch k's offsets at d_out_offsets + p_k + k) and *defer gets the shard's token total.
+// buffers (dense, shard-local ranks: sub-batch k's offsets at d_out_offsets + sub_batch_offsets_at(p_k, k)) and *defer gets the
+// shard's token total.
 int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, int G, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
                        const uint8_t* vocab_ids, uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
                        bool want_ids, uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out) {
@@ -363,11 +391,11 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
     // needs from its predecessor -- the token rank it starts at -- is read from the predecessor's device over NVLink (peer
     // memory), behind a cross-device event.  Uploads and downloads of the devices run side by side on their own PCIe links.
     Lane* ln = lns[0];                       // (host-side staging of the offsets and the trace live in the first lane)
-    // local offsets of every sub-batch, staged in pinned memory (sub-batch k occupies [p_k + k, p_{k+1} + k])
+    // local offsets of every sub-batch, staged in pinned memory in the device layout
     for (int k = 0; k < nc; ++k) {
         const uint32_t p0 = cut[k], p1 = cut[k + 1];
         const uint64_t o0 = offsets[p0];
-        uint64_t* dst = ln->h_offs_stage + p0 + k;
+        uint64_t* dst = ln->h_offs_stage + sub_batch_offsets_at(p0, k);
         for (uint32_t i = p0; i <= p1; ++i) dst[i - p0] = offsets[i] - o0;
     }
     // ---- enqueue everything that does not depend on the host knowing a result
@@ -388,11 +416,10 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (G > 1) CK(cudaSetDevice(dv->device));
         cudaStream_t cs = ln->stream, hs = ln->h2d_stream;
         const uint32_t p0 = cut[k], p1 = cut[k + 1], nk = p1 - p0;
-        const uint64_t o0 = offsets[p0], len = offsets[p1] - o0;
-        // every sub-batch lands on a 16-byte boundary of the device buffer (K1 reads 16 bytes per lane with one load)
-        uint8_t* const d_sub = ln->d_bytes + ((o0 + 15) & ~15ull) + 16ull * k;
+        const uint64_t o0 = offsets[p0], len = offsets[p1] - o0, q0 = sub_batch_offsets_at(p0, k);
+        uint8_t* const d_sub = ln->d_bytes + sub_batch_bytes_at(o0, k);
         if (len && !no_copy) CK(cudaMemcpyAsync(d_sub, bytes + o0, len, cudaMemcpyHostToDevice, hs));
-        CK(cudaMemcpyAsync(ln->d_offsets + p0 + k, lns[0]->h_offs_stage + p0 + k, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, hs));
+        CK(cudaMemcpyAsync(ln->d_offsets + q0, lns[0]->h_offs_stage + q0, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, hs));
         if (vocab_ids && nk) CK(cudaMemcpyAsync(ln->d_vocab_ids + p0, vocab_ids + p0, nk, cudaMemcpyHostToDevice, hs));
         CK(cudaEventRecord(ln->ev_h2d[k], hs));
         if (trace) CK(cudaEventRecord(ln->trace[k][0], hs));
@@ -400,22 +427,9 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         cudaStream_t ck = fk ? ln->front[fk] : cs;
         const int lv = ln->prio_mode == 2 ? (k * ln->prio_levels) / nc : 0;
         if (ln->prio_mode) ck = ln->pool[lv][(3 * k + 2) % kPoolSlots];   // the short-piece kernels of sub-batch k: priority falls with k (earlier sub-batches finish, and download, first)
-        Workspace w = ln->ws;
-        const uint64_t w0 = (o0 >> 5) + 4ull * k;
-        w.piece_bits += w0; w.tok_bits += w0; w.pstart_bits += w0;
-        w.block_prompt += (o0 >> kPromptBlockShift) + 2ull * k;
-        w.dense.by_piece += o0; w.dense.extras += o0; w.dense.extras_cap = static_cast<uint32_t>(len + 1);
-        w.dense.tile_pieces += (o0 >> 11) + 2ull * k; w.dense.piece_base += (o0 >> 11) + 2ull * k;
-        w.ids_by_pos += o0; w.lscratch.rank += o0; w.lscratch.aux0 += o0; w.lscratch.aux1 += o0;
-        w.long_list += (o0 >> 5) + k;
-        w.long_cap = static_cast<uint32_t>(len / 32 + 1);
-        const uint64_t t0 = (o0 >> 13) + 2ull * k;
-        w.tile_counts += t0; w.tile_base += t0;
+        Workspace w = slice_workspace(ln->ws, o0, len, static_cast<uint32_t>(k));
         w.status = ln->d_status_arr + k;
-        w.miss = slice_miss(ln->ws.miss, o0, len, static_cast<uint32_t>(k));
-        w.fix_list += (o0 >> 4) + 2ull * k;
-        w.fix_cap = static_cast<uint32_t>(len / 16 + 2);
-        BatchView b{d_sub, ln->d_offsets + p0 + k, vocab_ids ? ln->d_vocab_ids + p0 : nullptr, nk, len};
+        BatchView b{d_sub, ln->d_offsets + q0, vocab_ids ? ln->d_vocab_ids + p0 : nullptr, nk, len};
         // split, long pieces and the back stage run on a top-priority stream of their own: the long-piece kernels are a latency
         // chain that uses little of the machine, so they start as early as possible and the short-piece kernels fill the rest
         cudaStream_t ss = ln->prio_mode ? ln->pool[lv][(3 * k) % kPoolSlots] : ln->side[k % kSideStreams];
@@ -441,7 +455,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (k) CK(cudaStreamWaitEvent(ss, prev->ev_chain[k - 1], 0));    // token ranks chain through DeviceStatus::tok_end: only the scan waits
         enqueue_scan(b, w, ss, static_cast<ProfEvents*>(nullptr), k ? &prev->d_status_arr[k - 1].tok_end : nullptr);   // (G > 1: a peer pointer)
         CK(cudaEventRecord(ln->ev_chain[k], ss));
-        enqueue_emit(b, w, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets + p0 + k, ln->d_out_counts + p0,
+        enqueue_emit(b, w, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets + q0, ln->d_out_counts + p0,
                      ss, static_cast<ProfEvents*>(nullptr), out_starts ? ln->d_out_starts : nullptr, &dv->vs);
         CK(cudaGetLastError());
         status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr + k, ln->h_status_arr + k);
@@ -458,9 +472,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         CK(cudaEventSynchronize(ln->ev_done[k]));
         const DeviceStatus st = ln->h_status_arr[k];
         const uint32_t p0 = cut[k], p1 = cut[k + 1], nk = p1 - p0;
-        if ((st.long_overflow || st.miss_overflow) && !err) err = fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
-        if (st.bad_vocab && !err) err = fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
-        if (st.bad_utf8 && !err) err = fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
+        if (!err) err = fail_status(ctx, st);
         const uint64_t base = st.tok_end - st.n_tokens;
         tok_total = st.tok_end;
         if (err || defer) continue;
@@ -469,7 +481,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
             CK(cudaMemcpyAsync(out_ids + base, ln->d_out_ids + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (out_starts && st.tok_end <= out_cap && st.n_tokens)      // (prompt-relative: the same ranks and base as the ids)
             CK(cudaMemcpyAsync(out_starts + base, ln->d_out_starts + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
-        if (out_offsets) CK(cudaMemcpyAsync(out_offsets + p0, ln->d_out_offsets + p0 + k, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
+        if (out_offsets) CK(cudaMemcpyAsync(out_offsets + p0, ln->d_out_offsets + sub_batch_offsets_at(p0, k), (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
         if (out_counts && nk) CK(cudaMemcpyAsync(out_counts + p0, ln->d_out_counts + p0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (trace) { CK(cudaEventRecord(ln->trace[k][5], ds)); host_dl[k] = host_ms(); }
     }
@@ -494,10 +506,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
     }
     if (err) return err;
     if (defer) { *defer = tok_total; if (cut_out) { std::memcpy(cut_out, cut, sizeof(uint32_t) * (nc + 1)); *nc_out = nc; } return CFBPE_OK; }
-    if (want_ids && tok_total > out_cap) {
-        if (out_offsets) out_offsets[n] = tok_total;
-        return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(tok_total) + " ids");
-    }
+    if (want_ids && tok_total > out_cap) return fail_nospace(ctx, tok_total, out_offsets, n);
     return CFBPE_OK;
 }
 
@@ -508,8 +517,9 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
              uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
              uint64_t* defer = nullptr, uint32_t* cut_out = nullptr, int* nc_out = nullptr) {
     CK(cudaSetDevice(dv->device));
-    if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }   // an asynchronous device-path call still owns the workspace
-    if (out_starts) { const int rc = ensure_starts_lane(ctx, ln); if (rc) return rc; }
+    int rc = wait_for_device_call(ctx, ln);
+    if (!rc && out_starts) rc = ensure_starts_lane(ctx, ln);
+    if (rc) return rc;
     const bool profiling = ctx->profiling.load();
     if (!profiling && total >= ctx->pipe_min && n >= 2)
         return run_host_pipelined(ctx, &dv, &ln, 1, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
@@ -517,12 +527,11 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     cudaStream_t s = ln->stream;
     ProfEvents* prof = profiling ? &ln->prof : nullptr;
     if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); }
-    if (total) CK(cudaMemcpyAsync(ln->d_bytes, bytes, total, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ln->d_offsets, offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-    if (vocab_ids && n) CK(cudaMemcpyAsync(ln->d_vocab_ids, vocab_ids, n, cudaMemcpyHostToDevice, s));
+    BatchView b;
+    rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b);
+    if (rc) return rc;
     if (prof) cudaEventRecord(prof->h2d[1], s);
 
-    BatchView b{ln->d_bytes, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n, total};
     enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets,
                    ln->d_out_counts, static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
                    ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, out_starts ? ln->d_out_starts : nullptr);
@@ -535,15 +544,10 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     }
     CK(cudaStreamSynchronize(s));
     const DeviceStatus st = *ln->h_status;
-    if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
-    if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
-    if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
+    if ((rc = fail_status(ctx, st))) return rc;
     if (defer) { *defer = st.n_tokens; if (cut_out) { cut_out[0] = 0; cut_out[1] = n; *nc_out = 1; } return CFBPE_OK; }
     if (want_ids) {
-        if (st.n_tokens > out_cap) {
-            if (out_offsets) out_offsets[n] = st.n_tokens;
-            return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(st.n_tokens) + " ids");
-        }
+        if (st.n_tokens > out_cap) return fail_nospace(ctx, st.n_tokens, out_offsets, n);
         if (st.n_tokens) CK(cudaMemcpyAsync(out_ids, ln->d_out_ids, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         if (out_starts && st.n_tokens) CK(cudaMemcpyAsync(out_starts, ln->d_out_starts, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     }
@@ -601,32 +605,57 @@ SpecialWork special_work(Lane* ln) {
     return SpecialWork{sp.kept_n, sp.kept_base, sp.st_off, sp.st_vocab, sp.st_id, sp.st_base, sp.status};
 }
 
-// The special set of one call on device dv: the tables of the vocabularies that look for some special in it (every registered
-// special is DISALLOWED when modes[v] is NULL), the call's mode bytes uploaded into the lane.  *scan = false: no vocabulary looks
-// for any special, the call is the ordinary path.
+// The special set of one call on device dv (fill_special_set), with the lane's special buffers allocated and the call's mode bytes
+// uploaded into them.  *scan = false: no vocabulary looks for any special, the call is the ordinary path.
 int special_set(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const uint8_t* const* modes, SpecialSet* out, bool* scan, cudaStream_t s) {
-    *out = SpecialSet{};
-    *scan = false;
+    int rc = ensure_special_lane(ctx, ln);
+    if (rc) return rc;
+    const uint32_t* words[CFBPE_MAX_VOCABS];
+    for (uint32_t v = 0; v < CFBPE_MAX_VOCABS; ++v) words[v] = ctx->specials[v].empty() ? nullptr : ctx->specials[v].data();
+    uint32_t bad[2];
+    if (fill_special_set(words, dv->specials.v, modes, out, scan, bad))
+        return fail(ctx, CFBPE_EINVAL, "modes[" + std::to_string(bad[0]) + "][" + std::to_string(bad[1]) + "] is not a CFBPE_SPECIAL_* value");
     for (uint32_t v = 0; v < CFBPE_MAX_VOCABS; ++v) {
-        const std::vector<uint32_t>& w = ctx->specials[v];
-        if (w.empty()) continue;
-        const uint32_t n = w[0];
-        const uint8_t* m = modes ? modes[v] : nullptr;
-        if (m) {
-            bool looks = false;
-            for (uint32_t k = 0; k < n; ++k) {
-                if (m[k] > CFBPE_SPECIAL_DISALLOW) return fail(ctx, CFBPE_EINVAL, "modes[" + std::to_string(v) + "][" + std::to_string(k) + "] is not a CFBPE_SPECIAL_* value");
-                looks = looks || m[k] != CFBPE_SPECIAL_ORDINARY;
-            }
-            if (!looks) continue;
-            uint8_t* dm = ln->sp.modes + static_cast<uint64_t>(v) * kMaxSpecials;
-            CK(cudaMemcpyAsync(dm, m, n, cudaMemcpyHostToDevice, s));
-            out->modes[v] = dm;
-        }
-        out->v[v] = dv->specials.v[v];
-        for (uint32_t j = 0; j < 8; ++j) out->first_bytes[j] |= w[kSpHeaderWords + j];
-        *scan = true;
+        if (!out->modes[v]) continue;
+        uint8_t* dm = ln->sp.modes + static_cast<uint64_t>(v) * kMaxSpecials;
+        CK(cudaMemcpyAsync(dm, out->modes[v], words[v][0], cudaMemcpyHostToDevice, s));
+        out->modes[v] = dm;
     }
+    return CFBPE_OK;
+}
+
+// Where the ids, offsets and counts of an encode pass go
+struct EncodeOut { uint32_t* ids; uint64_t cap; uint64_t* offsets; uint32_t* counts; };
+
+// The rest of a special call once its batch is on the device and special_set has run: the scan (when some vocabulary looks for a
+// special) and what it found, then the ordinary path on the prompts as they are, into `plain`, or on the stretches followed by the
+// splice, into `spliced` (the stretches' own ids, offsets and counts go to the lane's d_out_* buffers).  *did_splice: which ran.
+int enqueue_special_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchView& b, const SpecialSet& sp, bool scan, cudaStream_t s,
+                         const EncodeOut& plain, const EncodeOut& spliced, uint32_t* out_bad, bool* did_splice) {
+    const SpecialWork sw = special_work(ln);
+    uint64_t n_str = b.n_prompts;
+    if (scan) {       // the one synchronisation of the call: the host needs the number of stretches for the launch geometry
+        enqueue_special_scan(b, sp, ln->ws, sw, s);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        const SpecialScanResult r = special_scan_result(*ln->sp.h_status, b.n_prompts, ctx->max_prompts);
+        if (r.disallowed) return fail_disallowed(ctx, r.prompt, r.vocab, r.index, out_bad);
+        if (!r.fits)
+            return fail(ctx, CFBPE_EINVAL, "n_prompts + 2 x special-token matches (" + std::to_string(r.n_stretches) + ") exceeds max_prompts of this context");
+        n_str = r.n_stretches;
+    }
+    *did_splice = n_str != b.n_prompts;
+    const uint32_t grid = static_cast<uint32_t>(dv->sm_count * 4);
+    if (!*did_splice) {
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, plain.ids, plain.cap, plain.offsets, plain.counts, grid,
+                       s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+    } else {
+        enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets,
+                               ln->d_out_counts, spliced.ids, spliced.cap, spliced.offsets, spliced.counts,
+                               grid, s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+    }
+    CK(cudaGetLastError());
     return CFBPE_OK;
 }
 
@@ -721,12 +750,12 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             ck(cudaSetDevice(ctx->devs[d]->device), "cudaSetDevice");
             cudaStream_t st = ln->stream;
             ck(cudaMemcpyAsync(ln->h_totals, ln->d_totals, sizeof(uint64_t) * G, cudaMemcpyDeviceToHost, st), "totals download");
-            for (int k = 0; k < s.nc; ++k) {     // sub-batch k's offsets sit at d_out_offsets + cut[k] + k (run_host_pipelined)
+            for (int k = 0; k < s.nc; ++k) {
                 const uint32_t q0 = s.cut[k], nk = s.cut[k + 1] - s.cut[k];
                 const bool last = (k + 1 == s.nc) && (d + 1 == G);
                 const uint64_t cnt = static_cast<uint64_t>(nk) + (last ? 1 : 0);      // the boundary entry belongs to the next sub-batch / shard
                 if (!cnt) continue;
-                uint64_t* src = ln->d_out_offsets + q0 + (s.nc > 1 ? k : 0);
+                uint64_t* src = ln->d_out_offsets + sub_batch_offsets_at(q0, k);
                 rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(src, cnt, ln->d_totals, d);
                 if (out_offsets) ck(cudaMemcpyAsync(out_offsets + p0 + q0, src, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st), "offsets download");
                 if (out_counts && nk) ck(cudaMemcpyAsync(out_counts + p0 + q0, ln->d_out_counts + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "counts download");
@@ -741,10 +770,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
         for (auto& t : th) t.join();
     }
     for (uint32_t d = 0; d < G; ++d) if (rcs[d]) return fail(ctx, rcs[d], errs[d]);
-    if (!fits) {
-        if (out_offsets) out_offsets[n] = grand;
-        return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(grand) + " ids");
-    }
+    if (!fits) return fail_nospace(ctx, grand, out_offsets, n);
     return CFBPE_OK;
 }
 
@@ -770,8 +796,10 @@ int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* o
                 dvs[g] = ctx->devs[g].get();
                 locks[g].reset(new LaneLock(dvs[g]));
                 lns[g] = locks[g]->ln;
-                if (lns[g]->ws_pending) { CK(cudaSetDevice(dvs[g]->device)); CK(cudaEventSynchronize(lns[g]->ev_ws)); lns[g]->ws_pending = false; }
-                if (out_starts) { CK(cudaSetDevice(dvs[g]->device)); rc = ensure_starts_lane(ctx, lns[g]); if (rc) return rc; }
+                CK(cudaSetDevice(dvs[g]->device));
+                rc = wait_for_device_call(ctx, lns[g]);
+                if (!rc && out_starts) rc = ensure_starts_lane(ctx, lns[g]);
+                if (rc) return rc;
             }
             return run_host_pipelined(ctx, dvs, lns, G, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
                                       nullptr, nullptr, nullptr);
@@ -792,52 +820,21 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
                      const uint8_t* const* modes, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
                      uint64_t total, uint32_t* out_bad, uint64_t* defer) {
     CK(cudaSetDevice(dv->device));
-    if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }
-    int rc = ensure_special_lane(ctx, ln);
+    int rc = wait_for_device_call(ctx, ln);
     if (rc) return rc;
     cudaStream_t s = ln->stream;
     SpecialSet sp;
-    bool scan = false;
-    rc = special_set(ctx, dv, ln, modes, &sp, &scan, s);
-    if (rc) return rc;
-    if (total) CK(cudaMemcpyAsync(ln->d_bytes, bytes, total, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ln->d_offsets, offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-    if (vocab_ids && n) CK(cudaMemcpyAsync(ln->d_vocab_ids, vocab_ids, n, cudaMemcpyHostToDevice, s));
-    const BatchView b{ln->d_bytes, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n, total};
-    const SpecialWork sw = special_work(ln);
-    uint64_t n_str = n;
-    if (scan) {
-        enqueue_special_scan(b, sp, ln->ws, sw, s);
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        const SpecialStatus ss = *ln->sp.h_status;
-        if (ss.bad_inv) {
-            const unsigned long long key = ~ss.bad_inv;
-            return fail_disallowed(ctx, ss.bad_prompt, static_cast<uint32_t>((key >> 12) & 7u), static_cast<uint32_t>(key & 0xFFFu), out_bad);
-        }
-        n_str = n + 2 * ss.kept.n_tokens;
-        if (n_str > ctx->max_prompts)
-            return fail(ctx, CFBPE_EINVAL, "n_prompts + 2 x special-token matches (" + std::to_string(n_str) + ") exceeds max_prompts of this context");
-    }
-    const bool spliced = n_str != n;
-    const uint32_t grid = static_cast<uint32_t>(dv->sm_count * 4);
-    if (!spliced) {
-        enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets, ln->d_out_counts, grid,
-                       s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
-    } else {
-        enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets,
-                               ln->d_out_counts, want_ids ? ln->ws.lscratch.rank : nullptr, ctx->max_bytes, ln->sp.fin_offsets, ln->sp.fin_counts,
-                               grid, s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
-        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
-    }
-    CK(cudaGetLastError());
+    bool scan = false, spliced = false;
+    BatchView b;
+    if ((rc = special_set(ctx, dv, ln, modes, &sp, &scan, s)) || (rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b))) return rc;
+    const EncodeOut plain{want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets, ln->d_out_counts};
+    const EncodeOut fin{want_ids ? ln->ws.lscratch.rank : nullptr, ctx->max_bytes, ln->sp.fin_offsets, ln->sp.fin_counts};
+    if ((rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, plain, fin, out_bad, &spliced))) return rc;
+    if (spliced) CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     const DeviceStatus st = *ln->h_status;
-    if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
-    if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
-    if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
+    if ((rc = fail_status(ctx, st))) return rc;
     const uint64_t n_tokens = spliced ? ln->sp.h_status->fin.n_tokens : st.n_tokens;
     // where the call's ids, offsets and counts are on the device
     const uint32_t* ids_src = spliced ? ln->ws.lscratch.rank : ln->d_out_ids;
@@ -857,8 +854,7 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
     if (out_counts && n) CK(cudaMemcpyAsync(out_counts, counts_src, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     if (want_ids && n_tokens > out_cap) {
         CK(cudaStreamSynchronize(s));
-        if (out_offsets) out_offsets[n] = n_tokens;
-        return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(n_tokens) + " ids");
+        return fail_nospace(ctx, n_tokens, out_offsets, n);
     }
     if (want_ids && n_tokens) CK(cudaMemcpyAsync(out_ids, ids_src, n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -895,13 +891,9 @@ void destroy_lane(Lane* ln) {
     free_special_lane(ln);
     cudaFree(ln->d_bytes); cudaFree(ln->d_offsets); cudaFree(ln->d_vocab_ids);
     cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts); cudaFree(ln->d_out_starts);
-    cudaFree(ln->ws.piece_bits); cudaFree(ln->ws.tok_bits); cudaFree(ln->ws.ids_by_pos);
-    cudaFree(ln->ws.lscratch.rank); cudaFree(ln->ws.lscratch.aux0); cudaFree(ln->ws.lscratch.aux1);
-    for (uint32_t c = 0; c < 3; ++c) cudaFree(ln->ws.miss.list[c]);
+    for_each_ws_buffer(ln->ws, [](auto*& p, WsKind) { cudaFree(p); });
+    cudaFree(ln->ws.status);
     cudaFree(ln->d_dec_sums); cudaFree(ln->d_dec_base); cudaFree(ln->d_totals);
-    cudaFree(ln->ws.dense.by_piece); cudaFree(ln->ws.dense.extras); cudaFree(ln->ws.dense.tile_pieces); cudaFree(ln->ws.dense.piece_base);
-    cudaFree(ln->ws.fix_list); cudaFree(ln->ws.pstart_bits); cudaFree(ln->ws.block_prompt);
-    cudaFree(ln->ws.long_list); cudaFree(ln->ws.tile_counts); cudaFree(ln->ws.tile_base); cudaFree(ln->ws.status);
     if (ln->h_status) cudaFreeHost(ln->h_status);
     if (ln->h_status_arr) cudaFreeHost(ln->h_status_arr);
     if (ln->h_offs_stage) cudaFreeHost(ln->h_offs_stage);
@@ -936,44 +928,21 @@ void destroy_lane(Lane* ln) {
 bool create_lane(Lane* ln, int device, uint64_t mb, uint64_t mp) {
     ln->device = device;
     ln->max_bytes = mb;
-    const uint64_t nw = n_flag_words(mb) + 4 + 4 * kMaxPipeChunks;      // + per-sub-batch slack of a pipelined call
-    const uint64_t nt = n_scan_tiles(mb) + 1 + 2 * kMaxPipeChunks;
     int prio_lo = 0, prio_hi = 0;
     cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
     bool ok = cudaStreamCreateWithPriority(&ln->stream, cudaStreamNonBlocking, prio_hi) == cudaSuccess;   // front stream of sub-batch 0
-    ok = ok && dmalloc(&ln->d_bytes, mb + 256 + 16 * (kMaxPipeChunks + 1)) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_offsets, mp + 1 + kMaxPipeChunks) == cudaSuccess;
+    ok = ok && dmalloc(&ln->d_bytes, lane_bytes_alloc(mb, kMaxPipeChunks)) == cudaSuccess;
+    ok = ok && dmalloc(&ln->d_offsets, lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
     ok = ok && dmalloc(&ln->d_vocab_ids, mp + 1) == cudaSuccess;
     ok = ok && dmalloc(&ln->d_out_ids, mb + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_out_offsets, mp + 1 + kMaxPipeChunks) == cudaSuccess;
+    ok = ok && dmalloc(&ln->d_out_offsets, lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
     ok = ok && dmalloc(&ln->d_out_counts, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.piece_bits, nw) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.tok_bits, nw) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.ids_by_pos, mb + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.lscratch.rank, mb + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.lscratch.aux0, mb + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.lscratch.aux1, mb + 1) == cudaSuccess;
-    ln->ws.long_cap = static_cast<uint32_t>(mb / 32 + 1 + kMaxPipeChunks);   // a long piece holds more than 32 bytes
-    ok = ok && dmalloc(&ln->ws.long_list, ln->ws.long_cap) == cudaSuccess;
-    for (uint32_t c = 0; c < 3; ++c) {
-        const uint64_t words = miss_list_words(mb, c, kMaxPipeChunks);      // 64-bit entries
-        ok = ok && dmalloc(&ln->ws.miss.list[c], words) == cudaSuccess;
-        ln->ws.miss.cap[c] = static_cast<uint32_t>(words);
-    }
-    ok = ok && dmalloc(&ln->ws.dense.by_piece, mb + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.dense.extras, mb + 1) == cudaSuccess;
-    ln->ws.dense.extras_cap = static_cast<uint32_t>(mb + 1);
-    ok = ok && dmalloc(&ln->ws.dense.tile_pieces, (mb >> 11) + 2 + 2 * kMaxPipeChunks) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.dense.piece_base, (mb >> 11) + 2 + 2 * kMaxPipeChunks) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.pstart_bits, nw) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.block_prompt, (mb >> kPromptBlockShift) + 2 + 2 * kMaxPipeChunks) == cudaSuccess;
-    ln->ws.fix_cap = static_cast<uint32_t>(mb / 16 + 2 + 2 * kMaxPipeChunks);
-    ok = ok && dmalloc(&ln->ws.fix_list, ln->ws.fix_cap) == cudaSuccess;
+    const WsSizes ws = workspace_alloc(mb, kMaxPipeChunks);
+    for_each_ws_buffer(ln->ws, [&](auto*& p, WsKind kind) { ok = ok && dmalloc(&p, ws.n[kind]) == cudaSuccess; });
+    set_workspace_caps(ln->ws, ws);      // a one-shot call may use all of it
     ok = ok && dmalloc(&ln->d_dec_sums, mb / kDecodeTile + 2) == cudaSuccess;
     ok = ok && dmalloc(&ln->d_dec_base, mb / kDecodeTile + 2) == cudaSuccess;
     ok = ok && dmalloc(&ln->d_totals, CFBPE_MAX_DEVICES + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.tile_counts, nt) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.tile_base, nt) == cudaSuccess;
     ok = ok && dmalloc(&ln->ws.status, 1) == cudaSuccess;
     ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_status), sizeof(DeviceStatus)) == cudaSuccess;
     ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_totals), sizeof(uint64_t) * (CFBPE_MAX_DEVICES + 1)) == cudaSuccess;
@@ -981,7 +950,7 @@ bool create_lane(Lane* ln, int device, uint64_t mb, uint64_t mp) {
     ok = ok && cudaStreamCreateWithFlags(&ln->d2h_stream, cudaStreamNonBlocking) == cudaSuccess;
     ok = ok && dmalloc(&ln->d_status_arr, kMaxPipeChunks) == cudaSuccess;
     ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_status_arr), sizeof(DeviceStatus) * kMaxPipeChunks) == cudaSuccess;
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_offs_stage), sizeof(uint64_t) * (mp + 1 + kMaxPipeChunks)) == cudaSuccess;
+    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_offs_stage), sizeof(uint64_t) * lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
     {   // a pipelined host call gives earlier sub-batches the higher priority, so that they finish first and their downloads
         // run while the later ones compute (with equal priorities the sub-batches finished together and the downloads queued up
         // at the end: tools/pipe_trace.py)
@@ -1011,7 +980,7 @@ bool create_lane(Lane* ln, int device, uint64_t mb, uint64_t mp) {
              cudaEventCreateWithFlags(&ln->ev_chain[k], cudaEventDisableTiming) == cudaSuccess &&
              cudaEventCreateWithFlags(&ln->ev_scan[k], cudaEventDisableTiming) == cudaSuccess &&
              cudaEventCreateWithFlags(&ln->ev_list[k], cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaMemset(ln->d_bytes, 0, mb + 256 + 16 * (kMaxPipeChunks + 1)) == cudaSuccess;
+    ok = ok && cudaMemset(ln->d_bytes, 0, lane_bytes_alloc(mb, kMaxPipeChunks)) == cudaSuccess;
     for (int k = 0; ok && k < CFBPE_NUM_KERNELS; ++k)
         ok = cudaEventCreate(&ln->prof.ev[k][0]) == cudaSuccess && cudaEventCreate(&ln->prof.ev[k][1]) == cudaSuccess;
     for (int k = 0; ok && k < 2; ++k)
@@ -1076,16 +1045,27 @@ bool load_nccl(NcclApi* n) {
     return n->CommInitAll && n->CommDestroy && n->GroupStart && n->GroupEnd && n->Broadcast && n->AllGather && n->GetErrorString;
 }
 
-// shared body of encode_batch_device / encode_batch_starts_device: d_out_starts (nullable) gets the starts, beside d_out_ids
-int run_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
-               const uint8_t* d_vocab_ids, uint32_t* d_out_ids, uint32_t* d_out_starts, uint64_t out_cap, uint64_t* d_out_offsets,
-               uint32_t* d_out_counts, uint64_t* n_tokens, void* stream) {
+// what the lane's last device-path call reports, once its status is in h_status: the status, then ENOSPC against its out_cap
+int device_call_status(cfbpe_ctx* ctx, const Lane* ln) {
+    const DeviceStatus& st = *ln->h_status;
+    if (const int rc = fail_status(ctx, st)) return rc;
+    if (ln->dev_want_ids && st.n_tokens > ln->dev_out_cap) return fail_nospace(ctx, st.n_tokens);
+    return CFBPE_OK;
+}
+
+// The shape of a device-path call (the caller's device buffers, the caller's stream): the checks; the device of the buffers (the
+// first of the context whose ordinal is current, else the first) and a lane of it; the stream ordered after the lane's previous
+// device-path call; then enqueue(dv, ln, b, s, prof) queues the work (prof: profiling, when `profiled` and the context profiles).
+// The lane's workspace stays busy until that has run (ev_ws).  With n_tokens or profiling the call waits and reports the status.
+template <typename F>
+int device_call(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                const uint8_t* d_vocab_ids, const uint64_t* d_out_offsets, bool want_ids, uint64_t out_cap, uint64_t* n_tokens, void* stream,
+                bool profiled, F&& enqueue) {
     std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
     if (n_prompts > ctx->max_prompts || total_bytes > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds the limits of this context");
     if (!d_offsets || !d_out_offsets || (total_bytes && !d_bytes)) return fail(ctx, CFBPE_EINVAL, "device pointer is NULL");
     if (!ctx->vocabs[0].loaded && !d_vocab_ids) return fail(ctx, CFBPE_ENOENT, "vocab 0 is not loaded");
     if (!ctx->loaded_mask) return fail(ctx, CFBPE_ENOENT, "no vocabulary is loaded");
-    // the buffers live on ONE device: the first of the context whose ordinal is current, else the first
     DeviceCtx* dv = ctx->devs[0].get();
     { int cur = -1; if (cudaGetDevice(&cur) == cudaSuccess) for (auto& d : ctx->devs) if (d->device == cur) dv = d.get(); }
     LaneLock lk(dv);
@@ -1095,32 +1075,53 @@ int run_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint6
     // a lane is one workspace: a call on another stream waits (on the device) for the lane's previous device-path call;
     // consecutive calls take different lanes when the context has several (n_workspaces) and then overlap
     if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws, 0));
-    const bool profiling = ctx->profiling.load();
-    ProfEvents* prof = profiling ? &ln->prof : nullptr;
+    ProfEvents* prof = profiled && ctx->profiling.load() ? &ln->prof : nullptr;
     if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); cudaEventRecord(prof->h2d[1], s); }
-    BatchView b{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes};
-    enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts,
-                   static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, d_out_starts);   // profiling: one stream, so that the per-kernel times do not overlap
-    CK(cudaGetLastError());
+    const int rc = enqueue(dv, ln, BatchView{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes}, s, prof);
+    if (rc) return rc;
     CK(cudaEventRecord(ln->ev_ws, s));
     ln->ws_pending = true;
     ln->dev_out_cap = out_cap;
-    ln->dev_want_ids = d_out_ids != nullptr;
+    ln->dev_want_ids = want_ids;
     tl_device_lane = ln;
     if (prof) { cudaEventRecord(prof->d2h[0], s); cudaEventRecord(prof->d2h[1], s); cudaEventRecord(prof->total[1], s); }
-    if (n_tokens || prof) {
-        CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        if (prof) fill_profile(ln, total_bytes);
-        const DeviceStatus st = *ln->h_status;
-        if (n_tokens) *n_tokens = st.n_tokens;
-        if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
-        if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
-        if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
-        if (d_out_ids && st.n_tokens > out_cap) return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(st.n_tokens) + " ids");
-    }
-    return CFBPE_OK;
+    if (!n_tokens && !prof) return CFBPE_OK;
+    CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (prof) fill_profile(ln, total_bytes);
+    if (n_tokens) *n_tokens = ln->h_status->n_tokens;
+    return device_call_status(ctx, ln);
+}
+
+// shared body of encode_batch_device / encode_batch_starts_device: d_out_starts (nullable) gets the starts, beside d_out_ids
+int run_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+               const uint8_t* d_vocab_ids, uint32_t* d_out_ids, uint32_t* d_out_starts, uint64_t out_cap, uint64_t* d_out_offsets,
+               uint32_t* d_out_counts, uint64_t* n_tokens, void* stream) {
+    return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_offsets, d_out_ids != nullptr, out_cap, n_tokens, stream, true,
+                       [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents* prof) {
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts,
+                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
+                       ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, d_out_starts);   // profiling: one stream, so that the per-kernel times do not overlap
+        CK(cudaGetLastError());
+        return CFBPE_OK;
+    });
+}
+
+// shared body of encode_batch_special_device
+int run_device_special(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                       const uint8_t* d_vocab_ids, const uint8_t* const* modes, uint32_t* d_out_ids, uint64_t out_cap, uint64_t* d_out_offsets,
+                       uint32_t* d_out_counts, uint64_t* n_tokens, uint32_t* out_bad, void* stream) {
+    return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_offsets, d_out_ids != nullptr, out_cap, n_tokens, stream, false,
+                       [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents*) {
+        SpecialSet sp;
+        bool scan = false, spliced = false;
+        const EncodeOut out{d_out_ids, out_cap, d_out_offsets, d_out_counts};
+        int rc = special_set(ctx, dv, ln, modes, &sp, &scan, s);
+        if (!rc) rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, out, out, out_bad, &spliced);
+        // the lane's status carries the call's id count (cfbpe_device_status checks it against out_cap): n_tokens and tok_end
+        if (!rc && spliced) CK(cudaMemcpyAsync(&ln->ws.status->n_tokens, &ln->sp.status->fin.n_tokens, 2 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+        return rc;
+    });
 }
 
 }  // namespace
@@ -1324,7 +1325,8 @@ int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, con
     LaneLock lk(dv);
     Lane* ln = lk.ln;
     CK(cudaSetDevice(dv->device));
-    if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }
+    const int rc = wait_for_device_call(ctx, ln);
+    if (rc) return rc;
     cudaStream_t s = ln->stream;
     if (n_ids) CK(cudaMemcpyAsync(ln->d_out_ids, ids, n_ids * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(ln->d_offsets, id_offsets, (static_cast<uint64_t>(n_seqs) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
@@ -1425,70 +1427,8 @@ int cfbpe_encode_batch_special_device(cfbpe_ctx* ctx, uint32_t n_prompts, const 
     DeviceGuard restore_device;
     if (!ctx) return CFBPE_EINVAL;
     tl_err.clear();
-    std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
-    if (n_prompts > ctx->max_prompts || total_bytes > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds the limits of this context");
-    if (!d_offsets || !d_out_offsets || (total_bytes && !d_bytes)) return fail(ctx, CFBPE_EINVAL, "device pointer is NULL");
-    if (!ctx->vocabs[0].loaded && !d_vocab_ids) return fail(ctx, CFBPE_ENOENT, "vocab 0 is not loaded");
-    if (!ctx->loaded_mask) return fail(ctx, CFBPE_ENOENT, "no vocabulary is loaded");
-    DeviceCtx* dv = ctx->devs[0].get();
-    { int cur = -1; if (cudaGetDevice(&cur) == cudaSuccess) for (auto& d : ctx->devs) if (d->device == cur) dv = d.get(); }
-    LaneLock lk(dv);
-    Lane* ln = lk.ln;
-    CK(cudaSetDevice(dv->device));
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws, 0));
-    int rc = ensure_special_lane(ctx, ln);
-    if (rc) return rc;
-    SpecialSet sp;
-    bool scan = false;
-    rc = special_set(ctx, dv, ln, modes, &sp, &scan, s);
-    if (rc) return rc;
-    const BatchView b{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes};
-    const SpecialWork sw = special_work(ln);
-    uint64_t n_str = n_prompts;
-    if (scan) {       // the one synchronisation of the call: the host needs the number of stretches for the launch geometry
-        enqueue_special_scan(b, sp, ln->ws, sw, s);
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        ln->ws_pending = false;
-        const SpecialStatus ss = *ln->sp.h_status;
-        if (ss.bad_inv) {
-            const unsigned long long key = ~ss.bad_inv;
-            return fail_disallowed(ctx, ss.bad_prompt, static_cast<uint32_t>((key >> 12) & 7u), static_cast<uint32_t>(key & 0xFFFu), out_bad);
-        }
-        n_str = n_prompts + 2 * ss.kept.n_tokens;
-        if (n_str > ctx->max_prompts)
-            return fail(ctx, CFBPE_EINVAL, "n_prompts + 2 x special-token matches (" + std::to_string(n_str) + ") exceeds max_prompts of this context");
-    }
-    const uint32_t grid = static_cast<uint32_t>(dv->sm_count * 4);
-    if (n_str == n_prompts) {
-        enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts, grid, s, ln->aux_stream, ln->aux2_stream,
-                       ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
-    } else {
-        enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets,
-                               ln->d_out_counts, d_out_ids, out_cap, d_out_offsets, d_out_counts, grid, s, ln->aux_stream, ln->aux2_stream,
-                               ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
-        // the lane's status carries the call's id count (cfbpe_device_status checks it against out_cap): n_tokens and tok_end
-        CK(cudaMemcpyAsync(&ln->ws.status->n_tokens, &ln->sp.status->fin.n_tokens, 2 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
-    }
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(ln->ev_ws, s));
-    ln->ws_pending = true;
-    ln->dev_out_cap = out_cap;
-    ln->dev_want_ids = d_out_ids != nullptr;
-    tl_device_lane = ln;
-    if (n_tokens) {
-        CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        const DeviceStatus st = *ln->h_status;
-        *n_tokens = st.n_tokens;
-        if (st.long_overflow || st.miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
-        if (st.bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
-        if (st.bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
-        if (d_out_ids && st.n_tokens > out_cap) return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(st.n_tokens) + " ids");
-    }
-    return CFBPE_OK;
+    return run_device_special(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, modes, d_out_ids, out_cap, d_out_offsets, d_out_counts,
+                              n_tokens, out_bad, stream);
 }
 
 int cfbpe_device_status(cfbpe_ctx* ctx, void* stream) {
@@ -1501,12 +1441,7 @@ int cfbpe_device_status(cfbpe_ctx* ctx, void* stream) {
     CK(cudaSetDevice(ln->device));
     CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    if (ln->h_status->long_overflow || ln->h_status->miss_overflow) return fail(ctx, CFBPE_EIO, "internal: long-piece list overflow");
-    if (ln->h_status->bad_vocab) return fail(ctx, CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded");
-    if (ln->h_status->bad_utf8) return fail(ctx, CFBPE_EILSEQ, "a prompt holds malformed UTF-8");
-    if (ln->dev_want_ids && ln->h_status->n_tokens > ln->dev_out_cap)
-        return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(ln->h_status->n_tokens) + " ids");
-    return CFBPE_OK;
+    return device_call_status(ctx, ln);
 }
 
 void* cfbpe_host_alloc(cfbpe_ctx* ctx, size_t size) {

@@ -8,6 +8,7 @@
 //   CFBPE_MARK(prof, idx, stream, begin)             optional per-kernel event record
 //   CFBPE_FORK(main, aux, ev) / CFBPE_JOIN(main, aux, ev)   make aux wait for main / main wait for aux
 #pragma once
+#include "../../include/cfbpe.h"
 #include "bpe_kernels.cuh"
 
 namespace cfbpe {
@@ -30,19 +31,99 @@ struct Workspace {
     uint32_t* block_prompt; // the prompt that holds the first byte of every 512-byte block           [total / 512 + 2]
 };
 
-// the slice of the miss lists that belongs to a sub-batch of `len` bytes starting at byte o0 (k-th sub-batch)
-inline MissLists slice_miss(const MissLists& all, uint64_t o0, uint64_t len, uint32_t k) {
-    MissLists m;
-    for (uint32_t c = 0; c < 3; ++c) {     // (entries are 64-bit: position | rank << 32)
-        const uint32_t L = miss_class_min_len(c) < 2 ? 2u : miss_class_min_len(c);   // no one-byte piece is ever a miss
-        m.list[c] = all.list[c] + o0 / L + 2ull * k;
-        m.cap[c] = static_cast<uint32_t>(len / L + 2);
+// ---------------------------------------------------------------------------------------
+// The workspace layout.  Every sized buffer of a Workspace follows one rule of the byte count: a pass over `len` bytes touches
+// extent = len / unit (rounded up or down) + add elements of it.  A pipelined host call runs its sub-batches side by side in
+// one lane's workspace: sub-batch k (first byte o0) starts at o0 / unit + per_k * k, which leaves room for the extent of every
+// sub-batch before it, and the lane allocates the extent of max_bytes + per_k per sub-batch + spare.
+// ---------------------------------------------------------------------------------------
+enum WsKind : uint32_t {
+    kWsFlagWords,     // piece_bits, tok_bits, pstart_bits: a bit per byte
+    kWsPerByte,       // ids_by_pos, lscratch.*, dense.by_piece, dense.extras: at most one piece, token or part per byte
+    kWsLongList,      // a long piece holds more than 32 bytes
+    kWsScanTiles,     // tile_counts, tile_base: a K3 tile per 8 KiB
+    kWsMiss0, kWsMiss1, kWsMiss2,   // miss lists: class c holds pieces of >= 13 | 7 | 2 bytes (no one-byte piece is ever a miss)
+    kWsFixList,       // K1 walkers that stopped undecided: at most one per 16-byte block
+    kWsPieceTiles,    // dense.tile_pieces, dense.piece_base: a piece tile per 2 KiB
+    kWsBlockPrompt,   // a prompt per 512-byte block
+    kWsKinds
+};
+struct WsRule { uint32_t unit; bool round_up; uint32_t add, per_k, spare; };
+constexpr WsRule kWsRules[kWsKinds] = {
+    {32, true, 2, 4, 2}, {1, false, 0, 0, 1}, {32, false, 1, 1, 0}, {kScanTileWords * 32, true, 1, 2, 0},
+    {13, false, 2, 2, 62}, {7, false, 2, 2, 62}, {2, false, 2, 2, 62},
+    {16, false, 2, 2, 0}, {kPieceTileBytes, false, 2, 2, 0}, {1u << kPromptBlockShift, false, 2, 2, 0},
+};
+
+// element counts, one per kind
+struct WsSizes { uint64_t n[kWsKinds]; };
+
+// what one pass over len bytes may touch: a one-shot call on its own buffers needs exactly this
+inline WsSizes workspace_extent(uint64_t len) {
+    WsSizes s;
+    for (uint32_t i = 0; i < kWsKinds; ++i) {
+        const WsRule& r = kWsRules[i];
+        s.n[i] = (r.round_up ? (len + r.unit - 1) / r.unit : len / r.unit) + r.add;
     }
-    return m;
+    return s;
 }
+// what a lane allocates: room for up to max_chunks sub-batches of a pipelined call over max_bytes
+inline WsSizes workspace_alloc(uint64_t max_bytes, uint32_t max_chunks) {
+    WsSizes s = workspace_extent(max_bytes);
+    for (uint32_t i = 0; i < kWsKinds; ++i) s.n[i] += static_cast<uint64_t>(kWsRules[i].per_k) * max_chunks + kWsRules[i].spare;
+    return s;
+}
+
+// the 64-bit entries of miss list c in a workspace with room for max_chunks sub-batches of max_bytes (a hand-built workspace,
+// such as the emulator harnesses', sizes its miss lists with it)
 inline uint64_t miss_list_words(uint64_t max_bytes, uint32_t c, uint32_t max_chunks) {
-    const uint32_t L = miss_class_min_len(c) < 2 ? 2u : miss_class_min_len(c);
-    return max_bytes / L + 2ull * max_chunks + 64;
+    return workspace_alloc(max_bytes, max_chunks).n[kWsMiss0 + c];
+}
+
+// every sized buffer of w with its kind: f(pointer&, kind).  One list for allocation, release, slicing and the emulator.
+template <typename F>
+inline void for_each_ws_buffer(Workspace& w, F&& f) {
+    f(w.piece_bits, kWsFlagWords); f(w.tok_bits, kWsFlagWords); f(w.pstart_bits, kWsFlagWords);
+    f(w.ids_by_pos, kWsPerByte); f(w.lscratch.rank, kWsPerByte); f(w.lscratch.aux0, kWsPerByte); f(w.lscratch.aux1, kWsPerByte);
+    f(w.dense.by_piece, kWsPerByte); f(w.dense.extras, kWsPerByte);
+    f(w.long_list, kWsLongList);
+    f(w.tile_counts, kWsScanTiles); f(w.tile_base, kWsScanTiles);
+    f(w.miss.list[0], kWsMiss0); f(w.miss.list[1], kWsMiss1); f(w.miss.list[2], kWsMiss2);
+    f(w.fix_list, kWsFixList);
+    f(w.dense.tile_pieces, kWsPieceTiles); f(w.dense.piece_base, kWsPieceTiles);
+    f(w.block_prompt, kWsBlockPrompt);
+}
+
+// the capacities the kernels check, for buffers of the given sizes
+inline void set_workspace_caps(Workspace& w, const WsSizes& s) {
+    w.long_cap = static_cast<uint32_t>(s.n[kWsLongList]);
+    w.fix_cap = static_cast<uint32_t>(s.n[kWsFixList]);
+    w.dense.extras_cap = static_cast<uint32_t>(s.n[kWsPerByte]);
+    for (uint32_t c = 0; c < 3; ++c) w.miss.cap[c] = static_cast<uint32_t>(s.n[kWsMiss0 + c]);
+}
+
+// sub-batch k's view of a lane's workspace `all`: the sub-batch holds len bytes from byte o0 of the call (status: set by the caller)
+inline Workspace slice_workspace(const Workspace& all, uint64_t o0, uint64_t len, uint32_t k) {
+    Workspace w = all;
+    for_each_ws_buffer(w, [&](auto*& p, WsKind kind) { p += o0 / kWsRules[kind].unit + static_cast<uint64_t>(kWsRules[kind].per_k) * k; });
+    set_workspace_caps(w, workspace_extent(len));
+    return w;
+}
+
+// The lane's inputs and outputs of a pipelined host call.  Sub-batch k's bytes start on a 16-byte boundary (K1 reads 16 bytes a
+// lane with one load; the allocation leaves >= 16 bytes of readable padding after the last); its n_k + 1 offsets start at p0 + k.
+inline uint64_t sub_batch_bytes_at(uint64_t o0, uint32_t k) { return ((o0 + 15) & ~15ull) + 16ull * k; }
+inline uint64_t lane_bytes_alloc(uint64_t max_bytes, uint32_t max_chunks) { return max_bytes + 256 + 16ull * (max_chunks + 1); }
+inline uint64_t sub_batch_offsets_at(uint32_t p0, uint32_t k) { return static_cast<uint64_t>(p0) + k; }
+inline uint64_t lane_offsets_alloc(uint64_t max_prompts, uint32_t max_chunks) { return max_prompts + 1 + max_chunks; }
+
+// the error a pass's status reports (overflow before vocabulary before UTF-8), or code CFBPE_OK
+struct StatusError { int code; const char* msg; };
+inline StatusError status_error(const DeviceStatus& st) {
+    if (st.long_overflow || st.miss_overflow) return {CFBPE_EIO, "internal: long-piece list overflow"};
+    if (st.bad_vocab) return {CFBPE_ENOENT, "a prompt names a vocabulary that is not loaded"};
+    if (st.bad_utf8) return {CFBPE_EILSEQ, "a prompt holds malformed UTF-8"};
+    return {CFBPE_OK, nullptr};
 }
 
 // K2b CTAs per SM (long_grid = 4 x SM count).  8 x 128 threads x 64 registers is the whole register file of an SM: the

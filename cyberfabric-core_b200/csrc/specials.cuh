@@ -30,6 +30,24 @@ struct SpecialStatus {
     DeviceStatus fin;             // tile_scan of the stretch counts: fin.n_tokens = ids of the call
 };
 
+// What the host learns from a special scan: the disallowed occurrence that fails the call (prompt, vocabulary, special index),
+// else the number of stretches of the ordinary pass, which must fit in max_prompts.
+struct SpecialScanResult { bool disallowed; uint32_t prompt, vocab, index; uint64_t n_stretches; bool fits; };
+inline SpecialScanResult special_scan_result(const SpecialStatus& ss, uint32_t n_prompts, uint64_t max_prompts) {
+    SpecialScanResult r{};
+    if (ss.bad_inv) {
+        const unsigned long long key = ~ss.bad_inv;
+        r.disallowed = true;
+        r.prompt = ss.bad_prompt;
+        r.vocab = static_cast<uint32_t>((key >> 12) & 7u);
+        r.index = static_cast<uint32_t>(key & 0xFFFu);
+        return r;
+    }
+    r.n_stretches = n_prompts + 2 * ss.kept.n_tokens;
+    r.fits = r.n_stretches <= max_prompts;
+    return r;
+}
+
 // the buffers of a special call beside the workspace (the candidate marks live in the workspace's tok_bits / ids_by_pos: they
 // are dead until the ordinary pass starts)
 struct SpecialWork {

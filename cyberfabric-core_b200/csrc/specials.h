@@ -85,6 +85,34 @@ inline SpecialView make_special_view(const uint32_t* dev_words, const std::vecto
     return v;
 }
 
+// The special set of one call.  words[v]: vocabulary v's table (nullptr: none registered), views[v]: the view the kernels read;
+// modes[v]: the call's mode bytes for v (modes or modes[v] NULL: every special DISALLOWED).  A vocabulary whose modes are all
+// ordinary is left out; out->modes[v] is the caller's pointer.  *scan = false: no vocabulary looks for any special.  Returns 0,
+// or CFBPE_EINVAL (-22) with bad = {v, k} for a mode byte that is not a SpecialMode.
+inline int fill_special_set(const uint32_t* const* words, const SpecialView* views, const uint8_t* const* modes, SpecialSet* out,
+                            bool* scan, uint32_t bad[2]) {
+    *out = SpecialSet{};
+    *scan = false;
+    for (uint32_t v = 0; v < 8; ++v) {
+        const uint32_t* w = words[v];
+        if (!w) continue;
+        const uint8_t* m = modes ? modes[v] : nullptr;
+        if (m) {
+            bool looks = false;
+            for (uint32_t k = 0; k < w[0]; ++k) {
+                if (m[k] > kSpDisallow) { bad[0] = v; bad[1] = k; return -22; }
+                looks = looks || m[k] != kSpOrdinary;
+            }
+            if (!looks) continue;
+        }
+        out->v[v] = views[v];
+        out->modes[v] = m;
+        for (uint32_t j = 0; j < 8; ++j) out->first_bytes[j] |= w[kSpHeaderWords + j];
+        *scan = true;
+    }
+    return 0;
+}
+
 // strict UTF-8 (no overlong forms, no surrogates, nothing above U+10FFFF): what a Python str encodes to
 inline bool sp_valid_utf8(const uint8_t* p, uint64_t n) {
     for (uint64_t i = 0; i < n;) {

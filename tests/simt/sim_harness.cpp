@@ -11,7 +11,9 @@
 #define CFBPE_FORK(main, aux, ev) ((void)0)
 #define CFBPE_JOIN(main, aux, ev) ((void)0)
 
+#include <algorithm>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../cyberfabric-core_b200/csrc/pipeline.cuh"
@@ -36,6 +38,27 @@ static UcTables uc_tables() {
     if (!init) { build_pretok_tables(fsm); build_ascii_classes(ascii); build_split_tables(&st); init = true; }
     return UcTables{cfbpe_uc_stage1, cfbpe_uc_stage2, ascii, fsm, st.cls256, st.fsm16, st.ctx16, st.prod, st.prod_info, st.prod_skip, st.prod_start};
 }
+
+// The workspace of one pass over `total` bytes on host memory: workspace_extent(total) elements of every buffer, as a one-shot
+// call needs.  ids_by_pos, by_piece and extras start as 0xDEADBEEF (a slot the kernels never wrote shows), the rest as zero.
+struct SimWorkspace {
+    std::vector<std::vector<uint64_t>> store;
+    DeviceStatus st{};
+    Workspace w{};
+    explicit SimWorkspace(uint64_t total) {
+        const WsSizes s = workspace_extent(total);
+        for_each_ws_buffer(w, [&](auto*& p, WsKind kind) {
+            store.emplace_back((s.n[kind] * sizeof(*p) + 7) / 8);
+            p = reinterpret_cast<std::remove_reference_t<decltype(*p)>*>(store.back().data());
+        });
+        set_workspace_caps(w, s);
+        w.status = &st;
+        for (uint32_t* p : {w.ids_by_pos, w.dense.by_piece, w.dense.extras}) std::fill_n(p, s.n[kWsPerByte], 0xDEADBEEFu);
+    }
+    SimWorkspace(const SimWorkspace&) = delete;
+    SimWorkspace& operator=(const SimWorkspace&) = delete;
+};
+
 extern "C" __attribute__((visibility("default"))) uint32_t sim_ctx_count(uint32_t cased) { static SplitTablesHost st; build_split_tables(&st); return st.n_ctx[cased & 1]; }
 extern "C" __attribute__((visibility("default"))) uint32_t sim_prod_count(uint32_t pat) { static SplitTablesHost st; build_split_tables(&st); return st.n_prod[pat & 3]; }
 
@@ -146,36 +169,44 @@ __attribute__((visibility("default"))) int sim_encode_batch(void* const* vocabs,
         SimVocab* v = static_cast<SimVocab*>(vocabs[i]);
         vs.v[i] = make_view(v->blob.data(), v->hdr);
     }
-    const uint64_t nw = n_flag_words(total);
-    const uint32_t nt = n_scan_tiles(total);
-    std::vector<uint32_t> piece_bits(nw + 2), tok_bits(nw + 2), ids(total + 1, 0xDEADBEEF), rk(total + 1), nx(total + 1), pv(total + 1);
-    std::vector<uint32_t> tile_counts(nt + 1);
-    std::vector<uint64_t> tile_base(nt + 1);
-    std::vector<LongPiece> ll(total / 32 + 1);
-    DeviceStatus st{};
-    std::vector<SplitFix> fix(total / 16 + 2);
-    std::vector<uint64_t> miss[3];
-    MissLists ml;
-    for (uint32_t c = 0; c < 3; ++c) {
-        miss[c].resize(miss_list_words(total, c, 1));
-        ml.list[c] = miss[c].data();
-        ml.cap[c] = static_cast<uint32_t>(miss[c].size());
-    }
-    std::vector<uint32_t> pstart(nw + 2), bprompt((total >> kPromptBlockShift) + 2);
-    std::vector<uint32_t> by_piece(total + 1, 0xDEADBEEF), extras(total + 1, 0xDEADBEEF), tile_pieces((total >> 11) + 2);
-    std::vector<uint64_t> piece_base((total >> 11) + 2);
-    Workspace w{piece_bits.data(), tok_bits.data(), ids.data(), LongScratch{rk.data(), nx.data(), pv.data()},
-                ll.data(), static_cast<uint32_t>(ll.size()), tile_counts.data(), tile_base.data(), &st, ml, fix.data(), static_cast<uint32_t>(fix.size()),
-                DenseIds{by_piece.data(), extras.data(), static_cast<uint32_t>(extras.size()), tile_pieces.data(), piece_base.data()},
-                pstart.data(), bprompt.data()};
+    SimWorkspace ws(total);
     vs.loaded_mask = n_vocabs >= 32 ? 0xFFFFFFFFu : ((1u << n_vocabs) - 1u);
     int* prof = nullptr;
-    enqueue_encode(b, vs, uc_tables(), w, out_ids, out_cap, out_offsets, out_counts, 4u, 0, 0, 0, 0, 0, 0, prof);
-    if (n_long_out) *n_long_out = static_cast<uint64_t>(st.n_long) + st.n_big;
-    if (st.bad_utf8) return CFBPE_EILSEQ;
-    if (st.long_overflow || st.miss_overflow) return CFBPE_EIO;
-    if (out_ids && st.n_tokens > out_cap) return CFBPE_ENOSPC;
+    enqueue_encode(b, vs, uc_tables(), ws.w, out_ids, out_cap, out_offsets, out_counts, 4u, 0, 0, 0, 0, 0, 0, prof);
+    if (n_long_out) *n_long_out = static_cast<uint64_t>(ws.st.n_long) + ws.st.n_big;
+    if (const int rc = status_error(ws.st).code) return rc;
+    if (out_ids && ws.st.n_tokens > out_cap) return CFBPE_ENOSPC;
     return 0;
+}
+
+// Where a pipelined host call puts sub-batch k (len bytes from byte o0, prompts from p0) in a lane of max_bytes / max_prompts
+// that holds max_chunks sub-batches; per workspace buffer in for_each_ws_buffer's order: its kind, element size, the slice's
+// first element and the lane's allocation
+struct SimLayout {
+    uint64_t n_buffers;
+    uint64_t kind[32], elem[32], start[32], alloc[32];
+    uint64_t extent[kWsKinds];             // workspace_extent(len)
+    uint64_t long_cap, fix_cap, extras_cap, miss_cap[3];   // the slice's caps
+    uint64_t bytes_at, bytes_alloc, offsets_at, offsets_alloc;
+};
+__attribute__((visibility("default"))) void sim_workspace_layout(uint64_t o0, uint64_t len, uint32_t k, uint32_t p0, uint64_t max_bytes,
+                                                                 uint64_t max_prompts, uint32_t max_chunks, SimLayout* out) {
+    Workspace base{};
+    for_each_ws_buffer(base, [](auto*& p, WsKind) { p = reinterpret_cast<std::remove_reference_t<decltype(*p)>*>(uintptr_t(1) << 40); });
+    Workspace sl = slice_workspace(base, o0, len, k);
+    const WsSizes ext = workspace_extent(len), all = workspace_alloc(max_bytes, max_chunks);
+    uintptr_t b0[32], s0[32];
+    uint64_t n = 0;
+    for_each_ws_buffer(base, [&](auto*& p, WsKind kind) { b0[n] = reinterpret_cast<uintptr_t>(p); out->kind[n] = kind; out->elem[n] = sizeof(*p); out->alloc[n] = all.n[kind]; ++n; });
+    n = 0;
+    for_each_ws_buffer(sl, [&](auto*& p, WsKind) { s0[n++] = reinterpret_cast<uintptr_t>(p); });
+    out->n_buffers = n;
+    for (uint64_t i = 0; i < n; ++i) out->start[i] = (s0[i] - b0[i]) / out->elem[i];
+    for (uint32_t i = 0; i < kWsKinds; ++i) out->extent[i] = ext.n[i];
+    out->long_cap = sl.long_cap; out->fix_cap = sl.fix_cap; out->extras_cap = sl.dense.extras_cap;
+    for (uint32_t c = 0; c < 3; ++c) out->miss_cap[c] = sl.miss.cap[c];
+    out->bytes_at = sub_batch_bytes_at(o0, k); out->bytes_alloc = lane_bytes_alloc(max_bytes, max_chunks);
+    out->offsets_at = sub_batch_offsets_at(p0, k); out->offsets_alloc = lane_offsets_alloc(max_prompts, max_chunks);
 }
 
 // the sub-batch plan of a pipelined host call (host code of the product, csrc/subbatch.h)

@@ -40,6 +40,8 @@ def lib():
         L.sim_validate_blob.argtypes = [C.c_void_p, C.c_uint64, C.c_char_p, C.c_size_t]
         L.sim_dbg_counter.restype = C.c_ulonglong
         L.sim_dbg_counter.argtypes = [C.c_uint32, C.c_int]
+        L.sim_workspace_layout.restype = None
+        L.sim_workspace_layout.argtypes = [C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p]
         _lib = L
     return _lib
 
@@ -152,6 +154,32 @@ def decode_batch(vocabs, ids, id_offsets, vocab_ids=None, out_cap=None):
     rc = lib().sim_decode_batch(vh, len(vocabs), n, ids.ctypes.data, id_offsets.ctypes.data,
                                 None if vid is None else vid.ctypes.data, out.ctypes.data, cap, out_off.ctypes.data)
     return rc, out[:int(out_off[n])] if rc == 0 else out[:0], out_off
+
+
+WS_KINDS = ["flag_words", "per_byte", "long_list", "scan_tiles", "miss0", "miss1", "miss2", "fix_list", "piece_tiles", "block_prompt"]
+WS_BUFFERS = ["piece_bits", "tok_bits", "pstart_bits", "ids_by_pos", "lscratch.rank", "lscratch.aux0", "lscratch.aux1", "dense.by_piece",
+              "dense.extras", "long_list", "tile_counts", "tile_base", "miss.list[0]", "miss.list[1]", "miss.list[2]", "fix_list",
+              "dense.tile_pieces", "dense.piece_base", "block_prompt"]
+
+
+class _Layout(C.Structure):
+    _fields_ = [("n_buffers", C.c_uint64), ("kind", C.c_uint64 * 32), ("elem", C.c_uint64 * 32), ("start", C.c_uint64 * 32),
+                ("alloc", C.c_uint64 * 32), ("extent", C.c_uint64 * len(WS_KINDS)), ("long_cap", C.c_uint64), ("fix_cap", C.c_uint64),
+                ("extras_cap", C.c_uint64), ("miss_cap", C.c_uint64 * 3), ("bytes_at", C.c_uint64), ("bytes_alloc", C.c_uint64),
+                ("offsets_at", C.c_uint64), ("offsets_alloc", C.c_uint64)]
+
+
+def workspace_layout(o0, length, k, p0, max_bytes, max_prompts, max_chunks=64):
+    """csrc/pipeline.cuh: where a pipelined call puts sub-batch k (length bytes from byte o0, prompts from p0) in a lane.
+    buffers: {name: (kind, element bytes, first element, lane allocation)}; extent: {kind: workspace_extent(length)}"""
+    r = _Layout()
+    lib().sim_workspace_layout(o0, length, k, p0, max_bytes, max_prompts, max_chunks, C.byref(r))
+    assert r.n_buffers == len(WS_BUFFERS)
+    return {"buffers": {name: (WS_KINDS[r.kind[i]], r.elem[i], r.start[i], r.alloc[i]) for i, name in enumerate(WS_BUFFERS)},
+            "extent": dict(zip(WS_KINDS, list(r.extent))),
+            "caps": {"long_list": r.long_cap, "fix_list": r.fix_cap, "per_byte": r.extras_cap,
+                     "miss0": r.miss_cap[0], "miss1": r.miss_cap[1], "miss2": r.miss_cap[2]},
+            "bytes_at": r.bytes_at, "bytes_alloc": r.bytes_alloc, "offsets_at": r.offsets_at, "offsets_alloc": r.offsets_alloc}
 
 
 def plan_sub_batches(offsets, chunk, max_chunks=64):
