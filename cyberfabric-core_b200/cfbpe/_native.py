@@ -12,6 +12,7 @@ SO_PATH = os.environ.get("CFBPE_SO_VARIANT") or os.path.join(_DIR, "libcfbpe.so"
 OK, ENOENT, EIO, ENOMEM, ENODEV, EINVAL, ENOSPC, EILSEQ, EBADMSG = 0, -2, -5, -12, -19, -22, -28, -84, -74
 SPECIAL_ORDINARY, SPECIAL_ALLOW, SPECIAL_DISALLOW = 0, 1, 2      # what an occurrence of a special token means in one call
 MAX_SPECIALS, MAX_SPECIAL_LEN = 4096, 64
+TRUNCATE_HEAD, TRUNCATE_TAIL = 0, 1      # keep the first / the last tokens of every prompt (cfbpe_truncate_batch)
 FORMAT_TIKTOKEN, FORMAT_TEKKEN_JSON = 0, 1
 PATTERN_CL100K, PATTERN_O200K, PATTERN_LLAMA3, PATTERN_TEKKEN = 0, 1, 2, 3
 PATTERN_IDS = {"cl100k": 0, "o200k": 1, "llama3": 2, "tekken": 3}
@@ -27,6 +28,7 @@ EXPORTS = [
     "cfbpe_profile_enable", "cfbpe_profile_read", "cfbpe_decode_batch",
     "cfbpe_vocab_set_specials", "cfbpe_encode_batch_special", "cfbpe_encode_batch_special_device",
     "cfbpe_encode_batch_starts", "cfbpe_encode_batch_starts_device",
+    "cfbpe_truncate_batch", "cfbpe_truncate_batch_device",
 ]
 
 
@@ -106,6 +108,10 @@ def load():
     L.cfbpe_encode_batch_starts_device.restype = C.c_int
     L.cfbpe_encode_batch_starts_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, C.c_uint64, vp, vp,
                                                    C.POINTER(C.c_uint64), vp]
+    L.cfbpe_truncate_batch.restype = C.c_int
+    L.cfbpe_truncate_batch.argtypes = [vp, C.c_uint32, u8p, vp, u8p, vp, C.c_uint32, vp, vp, vp]
+    L.cfbpe_truncate_batch_device.restype = C.c_int
+    L.cfbpe_truncate_batch_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
     L.cfbpe_vocab_set_specials.restype = C.c_int
     L.cfbpe_vocab_set_specials.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, vp, vp]
     L.cfbpe_encode_batch_special.restype = C.c_int
@@ -276,6 +282,36 @@ class Context:
         nt = int(out_offsets[n])
         return out_ids[:nt], out_starts[:nt], out_offsets, out_counts[:n]
 
+    @staticmethod
+    def budget_array(budgets, n):
+        """an int (every prompt) or one budget per prompt -> a C-contiguous uint32 array of max(n, 1) entries"""
+        if isinstance(budgets, (int, np.integer)):
+            if not 0 <= int(budgets) <= 0xFFFFFFFF:
+                raise NativeError(EINVAL, "a token budget must be in 0 .. 2^32 - 1")
+            return np.full(max(n, 1), int(budgets), dtype=np.uint32)
+        b = np.asarray(budgets)
+        if b.ndim != 1 or len(b) != n or (b.size and (b.dtype.kind not in "iu" or int(b.min()) < 0 or int(b.max()) > 0xFFFFFFFF)):
+            raise NativeError(EINVAL, "budgets must be one integer in 0 .. 2^32 - 1 per prompt")
+        return np.ascontiguousarray(b, dtype=np.uint32) if n else np.zeros(1, dtype=np.uint32)
+
+    def truncate_batch(self, data: np.ndarray, offsets: np.ndarray, budgets, mode=TRUNCATE_HEAD, vocab_ids=None, out_cut=None,
+                       out_kept=None, out_counts=None):
+        """cfbpe_truncate_batch: (cut, kept, counts), uint32 each, one entry per prompt.  budgets: an int or one per prompt.
+        TRUNCATE_HEAD keeps bytes[offsets[i] .. offsets[i] + cut[i]), TRUNCATE_TAIL keeps bytes[offsets[i] + cut[i] .. offsets[i + 1])."""
+        n = self._check_inputs(data, offsets, vocab_ids)
+        bud = self.budget_array(budgets, n)
+        outs = []
+        for a in (out_cut, out_kept, out_counts):
+            if a is None:
+                a = np.empty(max(n, 1), dtype=np.uint32)
+            elif not isinstance(a, np.ndarray) or a.dtype != np.uint32 or a.size < n or not a.flags.c_contiguous:
+                raise NativeError(EINVAL, "out_cut, out_kept and out_counts must be C-contiguous uint32 arrays with one entry per prompt")
+            outs.append(a)
+        vid = None if vocab_ids is None else vocab_ids.ctypes.data
+        self._check(load().cfbpe_truncate_batch(self._h, n, data.ctypes.data if data.size else None, offsets.ctypes.data, vid,
+                                                bud.ctypes.data, mode, outs[0].ctypes.data, outs[1].ctypes.data, outs[2].ctypes.data))
+        return outs[0][:n], outs[1][:n], outs[2][:n]
+
     def count_batch(self, data: np.ndarray, offsets: np.ndarray, vocab_ids=None, out_counts=None):
         n = self._check_inputs(data, offsets, vocab_ids)
         if out_counts is None:
@@ -326,6 +362,13 @@ class Context:
                                                      C.byref(nt) if sync else None, stream)
         self._check(rc)
         return nt.value if sync else None
+
+    def truncate_batch_device(self, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_budgets, mode, d_out_cut, d_out_kept,
+                              d_out_counts, stream=0):
+        """cfbpe_truncate_batch_device on raw device pointers (uint32 budgets, cuts, kept counts, counts: n_prompts each; counts
+        may be None).  Asynchronous: errors come from the next synchronising call or device_status."""
+        self._check(load().cfbpe_truncate_batch_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_budgets,
+                                                       mode, d_out_cut, d_out_kept, d_out_counts, stream))
 
     # ---- special tokens
     @staticmethod

@@ -110,6 +110,58 @@ class EncodeBatchResponse:
 
 
 @dataclass
+class TruncateBatchResponse:
+    """where each prompt is cut to its token budget (TokenizerPluginClient.truncate_batch), one entry per prompt"""
+    cut: np.ndarray              # uint32: byte position of the cut in the prompt; "head" keeps [0, cut), "tail" keeps [cut, len)
+    kept: np.ndarray             # uint32: tokens of the prompt's encoding wholly inside the kept text
+    counts: np.ndarray           # uint32: tokens of the whole prompt
+
+
+TRUNCATE_KEEP = {"head": N.TRUNCATE_HEAD, "tail": N.TRUNCATE_TAIL}
+
+
+def _truncate_mode(keep: str) -> int:
+    if keep not in TRUNCATE_KEEP:
+        raise InvalidInput("keep must be 'head' or 'tail', not %r" % (keep,))
+    return TRUNCATE_KEEP[keep]
+
+
+def _budgets(budgets, n: int) -> np.ndarray:
+    try:
+        return N.Context.budget_array(budgets, n)[:n]
+    except N.NativeError as e:
+        raise InvalidInput(str(e)) from e
+
+
+def truncate_cuts(data: np.ndarray, offsets: np.ndarray, id_offsets: np.ndarray, starts: np.ndarray, budgets: np.ndarray,
+                  tail: bool) -> Tuple[np.ndarray, np.ndarray]:
+    """The truncation contract (include/cfbpe.h, cfbpe_truncate_batch) from every token's start: (cut, kept), uint32 per prompt.
+    head: the first k = min(budget, c) tokens end at x; the cut is the character start at or before x.  tail: the last k tokens
+    start at x; the cut is the character start at or after x (or the end).  kept: the tokens wholly inside the kept text."""
+    n = len(offsets) - 1
+    cut = np.zeros(n, dtype=np.uint32)
+    kept = np.zeros(n, dtype=np.uint32)
+    for i in range(n):
+        o, ln = int(offsets[i]), int(offsets[i + 1]) - int(offsets[i])
+        st = starts[int(id_offsets[i]):int(id_offsets[i + 1])].astype(np.int64)
+        c = len(st)
+        k = min(int(budgets[i]), c)
+        j = c - k if tail else k
+        x = int(st[j]) if j < c else ln                 # the first byte of token j (the end of token j - 1)
+        if tail:
+            while x < ln and data[o + x] & 0xC0 == 0x80:
+                x += 1
+            kept[i] = c - int(np.searchsorted(st, x, side="left"))
+        else:
+            while 0 < x < ln and data[o + x] & 0xC0 == 0x80:
+                x -= 1
+            ends = np.append(st[1:], ln) if c else st
+            kept[i] = int(np.searchsorted(ends, x, side="right"))
+        cut[i] = x
+    return cut, kept
+
+
+@dataclass
 class CountTokensRequest:
     vocab: VocabRef
     bytes: np.ndarray
@@ -239,6 +291,20 @@ class TokenizerPluginClient:
         offsets[1:] = np.cumsum(counts, dtype=np.uint64)
         ids = np.concatenate(parts).astype(np.uint32) if parts else np.zeros(0, dtype=np.uint32)
         return EncodeBatchResponse(ids, offsets, counts)
+
+    def truncate_batch(self, ctx: SecurityContext, req: EncodeBatchRequest, budgets, keep: str = "head") -> TruncateBatchResponse:
+        """Cut every prompt of `req` to a token budget (an int, or one per prompt): keep its first ("head") or last ("tail")
+        min(budget, count) tokens of the encoding of the whole prompt, cut at a character boundary -- include/cfbpe.h,
+        cfbpe_truncate_batch.  This default works on any plugin: encode_batch with token starts, then the cut on the host."""
+        tail = _truncate_mode(keep) == N.TRUNCATE_TAIL
+        n = len(req.offsets) - 1
+        bud = _budgets(budgets, n)
+        r = self.encode_batch(ctx, EncodeBatchRequest(req.vocab, req.bytes, req.offsets, req.vocabs_per_prompt, req.vocab_index,
+                                                      with_starts=True))
+        if r.starts is None:
+            raise ServiceUnavailable("the tokenizer plugin does not return token starts")
+        cut, kept = truncate_cuts(req.bytes, req.offsets, r.offsets, r.starts, bud, tail)
+        return TruncateBatchResponse(cut, kept, np.asarray(r.counts[:n], dtype=np.uint32))
 
 
 GTS_PLUGIN_SCHEMA = "gts.x.core.modkit.plugin.v1~x.llmgw.tokenizer.plugin.v1~"
@@ -456,6 +522,19 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
             raise _map_native(e) from e
         return EncodeBatchResponse(ids, offs, counts)
 
+    def truncate_batch(self, ctx: SecurityContext, req: EncodeBatchRequest, budgets, keep: str = "head") -> TruncateBatchResponse:
+        """the device path (cfbpe_truncate_batch): the cut is computed where the ids are; only the cuts, kept counts and counts
+        come back"""
+        mode = _truncate_mode(keep)
+        self._check_arrays(req)
+        vid = self._vocab_ids(req)
+        bud = _budgets(budgets, len(req.offsets) - 1)
+        try:
+            cut, kept, counts = self.ctx.truncate_batch(req.bytes, req.offsets, bud, mode, vid)
+        except N.NativeError as e:
+            raise _map_native(e) from e
+        return TruncateBatchResponse(cut, kept, counts)
+
     def close(self):
         self.ctx.close()
 
@@ -512,6 +591,22 @@ class LlmGatewayTokenizerService:
             if b > a:
                 spans[-1, 1] = int(offs[i + 1]) - int(offs[i])
             out.append((r.ids[a:b], spans))
+        return out
+
+    def truncate(self, ctx: SecurityContext, model: str, texts: Sequence[str], max_tokens, keep: str = "head") -> List[Tuple[str, int, int]]:
+        """Fit texts into a context window: per text, (the kept text, its tokens, the tokens of the whole text).  max_tokens: one
+        budget for all texts or one per text; keep="head" keeps the first tokens (a long document, retrieved context), "tail" the
+        last ones (a chat history).  The cut is at a token boundary of the whole text's encoding, moved to a character boundary
+        so that the kept text is valid UTF-8 (its token count is then one to three less than the budget).  Encoding the kept text
+        again may give other tokens: BPE is not prefix-stable."""
+        data, offs = pack_texts(texts)
+        r = self._plugin().truncate_batch(ctx, EncodeBatchRequest(VocabRef(model), data, offs), max_tokens, keep)
+        tail = _truncate_mode(keep) == N.TRUNCATE_TAIL
+        out = []
+        for i in range(len(texts)):
+            b = data[int(offs[i]):int(offs[i + 1])].tobytes()
+            c = int(r.cut[i])
+            out.append(((b[c:] if tail else b[:c]).decode("utf-8"), int(r.kept[i]), int(r.counts[i])))
         return out
 
     def count_tokens(self, ctx: SecurityContext, model: str, messages: Sequence[dict]) -> Usage:

@@ -1735,6 +1735,120 @@ starts_emit_kernel(BatchView b, const uint64_t* __restrict__ out_offsets, uint64
     }
 }
 
+// Truncation (pipeline.cuh, enqueue_emit): where to cut prompt p so that it keeps the first (head) or the last (tail) k = min(budget, c)
+// of its c tokens, moved to a character boundary; kept = the tokens wholly inside the kept span.  The boundary is token j (head:
+// j = k, tail: j = c - k) and its byte position is the sum of the lengths of the tokens before it -- or the prompt's length minus
+// the sum from j on: whichever end of the prompt's contiguous id run is nearer, a sum over m = min(k, c - k) ids.  c <= budget
+// gives m = 0: no id is read.  Then the cut moves to a character start (at most 3 bytes: back for head, on for tail) and kept
+// drops the tokens the move cut through (at most 3: every token holds >= 1 byte).
+//   truncate:      a warp per prompt, sums the first kTruncPartIds ids of the range; a prompt with no more finishes here, a
+//                  longer one parks that sum in cut[p] (and 0 in kept[p])
+//   truncate_long: the other parts of the long prompts, a warp each.  Warp w takes the kTruncChunkBytes chunk of text that starts
+//                  at w x kTruncChunkBytes; the chunks that start inside prompt p take its parts 1, 2, ... (m <= c / 2 <= len / 2,
+//                  so a prompt has a chunk for every part after the first).  Each adds its sum into cut[p] and counts itself in
+//                  kept[p]; the last to arrive finishes.  A long prompt is spread over as many warps as it has parts.
+struct TruncateView {
+    const uint32_t* budgets;   // per prompt of the (sub-)batch
+    uint32_t tail;             // 1: keep the last tokens, 0: the first
+    uint32_t* cut;             // out: byte position of the cut within the prompt
+    uint32_t* kept;            // out: tokens wholly inside the kept span
+};
+constexpr uint32_t kTruncPartIds = 4096;
+constexpr uint32_t kTruncChunkBytes = 2 * kTruncPartIds;
+
+struct TruncPlan { uint32_t c, k, j, lo, m; bool front; };
+__device__ __forceinline__ TruncPlan truncate_plan(const uint64_t* __restrict__ out_offsets, const TruncateView& tv, uint32_t p) {
+    TruncPlan t;
+    t.c = static_cast<uint32_t>(out_offsets[p + 1] - out_offsets[p]);
+    const uint32_t budget = tv.budgets[p];
+    t.k = budget < t.c ? budget : t.c;
+    t.j = tv.tail ? t.c - t.k : t.k;
+    t.front = t.j <= t.c - t.j;                   // sum the ids before j, else those from j on
+    t.lo = t.front ? 0u : t.j;
+    t.m = t.front ? t.j : t.c - t.j;
+    return t;
+}
+__device__ __forceinline__ const TablesView& prompt_tables(const BatchView& b, const VocabSet& vs, uint32_t p) {
+    const uint32_t v = b.vocab_ids ? b.vocab_ids[p] : 0u;
+    return vs.v[v < kMaxVocabs ? v : 0u];        // (a bad id is reported by prompt_map_kernel; unloaded slots alias a loaded one)
+}
+__device__ __forceinline__ uint32_t token_bytes(const TablesView& T, uint32_t id) {
+    return id < T.n_ranks ? T.tokoff[id + 1] - T.tokoff[id] : 0u;   // (ids of a failed pass may be anything)
+}
+// byte length of ids[r .. r + n), the warp together: lane l reads ids r + l, r + l + 32, ... (coalesced), four loads in flight
+__device__ __forceinline__ uint32_t warp_token_bytes(const TablesView& T, const uint32_t* __restrict__ ids, uint64_t r, uint32_t n) {
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t s = 0;
+    for (uint32_t i0 = 0; i0 < n; i0 += 4 * 32) {
+        uint32_t id[4];
+#pragma unroll
+        for (uint32_t h = 0; h < 4; ++h) { const uint32_t i = i0 + 32 * h + lane; id[h] = i < n ? __ldg(ids + r + i) : 0xFFFFFFFFu; }
+#pragma unroll
+        for (uint32_t h = 0; h < 4; ++h) s += token_bytes(T, id[h]);
+    }
+    return __reduce_add_sync(kFull, s);
+}
+// one thread: the cut and the kept count of prompt p from `sum` (the byte length of the m ids from lo)
+__device__ void truncate_finish(const BatchView& b, const TablesView& T, const uint32_t* __restrict__ ids, uint64_t r0, const TruncPlan& t,
+                                const TruncateView& tv, uint32_t p, uint32_t sum) {
+    const uint64_t o = b.offsets[p];
+    const uint32_t len = static_cast<uint32_t>(b.offsets[p + 1] - o);
+    uint32_t x = t.front ? sum : len - (sum < len ? sum : len);   // the byte position of token j
+    if (x > len) x = len;
+    const uint8_t* s = b.bytes + o;
+    uint32_t cut = x, kept = t.k;
+    if (tv.tail) {
+        while (cut < len && (s[cut] & 0xC0u) == 0x80u) ++cut;      // the next character start, or the end
+        for (uint32_t r = t.j, e = x; e < cut && r < t.c && kept; ++r, --kept) e += token_bytes(T, ids[r0 + r]);
+    } else {
+        while (cut > 0 && cut < len && (s[cut] & 0xC0u) == 0x80u) --cut;   // the character start at or before x
+        for (uint32_t r = t.j, e = x; e > cut && r > 0 && kept; --kept) { --r; e -= token_bytes(T, ids[r0 + r]); }
+    }
+    tv.cut[p] = cut;
+    tv.kept[p] = kept;
+}
+
+__global__ void __launch_bounds__(256)
+truncate_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ ids, const uint64_t* __restrict__ out_offsets, TruncateView tv) {
+    const uint64_t p = (static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    if (p >= b.n_prompts) return;
+    const TruncPlan t = truncate_plan(out_offsets, tv, static_cast<uint32_t>(p));
+    const TablesView& T = prompt_tables(b, vs, static_cast<uint32_t>(p));
+    const uint64_t r0 = out_offsets[p];
+    const uint32_t sum = warp_token_bytes(T, ids, r0 + t.lo, t.m < kTruncPartIds ? t.m : kTruncPartIds);
+    if (threadIdx.x & 31) return;
+    if (t.m <= kTruncPartIds) {
+        truncate_finish(b, T, ids, r0, t, tv, static_cast<uint32_t>(p), sum);
+    } else {
+        tv.cut[p] = sum;
+        tv.kept[p] = 0;
+    }
+}
+
+__global__ void __launch_bounds__(256)
+truncate_long_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ ids, const uint64_t* __restrict__ out_offsets, TruncateView tv) {
+    const uint64_t w = (static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    const uint64_t pos = w * kTruncChunkBytes;
+    if (pos >= b.total_bytes) return;
+    const uint32_t p = find_prompt(b.offsets, b.n_prompts, pos);
+    const TruncPlan t = truncate_plan(out_offsets, tv, p);
+    if (t.m <= kTruncPartIds) return;
+    const uint32_t part = static_cast<uint32_t>(w - (b.offsets[p] + kTruncChunkBytes - 1) / kTruncChunkBytes) + 1;
+    const uint32_t parts = (t.m + kTruncPartIds - 1) / kTruncPartIds;
+    if (part >= parts) return;
+    const TablesView& T = prompt_tables(b, vs, p);
+    const uint64_t r0 = out_offsets[p];
+    const uint32_t i0 = part * kTruncPartIds;
+    const uint32_t sum = warp_token_bytes(T, ids, r0 + t.lo + i0, t.m - i0 < kTruncPartIds ? t.m - i0 : kTruncPartIds);
+    if (threadIdx.x & 31) return;
+    atomicAdd(&tv.cut[p], sum);
+    __threadfence();
+    if (atomicAdd(&tv.kept[p], 1u) + 2 == parts) {            // the last of parts 1 .. parts - 1: every sum is in
+        __threadfence();
+        truncate_finish(b, T, ids, r0, t, tv, p, atomicAdd(&tv.cut[p], 0u));
+    }
+}
+
 // ---------------------------------------------------------------------------------------
 // Decode (SURVEY.md section 8(f) item 2): ids -> bytes.  tiktoken's decode_bytes: the concatenation of the tokens' bytes.
 //   decode_len:    length of every token (0xFFFFFFFF + status->bad_utf8-style flag for an id outside the vocabulary),

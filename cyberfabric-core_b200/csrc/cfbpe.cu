@@ -132,6 +132,8 @@ struct Lane {
     uint64_t* d_out_offsets = nullptr;
     uint32_t* d_out_counts = nullptr;
     uint32_t* d_out_starts = nullptr;    // host calls with token starts: [max_bytes + 1], allocated on the lane's first such call
+    uint32_t* d_trunc = nullptr;         // host truncate calls: budgets, cuts, kept counts [3 x (max_prompts + 1)], allocated on the
+                                         // lane's first such call
     Workspace ws{};
     DeviceStatus* h_status = nullptr;  // pinned
     ProfEvents prof{};
@@ -356,6 +358,38 @@ int ensure_starts_lane(cfbpe_ctx* ctx, Lane* ln) {
     return CFBPE_OK;
 }
 
+// A host truncate call (cfbpe_truncate_batch): budgets in, cuts and kept counts out, one per prompt of the call.  The ids it needs go to
+// the lane's id buffer and are never downloaded.
+struct TruncateArgs { const uint32_t* budgets; uint32_t tail; uint32_t* cut; uint32_t* kept; };
+TruncateArgs truncate_from(const TruncateArgs& t, uint32_t p0) { return TruncateArgs{t.budgets + p0, t.tail, t.cut + p0, t.kept + p0}; }
+
+// the lane's truncate buffers (host truncate calls), allocated on its first such call: a context that never truncates keeps the
+// footprint it had.  The caller has selected the lane's device.
+int ensure_truncate_lane(cfbpe_ctx* ctx, Lane* ln) {
+    if (ln->d_trunc) return CFBPE_OK;
+    if (dmalloc(&ln->d_trunc, 3 * (static_cast<uint64_t>(ctx->max_prompts) + 1)) != cudaSuccess) {
+        cudaGetLastError(); ln->d_trunc = nullptr;
+        return fail(ctx, CFBPE_ENOMEM, "no device memory for the truncate buffers");
+    }
+    return CFBPE_OK;
+}
+// prompts p0 .. of the call in the lane's truncate buffers (a sub-batch's prompts keep their index in the call)
+TruncateView lane_truncate_view(cfbpe_ctx* ctx, Lane* ln, uint32_t tail, uint32_t p0) {
+    const uint64_t m = static_cast<uint64_t>(ctx->max_prompts) + 1;
+    return TruncateView{ln->d_trunc + p0, tail, ln->d_trunc + m + p0, ln->d_trunc + 2 * m + p0};
+}
+int upload_budgets(cfbpe_ctx* ctx, Lane* ln, const TruncateArgs& t, uint32_t p0, uint32_t n, cudaStream_t s) {
+    if (n) CK(cudaMemcpyAsync(ln->d_trunc + p0, t.budgets + p0, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    return CFBPE_OK;
+}
+int download_cuts(cfbpe_ctx* ctx, Lane* ln, const TruncateArgs& t, uint32_t p0, uint32_t n, cudaStream_t s) {
+    if (!n) return CFBPE_OK;
+    const TruncateView v = lane_truncate_view(ctx, ln, t.tail, p0);
+    CK(cudaMemcpyAsync(t.cut + p0, v.cut, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(t.kept + p0, v.kept, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    return CFBPE_OK;
+}
+
 // an asynchronous device-path call may still own the lane's workspace: wait for it (the caller has selected the lane's device)
 int wait_for_device_call(cfbpe_ctx* ctx, Lane* ln) {
     if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }
@@ -379,10 +413,11 @@ int upload_batch(cfbpe_ctx* ctx, Lane* ln, uint32_t n, const uint8_t* bytes, con
 // ids to fetch.
 // defer != nullptr (a shard of a multi-device call): nothing is downloaded here -- ids, offsets and counts stay in the lane's device
 // buffers (dense, shard-local ranks: sub-batch k's offsets at d_out_offsets + sub_batch_offsets_at(p_k, k)) and *defer gets the
-// shard's token total.
+// shard's token total.  trunc (nullable): a truncate call; its cuts and kept counts are final (per prompt, prompt-relative) and
+// are downloaded under `defer` too.
 int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, int G, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
                        const uint8_t* vocab_ids, uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
-                       bool want_ids, uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out) {
+                       bool want_ids, uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out, const TruncateArgs* trunc) {
     // ---- cut
     uint32_t cut[kMaxPipeChunks + 1];
     const int nc = plan_sub_batches(offsets, n, total, ctx->pipe_chunk, kMaxPipeChunks, cut);
@@ -421,6 +456,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (len && !no_copy) CK(cudaMemcpyAsync(d_sub, bytes + o0, len, cudaMemcpyHostToDevice, hs));
         CK(cudaMemcpyAsync(ln->d_offsets + q0, lns[0]->h_offs_stage + q0, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, hs));
         if (vocab_ids && nk) CK(cudaMemcpyAsync(ln->d_vocab_ids + p0, vocab_ids + p0, nk, cudaMemcpyHostToDevice, hs));
+        if (trunc) { const int rc = upload_budgets(ctx, ln, *trunc, p0, nk, hs); if (rc) return rc; }
         CK(cudaEventRecord(ln->ev_h2d[k], hs));
         if (trace) CK(cudaEventRecord(ln->trace[k][0], hs));
         const int fk = k < kFrontStreams ? k : kFrontStreams - 1;
@@ -455,8 +491,9 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (k) CK(cudaStreamWaitEvent(ss, prev->ev_chain[k - 1], 0));    // token ranks chain through DeviceStatus::tok_end: only the scan waits
         enqueue_scan(b, w, ss, static_cast<ProfEvents*>(nullptr), k ? &prev->d_status_arr[k - 1].tok_end : nullptr);   // (G > 1: a peer pointer)
         CK(cudaEventRecord(ln->ev_chain[k], ss));
+        const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, p0) : TruncateView{};
         enqueue_emit(b, w, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets + q0, ln->d_out_counts + p0,
-                     ss, static_cast<ProfEvents*>(nullptr), out_starts ? ln->d_out_starts : nullptr, &dv->vs);
+                     ss, static_cast<ProfEvents*>(nullptr), out_starts ? ln->d_out_starts : nullptr, &dv->vs, trunc ? &tv : nullptr);
         CK(cudaGetLastError());
         status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr + k, ln->h_status_arr + k);
         CK(cudaEventRecord(ln->ev_done[k], ss));
@@ -475,9 +512,10 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (!err) err = fail_status(ctx, st);
         const uint64_t base = st.tok_end - st.n_tokens;
         tok_total = st.tok_end;
+        if (!err && trunc) { const int rc = download_cuts(ctx, ln, *trunc, p0, nk, ds); if (rc) return rc; }
         if (err || defer) continue;
         if (no_copy) continue;
-        if (want_ids && st.tok_end <= out_cap && st.n_tokens)
+        if (want_ids && out_ids && st.tok_end <= out_cap && st.n_tokens)
             CK(cudaMemcpyAsync(out_ids + base, ln->d_out_ids + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (out_starts && st.tok_end <= out_cap && st.n_tokens)      // (prompt-relative: the same ranks and base as the ids)
             CK(cudaMemcpyAsync(out_starts + base, ln->d_out_starts + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
@@ -513,31 +551,36 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
 // One device's share of a host call (the whole call on a single-device context): validation is done, the lane is locked.
 // defer / cut_out / nc_out: see run_host_pipelined; the one-shot path under `defer` leaves everything on the device as ONE sub-batch.
 // out_starts != nullptr: the tokens' starts too (in ln->d_out_starts, beside the ids; under `defer` it is only a flag).
+// trunc != nullptr: a truncate call (the ids stay in the lane; the cuts and kept counts are downloaded, under `defer` too).
 int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
              uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
-             uint64_t* defer = nullptr, uint32_t* cut_out = nullptr, int* nc_out = nullptr) {
+             uint64_t* defer = nullptr, uint32_t* cut_out = nullptr, int* nc_out = nullptr, const TruncateArgs* trunc = nullptr) {
     CK(cudaSetDevice(dv->device));
     int rc = wait_for_device_call(ctx, ln);
     if (!rc && out_starts) rc = ensure_starts_lane(ctx, ln);
+    if (!rc && trunc) rc = ensure_truncate_lane(ctx, ln);
     if (rc) return rc;
     const bool profiling = ctx->profiling.load();
     if (!profiling && total >= ctx->pipe_min && n >= 2)
         return run_host_pipelined(ctx, &dv, &ln, 1, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                                  defer, cut_out, nc_out);
+                                  defer, cut_out, nc_out, trunc);
     cudaStream_t s = ln->stream;
     ProfEvents* prof = profiling ? &ln->prof : nullptr;
     if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); }
     BatchView b;
     rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b);
+    if (!rc && trunc) rc = upload_budgets(ctx, ln, *trunc, 0, n, s);
     if (rc) return rc;
     if (prof) cudaEventRecord(prof->h2d[1], s);
 
+    const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, 0) : TruncateView{};
     enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets,
                    ln->d_out_counts, static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, out_starts ? ln->d_out_starts : nullptr);
+                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, out_starts ? ln->d_out_starts : nullptr, trunc ? &tv : nullptr);
     CK(cudaGetLastError());
     if (prof) cudaEventRecord(prof->d2h[0], s);
     CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    if (trunc && (rc = download_cuts(ctx, ln, *trunc, 0, n, s))) return rc;
     if (!defer) {
         if (out_offsets) CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
         if (out_counts && n) CK(cudaMemcpyAsync(out_counts, ln->d_out_counts, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
@@ -548,7 +591,7 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     if (defer) { *defer = st.n_tokens; if (cut_out) { cut_out[0] = 0; cut_out[1] = n; *nc_out = 1; } return CFBPE_OK; }
     if (want_ids) {
         if (st.n_tokens > out_cap) return fail_nospace(ctx, st.n_tokens, out_offsets, n);
-        if (st.n_tokens) CK(cudaMemcpyAsync(out_ids, ln->d_out_ids, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        if (out_ids && st.n_tokens) CK(cudaMemcpyAsync(out_ids, ln->d_out_ids, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         if (out_starts && st.n_tokens) CK(cudaMemcpyAsync(out_starts, ln->d_out_starts, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     }
     if (prof) { cudaEventRecord(prof->d2h[1], s); cudaEventRecord(prof->total[1], s); }
@@ -680,7 +723,7 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
 struct SpecialArgs { const uint8_t* const* modes; uint32_t* bad; };
 int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
                      uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
-                     const SpecialArgs* special = nullptr) {
+                     const SpecialArgs* special = nullptr, const TruncateArgs* trunc = nullptr) {
     const uint32_t G = static_cast<uint32_t>(ctx->devs.size());
     std::vector<uint32_t> lo(G + 1, 0);
     for (uint32_t d = 1; d < G; ++d) {      // first prompt whose start is >= d * total / G
@@ -710,8 +753,10 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
                                         special->modes, nullptr, 0, nullptr, nullptr, want_ids, s.local_offs[nd], s.bad, &s.tokens);
                 s.cut[0] = 0; s.cut[1] = nd; s.nc = 1;
             } else {
+                const TruncateArgs shard_trunc = trunc ? truncate_from(*trunc, p0) : TruncateArgs{};
                 s.rc = run_lane(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
-                                nullptr, out_starts, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc);
+                                nullptr, out_starts, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc,
+                                trunc ? &shard_trunc : nullptr);
             }
             if (s.rc) s.err = tl_err;
         });
@@ -763,7 +808,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             ck(cudaStreamSynchronize(st), "stream sync");
             uint64_t base = 0;
             for (uint32_t e = 0; e < d; ++e) base += ln->h_totals[e];
-            if (want_ids && fits && s.tokens) ck(cudaMemcpyAsync(out_ids + base, ln->d_out_ids, s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "ids download");
+            if (want_ids && out_ids && fits && s.tokens) ck(cudaMemcpyAsync(out_ids + base, ln->d_out_ids, s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "ids download");
             if (out_starts && fits && s.tokens) ck(cudaMemcpyAsync(out_starts + base, ln->d_out_starts, s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "starts download");
             ck(cudaStreamSynchronize(st), "stream sync");
         });
@@ -774,16 +819,18 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     return CFBPE_OK;
 }
 
-// shared body of encode_batch / encode_batch_starts / count_batch (host buffers); out_starts: NULL but for encode_batch_starts
+// shared body of encode_batch / encode_batch_starts / count_batch / truncate_batch (host buffers); out_starts: NULL but for
+// encode_batch_starts; trunc: NULL but for truncate_batch (which emits the ids into the lane, out_ids NULL, out_cap unlimited)
 int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
-             uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids) {
+             uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
+             const TruncateArgs* trunc = nullptr) {
     tl_err.clear();
     std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
     uint64_t total = 0;
     int rc = validate_batch(ctx, n, offsets, vocab_ids, &total);
     if (rc) return rc;
     if (total && !bytes) return fail(ctx, CFBPE_EINVAL, "bytes is NULL");
-    if (want_ids && (!out_offsets || (!out_ids && out_cap))) return fail(ctx, CFBPE_EINVAL, "output pointer is NULL");
+    if (want_ids && !trunc && (!out_offsets || (!out_ids && out_cap))) return fail(ctx, CFBPE_EINVAL, "output pointer is NULL");
     if (ctx->devs.size() > 1 && n >= ctx->devs.size() && !ctx->profiling.load()) {
         // Two ways over several devices.  When every device can hold the whole batch (and the devices see each other's memory):
         // the sub-batches of ONE pipelined call go round-robin over the devices -- uploads, kernels and downloads of all devices
@@ -799,17 +846,19 @@ int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* o
                 CK(cudaSetDevice(dvs[g]->device));
                 rc = wait_for_device_call(ctx, lns[g]);
                 if (!rc && out_starts) rc = ensure_starts_lane(ctx, lns[g]);
+                if (!rc && trunc) rc = ensure_truncate_lane(ctx, lns[g]);
                 if (rc) return rc;
             }
             return run_host_pipelined(ctx, dvs, lns, G, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                                      nullptr, nullptr, nullptr);
+                                      nullptr, nullptr, nullptr, trunc);
         }
-        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total);
+        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total, nullptr, trunc);
     }
     if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds max_batch_bytes of this context");
     DeviceCtx* dv = ctx->devs[0].get();
     LaneLock lk(dv);
-    return run_lane(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total);
+    return run_lane(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
+                    nullptr, nullptr, nullptr, trunc);
 }
 
 
@@ -890,7 +939,7 @@ void destroy_lane(Lane* ln) {
     cudaSetDevice(ln->device);
     free_special_lane(ln);
     cudaFree(ln->d_bytes); cudaFree(ln->d_offsets); cudaFree(ln->d_vocab_ids);
-    cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts); cudaFree(ln->d_out_starts);
+    cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts); cudaFree(ln->d_out_starts); cudaFree(ln->d_trunc);
     for_each_ws_buffer(ln->ws, [](auto*& p, WsKind) { cudaFree(p); });
     cudaFree(ln->ws.status);
     cudaFree(ln->d_dec_sums); cudaFree(ln->d_dec_base); cudaFree(ln->d_totals);
@@ -1053,17 +1102,18 @@ int device_call_status(cfbpe_ctx* ctx, const Lane* ln) {
     return CFBPE_OK;
 }
 
-// The shape of a device-path call (the caller's device buffers, the caller's stream): the checks; the device of the buffers (the
+// The shape of a device-path call (the caller's device buffers, the caller's stream): the checks (d_out: the call's required output);
+// the device of the buffers (the
 // first of the context whose ordinal is current, else the first) and a lane of it; the stream ordered after the lane's previous
 // device-path call; then enqueue(dv, ln, b, s, prof) queues the work (prof: profiling, when `profiled` and the context profiles).
 // The lane's workspace stays busy until that has run (ev_ws).  With n_tokens or profiling the call waits and reports the status.
 template <typename F>
 int device_call(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
-                const uint8_t* d_vocab_ids, const uint64_t* d_out_offsets, bool want_ids, uint64_t out_cap, uint64_t* n_tokens, void* stream,
+                const uint8_t* d_vocab_ids, const void* d_out, bool want_ids, uint64_t out_cap, uint64_t* n_tokens, void* stream,
                 bool profiled, F&& enqueue) {
     std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
     if (n_prompts > ctx->max_prompts || total_bytes > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds the limits of this context");
-    if (!d_offsets || !d_out_offsets || (total_bytes && !d_bytes)) return fail(ctx, CFBPE_EINVAL, "device pointer is NULL");
+    if (!d_offsets || !d_out || (total_bytes && !d_bytes)) return fail(ctx, CFBPE_EINVAL, "device pointer is NULL");
     if (!ctx->vocabs[0].loaded && !d_vocab_ids) return fail(ctx, CFBPE_ENOENT, "vocab 0 is not loaded");
     if (!ctx->loaded_mask) return fail(ctx, CFBPE_ENOENT, "no vocabulary is loaded");
     DeviceCtx* dv = ctx->devs[0].get();
@@ -1121,6 +1171,21 @@ int run_device_special(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_byte
         // the lane's status carries the call's id count (cfbpe_device_status checks it against out_cap): n_tokens and tok_end
         if (!rc && spliced) CK(cudaMemcpyAsync(&ln->ws.status->n_tokens, &ln->sp.status->fin.n_tokens, 2 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
         return rc;
+    });
+}
+
+// shared body of truncate_batch_device: the ids and offsets go to the lane's buffers (max_batch_bytes ids fit: no ENOSPC)
+int run_device_truncate(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                        const uint8_t* d_vocab_ids, const uint32_t* d_budgets, uint32_t mode, uint32_t* d_out_cut, uint32_t* d_out_kept,
+                        uint32_t* d_out_counts, void* stream) {
+    return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_cut, false, 0, nullptr, stream, true,
+                       [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents* prof) {
+        const TruncateView tv{d_budgets, mode == CFBPE_TRUNCATE_TAIL ? 1u : 0u, d_out_cut, d_out_kept};
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets, d_out_counts,
+                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
+                       ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, nullptr, &tv);
+        CK(cudaGetLastError());
+        return CFBPE_OK;
     });
 }
 
@@ -1305,6 +1370,16 @@ int cfbpe_count_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, 
     return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, nullptr, nullptr, 0, nullptr, out_counts, false);
 }
 
+int cfbpe_truncate_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                         const uint32_t* budgets, uint32_t mode, uint32_t* out_cut, uint32_t* out_kept, uint32_t* out_counts) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (const char* e = truncate_args_error(budgets, mode, out_cut, out_kept)) return fail(ctx, CFBPE_EINVAL, e);
+    const TruncateArgs t{budgets, mode == CFBPE_TRUNCATE_TAIL ? 1u : 0u, out_cut, out_kept};
+    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, nullptr, nullptr, UINT64_MAX, nullptr, out_counts, true, &t);
+}
+
 int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, const uint64_t* id_offsets,
                        const uint8_t* vocab_ids, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets) {
     DeviceGuard restore_device;
@@ -1376,6 +1451,17 @@ int cfbpe_encode_batch_starts_device(cfbpe_ctx* ctx, uint32_t n_prompts, const u
     if (!d_out_ids || !d_out_starts) return fail(ctx, CFBPE_EINVAL, "d_out_ids and d_out_starts are required");
     return run_device(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, d_out_starts, out_cap, d_out_offsets, d_out_counts,
                       n_tokens, stream);
+}
+
+int cfbpe_truncate_batch_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                                const uint8_t* d_vocab_ids, const uint32_t* d_budgets, uint32_t mode, uint32_t* d_out_cut, uint32_t* d_out_kept,
+                                uint32_t* d_out_counts, void* stream) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (const char* e = truncate_args_error(d_budgets, mode, d_out_cut, d_out_kept)) return fail(ctx, CFBPE_EINVAL, e);
+    return run_device_truncate(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_budgets, mode, d_out_cut, d_out_kept, d_out_counts,
+                               stream);
 }
 
 int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* ids) {

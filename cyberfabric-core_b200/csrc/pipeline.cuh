@@ -126,6 +126,13 @@ inline StatusError status_error(const DeviceStatus& st) {
     return {CFBPE_OK, nullptr};
 }
 
+// the checks of a truncate call's own arguments (cfbpe_truncate_batch and its device form): the error, or nullptr
+inline const char* truncate_args_error(const uint32_t* budgets, uint32_t mode, const uint32_t* cut, const uint32_t* kept) {
+    if (mode != CFBPE_TRUNCATE_HEAD && mode != CFBPE_TRUNCATE_TAIL) return "mode is not a CFBPE_TRUNCATE_* value";
+    if (!budgets || !cut || !kept) return "budgets, out_cut and out_kept are required";
+    return nullptr;
+}
+
 // K2b CTAs per SM (long_grid = 4 x SM count).  8 x 128 threads x 64 registers is the whole register file of an SM: the
 // short-piece kernels on the other stream then wait for K2b instead of running beside it.
 #ifndef CFBPE_LONG_CTAS
@@ -244,9 +251,12 @@ inline void enqueue_scan(const BatchView& b, const Workspace& w, Stream stream, 
 // starts come from the ids: the tokens tile the text, so a token's byte position is the sum of the byte lengths of the tokens
 // before it.  Lengths and their per-tile sums, a scan of the tile sums, then the scan inside every tile minus the prompt's offset.
 // The dense-id tile arrays are free once the ids are out (the tiles of 2048 tokens are no more than the 2 KiB piece tiles).
+// trunc (nullable; only with out_ids, and then vs too): every prompt's cut to its token budget, from the ids where they are
+// (truncate_kernel, and truncate_long_kernel for the prompts with more ids to sum than one warp takes).
 template <typename Stream, typename Prof>
 inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
-                         uint32_t* out_counts, Stream stream, Prof* prof, uint32_t* out_starts = nullptr, const VocabSet* vs = nullptr) {
+                         uint32_t* out_counts, Stream stream, Prof* prof, uint32_t* out_starts = nullptr, const VocabSet* vs = nullptr,
+                         const TruncateView* trunc = nullptr) {
     CFBPE_MARK(prof, K_EMIT, stream, true);
     if (b.total_bytes && out_ids) {
         CFBPE_LAUNCH(emit_compact_kernel, n_scan_tiles(b.total_bytes), 256, stream, w.tok_bits, w.piece_bits, n_flag_words(b.total_bytes), w.tile_base,
@@ -262,24 +272,33 @@ inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_i
                      static_cast<const uint64_t*>(nullptr));
         CFBPE_LAUNCH(starts_emit_kernel, n_tiles, 256, stream, b, out_offsets, out_cap, w.status, w.dense.piece_base, out_starts);
     }
+    if (out_ids && trunc && b.n_prompts) {
+        CFBPE_LAUNCH(truncate_kernel, static_cast<unsigned>((static_cast<uint64_t>(b.n_prompts) + 7) / 8), 256, stream,    // a warp per prompt
+                     b, *vs, out_ids, out_offsets, *trunc);
+        if (b.total_bytes > kTruncChunkBytes) {       // (else no prompt has more than kTruncPartIds ids to sum)
+            const uint64_t n_chunks = (b.total_bytes + kTruncChunkBytes - 1) / kTruncChunkBytes;
+            CFBPE_LAUNCH(truncate_long_kernel, static_cast<unsigned>((n_chunks + 7) / 8), 256, stream, b, *vs, out_ids, out_offsets, *trunc);
+        }
+    }
 }
 template <typename Stream, typename Prof>
 inline void enqueue_back(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
                          uint32_t* out_counts, Stream stream, Prof* prof, const uint64_t* token_base, uint32_t* out_starts = nullptr,
-                         const VocabSet* vs = nullptr) {
+                         const VocabSet* vs = nullptr, const TruncateView* trunc = nullptr) {
     enqueue_count(b, w, stream, prof);
     enqueue_scan(b, w, stream, prof, token_base);
-    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs);
+    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs, trunc);
 }
 
 // The whole path.  `aux` / `aux2` are streams of their own for the two long-piece kernels (pass the main stream to run everything
 // in order); CFBPE_FORK / CFBPE_JOIN order them.  out_ids may be nullptr (count only); out_starts (nullable, with out_ids): the
-// tokens' byte offsets within their prompts.  Everything is asynchronous.
+// tokens' byte offsets within their prompts; trunc (nullable, with out_ids): the prompts' cuts to their token budgets.  Everything
+// is asynchronous.
 template <typename Stream, typename Prof, typename Ev>
 inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTables& uc, const Workspace& w,
                            uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
                            uint32_t long_grid, Stream stream, Stream aux, Stream aux2, Ev ev_fork, Ev ev_join, Ev ev_join2, Prof* prof,
-                           const uint64_t* token_base = nullptr, uint32_t* out_starts = nullptr) {
+                           const uint64_t* token_base = nullptr, uint32_t* out_starts = nullptr, const TruncateView* trunc = nullptr) {
     enqueue_split(b, vs, uc, w, stream, prof, long_grid / 4);
     CFBPE_FORK(stream, aux2, ev_fork);
     enqueue_list(b, vs, w, long_grid, aux2, prof);
@@ -288,7 +307,7 @@ inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTable
     enqueue_short(b, vs, w, long_grid, stream, prof);
     CFBPE_JOIN(stream, aux, ev_join);
     CFBPE_JOIN(stream, aux2, ev_join2);
-    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base, out_starts, &vs);
+    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base, out_starts, &vs, trunc);
 }
 
 }  // namespace cfbpe

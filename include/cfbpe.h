@@ -172,6 +172,31 @@ CFBPE_API int cfbpe_encode_batch_starts(cfbpe_ctx *ctx, uint32_t n_prompts, cons
 CFBPE_API int cfbpe_count_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
                       const uint8_t *vocab_ids, uint32_t *out_counts);
 
+/* which tokens a truncation keeps (cfbpe_truncate_batch) */
+#define CFBPE_TRUNCATE_HEAD 0u   /* the first ones: a long document or retrieved context */
+#define CFBPE_TRUNCATE_TAIL 1u   /* the last ones: a chat history */
+/* Cut every prompt to a token budget: where its text must be cut so that it keeps budgets[i] tokens, as one byte position.
+ * For prompt i with bytes b, ids t_0 .. t_{c-1} (cfbpe_encode_batch) and k = min(budgets[i], c):
+ *   CFBPE_TRUNCATE_HEAD: x = the byte length of t_0 .. t_{k-1}; out_cut[i] = the largest character start <= x, and the kept text
+ *                        is b[0 .. out_cut[i]).
+ *   CFBPE_TRUNCATE_TAIL: x = len(b) - the byte length of t_{c-k} .. t_{c-1}; out_cut[i] = the smallest character start >= x, or
+ *                        len(b), and the kept text is b[out_cut[i] .. len(b)).
+ * A byte-level token may end inside a UTF-8 character; the cut always moves to a character boundary, so the kept text is valid
+ * UTF-8 (a caller who needs the token boundary itself has cfbpe_encode_batch_starts).  out_kept[i] = the tokens of the encoding
+ * that lie wholly inside the kept text: k, or fewer when the cut moved.  out_counts[i] = c, as cfbpe_count_batch (may be NULL).
+ * A budget of 0 keeps nothing (head: cut 0, tail: cut len(b)); a budget >= c keeps the whole prompt.  Cuts and kept counts are
+ * per prompt and relative to it.
+ * The boundaries are those of the encoding of the WHOLE prompt, as decode(ids[:N]) of tiktoken or the id truncation of Hugging
+ * Face tokenizers: BPE is not prefix-stable, so encoding the kept text again may give other ids (and another count).
+ * mode: a CFBPE_TRUNCATE_* value.  budgets, out_cut, out_kept: n_prompts entries each, required.  Errors: an unknown mode or a
+ * NULL budgets / out_cut / out_kept is CFBPE_EINVAL; the rest as cfbpe_count_batch.  The ids stay on the device: the cut is a
+ * sum of token lengths over the nearer end of each prompt's ids, at most min(k, c - k) of them, and a prompt with c <= budget reads
+ * none.  Costs: 12 bytes of device memory per prompt of max_prompts on each lane that runs a host call of it, allocated on its
+ * first one (CFBPE_ENOMEM if that fails). */
+CFBPE_API int cfbpe_truncate_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
+                                   const uint8_t *vocab_ids, const uint32_t *budgets, uint32_t mode, uint32_t *out_cut,
+                                   uint32_t *out_kept, uint32_t *out_counts);
+
 /* Decode (SURVEY.md section 8(f) item 2; tiktoken CoreBPE.decode_bytes): out_bytes = the concatenation of the tokens' bytes.
  * ids: the packed token ids of n_seqs sequences, id_offsets[n_seqs + 1] their boundaries (in ids), vocab_ids[n_seqs] or NULL.
  * out_offsets[n_seqs + 1]: byte boundaries of the decoded sequences in out_bytes.  CFBPE_ENOSPC if out_cap is too small
@@ -233,6 +258,14 @@ CFBPE_API int cfbpe_encode_batch_starts_device(cfbpe_ctx *ctx, uint32_t n_prompt
                                                const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t *d_out_ids,
                                                uint32_t *d_out_starts, uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
                                                uint64_t *n_tokens, void *stream);
+/* cfbpe_truncate_batch on device-resident buffers, enqueued on `stream` as cfbpe_encode_batch_device (d_bytes readable for 32
+ * bytes past total_bytes).  d_budgets, d_out_cut, d_out_kept and d_out_counts (may be NULL) are device memory.  Fully
+ * asynchronous: nothing has to come back to the host, and the ids, which never exceed max_batch_bytes, stay in the lane's
+ * buffers (no CFBPE_ENOSPC).  Malformed UTF-8 and an unloaded vocabulary are reported by the next call that synchronises (or
+ * cfbpe_device_status). */
+CFBPE_API int cfbpe_truncate_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
+                                          const uint64_t *d_offsets, const uint8_t *d_vocab_ids, const uint32_t *d_budgets, uint32_t mode,
+                                          uint32_t *d_out_cut, uint32_t *d_out_kept, uint32_t *d_out_counts, void *stream);
 /* Synchronise `stream` and return the status word of the last device call (0, CFBPE_EILSEQ, CFBPE_ENOSPC). */
 CFBPE_API int cfbpe_device_status(cfbpe_ctx *ctx, void *stream);
 

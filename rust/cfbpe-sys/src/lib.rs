@@ -25,6 +25,10 @@ pub const CFBPE_SPECIAL_ALLOW: u8 = 1;
 pub const CFBPE_SPECIAL_DISALLOW: u8 = 2;
 pub const CFBPE_MAX_SPECIALS: usize = 4096;
 
+/// `cfbpe_truncate_batch`: keep the first / the last tokens of every prompt
+pub const CFBPE_TRUNCATE_HEAD: u32 = 0;
+pub const CFBPE_TRUNCATE_TAIL: u32 = 1;
+
 pub const CFBPE_FORMAT_TIKTOKEN: u32 = 0;
 pub const CFBPE_FORMAT_TEKKEN_JSON: u32 = 1;
 pub const CFBPE_MAX_VOCABS: u32 = 8;
@@ -82,6 +86,11 @@ extern "C" {
                                             d_out_offsets: *mut u64, d_out_counts: *mut u32, n_tokens: *mut u64, stream: *mut c_void) -> c_int;
     pub fn cfbpe_count_batch(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64,
                              vocab_ids: *const u8, out_counts: *mut u32) -> c_int;
+    pub fn cfbpe_truncate_batch(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64, vocab_ids: *const u8,
+                                budgets: *const u32, mode: u32, out_cut: *mut u32, out_kept: *mut u32, out_counts: *mut u32) -> c_int;
+    pub fn cfbpe_truncate_batch_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64, d_offsets: *const u64,
+                                       d_vocab_ids: *const u8, d_budgets: *const u32, mode: u32, d_out_cut: *mut u32, d_out_kept: *mut u32,
+                                       d_out_counts: *mut u32, stream: *mut c_void) -> c_int;
     pub fn cfbpe_decode_batch(ctx: *mut cfbpe_ctx, n_seqs: u32, ids: *const u32, id_offsets: *const u64,
                               vocab_ids: *const u8, out_bytes: *mut u8, out_cap: u64, out_offsets: *mut u64) -> c_int;
     pub fn cfbpe_encode_batch_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64,
@@ -114,6 +123,15 @@ pub struct NativeError {
 pub struct Encoded {
     pub ids: Vec<u32>,
     pub offsets: Vec<u64>,
+    pub counts: Vec<u32>,
+}
+
+/// Result of [`Ctx::truncate_batch`], one entry per prompt: where to cut it (a byte position within the prompt; head keeps
+/// `[0, cut)`, tail keeps `[cut, len)`), the tokens wholly inside the kept text, and the tokens of the whole prompt.
+#[derive(Debug, Default)]
+pub struct Truncated {
+    pub cut: Vec<u32>,
+    pub kept: Vec<u32>,
     pub counts: Vec<u32>,
 }
 
@@ -282,6 +300,31 @@ impl Ctx {
         self.check(rc)?;
         counts.truncate(n as usize);
         Ok(counts)
+    }
+
+    /// Cut every prompt to its token budget (`budgets[i]`; `mode`: `CFBPE_TRUNCATE_HEAD` or `CFBPE_TRUNCATE_TAIL`): the cut is at
+    /// a token boundary of the whole prompt's encoding moved to a character boundary, so the kept text is valid UTF-8.  Only the
+    /// cuts, kept counts and counts leave the device.
+    pub fn truncate_batch(&self, bytes: &[u8], offsets: &[u64], vocab_ids: Option<&[u8]>, budgets: &[u32], mode: u32)
+        -> Result<Truncated, NativeError> {
+        let n = Self::check_inputs(bytes.len(), offsets, vocab_ids)?;
+        if budgets.len() < n as usize {
+            return Err(NativeError { code: CFBPE_EINVAL, message: "budgets needs one entry per prompt".to_owned() });
+        }
+        let m = (n as usize).max(1);
+        let mut out = Truncated { cut: vec![0; m], kept: vec![0; m], counts: vec![0; m] };
+        let bud_one = [0u32; 1];
+        let bud = if budgets.is_empty() { &bud_one[..] } else { budgets };
+        // SAFETY: every per-prompt buffer holds at least n entries and none is retained.
+        let rc = unsafe {
+            cfbpe_truncate_batch(self.0.as_ptr(), n, bytes.as_ptr(), offsets.as_ptr(), vocab_ids.map_or(std::ptr::null(), <[u8]>::as_ptr),
+                                 bud.as_ptr(), mode, out.cut.as_mut_ptr(), out.kept.as_mut_ptr(), out.counts.as_mut_ptr())
+        };
+        self.check(rc)?;
+        for v in [&mut out.cut, &mut out.kept, &mut out.counts] {
+            v.truncate(n as usize);
+        }
+        Ok(out)
     }
 
     /// ids -> bytes (tiktoken `decode_bytes`); grows the output once when the library reports `CFBPE_ENOSPC`.

@@ -7,7 +7,7 @@ use async_trait::async_trait;
 use cfbpe_sys::{Ctx, NativeError};
 use llm_gateway_sdk::{
     CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens, TokenizerError,
-    TokenizerPluginClient, VocabRef,
+    TokenizerPluginClient, TruncateBatchResponse, TruncateKeep, VocabRef,
 };
 use modkit_security::SecurityContext;
 use sha2::{Digest, Sha256};
@@ -145,6 +145,23 @@ impl TokenizerPluginClient for Service {
             .map_err(|e| TokenizerError::Internal(e.to_string()))?
             .map_err(map_native)?;
         Ok(DecodeBatchResponse { bytes, offsets })
+    }
+
+    /// The device path (`cfbpe_truncate_batch`): the cut is a sum of token lengths where the ids are; no id leaves the device.
+    async fn truncate_batch(&self, _ctx: &SecurityContext, req: EncodeBatchRequest, budgets: &[u32], keep: TruncateKeep)
+        -> Result<TruncateBatchResponse, TokenizerError> {
+        let n = req.offsets.len().saturating_sub(1);
+        if budgets.len() != n {
+            return Err(TokenizerError::InvalidInput("one token budget per prompt".to_owned()));
+        }
+        let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
+        let mode = match keep { TruncateKeep::Head => cfbpe_sys::CFBPE_TRUNCATE_HEAD, TruncateKeep::Tail => cfbpe_sys::CFBPE_TRUNCATE_TAIL };
+        let (native, budgets) = (self.native.clone(), budgets.to_vec());
+        let out = tokio::task::spawn_blocking(move || native.truncate_batch(&req.bytes, &req.offsets, vid.as_deref(), &budgets, mode))
+            .await
+            .map_err(|e| TokenizerError::Internal(e.to_string()))?
+            .map_err(map_native)?;
+        Ok(TruncateBatchResponse { cut: out.cut, kept: out.kept, counts: out.counts })
     }
 
     /// The device path: scan, cut and splice run as CUDA kernels (`cfbpe_encode_batch_special`).  The caller's special tokens

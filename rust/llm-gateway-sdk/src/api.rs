@@ -5,7 +5,7 @@ use modkit_security::SecurityContext;
 use serde_json::Value;
 
 use crate::error::TokenizerError;
-use crate::models::{ChatTemplate, SpecialTokens, Usage};
+use crate::models::{ChatTemplate, SpecialTokens, TruncateKeep, Usage};
 
 #[async_trait]
 pub trait TokenizerClient: Send + Sync {
@@ -15,6 +15,11 @@ pub trait TokenizerClient: Send + Sync {
     /// Per text: the ids and each token's `[start, end)` byte span in the text's UTF-8 (cut to a context window or into chunks
     /// at a span boundary).
     async fn encode_with_offsets(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError>;
+
+    /// Fit texts into a context window: per text, (the kept text, its tokens, the tokens of the whole text).  `max_tokens`: one
+    /// budget per text; `keep`: the first or the last tokens.  The cut is at a character boundary, so the kept text is valid UTF-8.
+    async fn truncate(&self, ctx: &SecurityContext, model: &str, texts: &[String], max_tokens: &[u32], keep: TruncateKeep)
+        -> Result<Vec<(String, u32, u32)>, TokenizerError>;
 
     /// tiktoken's `encode(text, allowed_special = …, disallowed_special = …)`.
     async fn encode_with_special(&self, ctx: &SecurityContext, model: &str, texts: &[String], special: &SpecialTokens)

@@ -42,6 +42,52 @@ pub struct EncodeBatchResponse {
     pub starts: Option<Vec<u32>>,
 }
 
+/// Which tokens a truncation keeps.
+#[derive(Debug, Clone, Copy, PartialEq, Eq, Default, Serialize, Deserialize, schemars::JsonSchema)]
+#[serde(rename_all = "lowercase")]
+pub enum TruncateKeep {
+    /// the first ones: a long document or retrieved context
+    #[default]
+    Head,
+    /// the last ones: a chat history
+    Tail,
+}
+
+/// Where every prompt of a batch is cut to its token budget, one entry per prompt (`include/cfbpe.h`, `cfbpe_truncate_batch`).
+/// For prompt i with tokens t_0 .. t_{c-1} and k = min(budget, c): `Head` keeps `bytes[0 .. cut)`, cut = the character start at or
+/// before the end of t_{k-1}; `Tail` keeps `bytes[cut .. len)`, cut = the character start at or after the start of t_{c-k}.  The
+/// boundaries are those of the WHOLE prompt's encoding; encoding the kept text again may give other ids (BPE is not prefix-stable).
+#[derive(Debug, Clone, Default, Serialize, Deserialize)]
+pub struct TruncateBatchResponse {
+    /// byte position of the cut within the prompt (always a character boundary: the kept text is valid UTF-8)
+    pub cut: Vec<u32>,
+    /// tokens of the prompt's encoding wholly inside the kept text: k, or fewer when the cut moved off a token boundary
+    pub kept: Vec<u32>,
+    /// tokens of the whole prompt
+    pub counts: Vec<u32>,
+}
+
+/// The truncation contract on the host, from every token's start (`EncodeBatchResponse::starts`): `(cut, kept)` of prompt
+/// `prompt` (its UTF-8 bytes), whose tokens start at `starts`.
+pub fn truncate_cut(prompt: &[u8], starts: &[u32], budget: u32, keep: TruncateKeep) -> (u32, u32) {
+    let (c, len) = (starts.len(), prompt.len());
+    let k = (budget as usize).min(c);
+    let j = if keep == TruncateKeep::Tail { c - k } else { k };
+    let mut x = if j < c { starts[j] as usize } else { len };
+    let cont = |b: u8| b & 0xC0 == 0x80;
+    match keep {
+        TruncateKeep::Tail => {
+            while x < len && cont(prompt[x]) { x += 1; }
+            (x as u32, (c - starts.partition_point(|&s| (s as usize) < x)) as u32)
+        }
+        TruncateKeep::Head => {
+            while x > 0 && x < len && cont(prompt[x]) { x -= 1; }
+            let ends = |i: usize| if i + 1 < c { starts[i + 1] as usize } else { len };
+            ((x as u32), (0..c).take_while(|&i| ends(i) <= x).count() as u32)
+        }
+    }
+}
+
 #[derive(Debug, Clone)]
 pub struct CountTokensRequest {
     pub vocab: VocabRef,

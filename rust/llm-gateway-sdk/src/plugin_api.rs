@@ -4,7 +4,8 @@ use async_trait::async_trait;
 use modkit_security::SecurityContext;
 
 use crate::error::TokenizerError;
-use crate::models::{CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens, VocabRef};
+use crate::models::{truncate_cut, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens,
+                    TruncateBatchResponse, TruncateKeep, VocabRef};
 
 /// Each plugin registers this trait with a scoped `ClientHub` entry using its GTS instance id as the scope.  Clients are
 /// `Arc<dyn … + Send + Sync>` shared by all tokio tasks (`libs/modkit/src/client_hub.rs:142-165`): calls are concurrent and
@@ -22,6 +23,30 @@ pub trait TokenizerPluginClient: Send + Sync {
 
     /// ids -> bytes; `InvalidInput` for an id outside its vocabulary.
     async fn decode_batch(&self, ctx: &SecurityContext, req: DecodeBatchRequest) -> Result<DecodeBatchResponse, TokenizerError>;
+
+    /// Cut every prompt of the batch to its token budget (`budgets`: one per prompt), keeping its first or last tokens, at a
+    /// character boundary (`TruncateBatchResponse`).  The default works on any plugin that returns token starts: one
+    /// `encode_batch` with `with_starts`, then the cut on the host.  `gpu-bpe-tokenizer-plugin` overrides it with the device
+    /// call, which downloads no ids.
+    async fn truncate_batch(&self, ctx: &SecurityContext, req: EncodeBatchRequest, budgets: &[u32], keep: TruncateKeep)
+        -> Result<TruncateBatchResponse, TokenizerError> {
+        let n = req.offsets.len().saturating_sub(1);
+        if budgets.len() != n {
+            return Err(TokenizerError::InvalidInput("one token budget per prompt".to_owned()));
+        }
+        let bytes = req.bytes.clone();
+        let offsets = req.offsets.clone();
+        let enc = self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, ..req }).await?;
+        let starts = enc.starts.ok_or_else(|| TokenizerError::ServiceUnavailable("the tokenizer plugin does not return token starts".to_owned()))?;
+        let mut out = TruncateBatchResponse { cut: Vec::with_capacity(n), kept: Vec::with_capacity(n), counts: enc.counts };
+        for i in 0..n {
+            let prompt = &bytes[offsets[i] as usize..offsets[i + 1] as usize];
+            let (cut, kept) = truncate_cut(prompt, &starts[enc.offsets[i] as usize..enc.offsets[i + 1] as usize], budgets[i], keep);
+            out.cut.push(cut);
+            out.kept.push(kept);
+        }
+        Ok(out)
+    }
 
     /// tiktoken's `encode(text, allowed_special = …, disallowed_special = …)` for every prompt of the batch; `InvalidInput` when
     /// a prompt spells a special token that is not allowed.  The default works on any plugin: it cuts every text at the

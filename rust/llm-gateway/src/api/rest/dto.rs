@@ -1,4 +1,4 @@
-//! REST DTOs of `POST /llm-gateway/v1/tokenize` and `POST /llm-gateway/v1/count-tokens`.
+//! REST DTOs of `POST /llm-gateway/v1/tokenize`, `POST /llm-gateway/v1/count-tokens` and `POST /llm-gateway/v1/truncate`.
 
 use schemars::JsonSchema;
 use serde::{Deserialize, Serialize};
@@ -29,6 +29,38 @@ pub struct TokenizeResponse {
     /// byte span of every token of every text, when asked for
     #[serde(skip_serializing_if = "Option::is_none")]
     pub offsets: Option<Vec<Vec<[u64; 2]>>>,
+}
+
+/// A token budget: one for every text, or one per text.
+#[derive(Debug, Deserialize, JsonSchema)]
+#[serde(untagged)]
+pub enum MaxTokens {
+    All(u32),
+    PerText(Vec<u32>),
+}
+
+#[derive(Debug, Deserialize, JsonSchema)]
+#[serde(deny_unknown_fields)]
+pub struct TruncateRequest {
+    /// canonical model id or vocabulary name
+    pub model: String,
+    /// texts to fit into the budget (one entry per prompt)
+    pub texts: Vec<String>,
+    /// the token budget
+    pub max_tokens: MaxTokens,
+    /// `head` keeps the first tokens (a document, retrieved context), `tail` the last ones (a chat history); default `head`
+    #[serde(default)]
+    pub keep: llm_gateway_sdk::TruncateKeep,
+}
+
+#[derive(Debug, Serialize, JsonSchema)]
+pub struct TruncateResponse {
+    /// every text cut at a token boundary of its whole encoding, moved to a character boundary (valid UTF-8)
+    pub texts: Vec<String>,
+    /// tokens of every text's encoding wholly inside the kept text: the budget, or one to three fewer when the cut moved
+    pub kept_tokens: Vec<u32>,
+    /// token count of every whole text, as `counts` of `/tokenize`
+    pub counts: Vec<u32>,
 }
 
 /// How the provider frames the messages (`llm_gateway_sdk::ChatTemplate`); absent: content only.

@@ -7,7 +7,9 @@ use llm_gateway_sdk::{ChatTemplate, TokenizerClient, TokenizerError};
 use modkit_errors::Problem;
 use modkit_security::SecurityContext;
 
-use crate::api::rest::dto::{ChatTemplateDto, CountTokensRequest, CountTokensResponse, TokenizeRequest, TokenizeResponse};
+use crate::api::rest::dto::{
+    ChatTemplateDto, CountTokensRequest, CountTokensResponse, MaxTokens, TokenizeRequest, TokenizeResponse, TruncateRequest, TruncateResponse,
+};
 use crate::domain::service::TokenizerService;
 
 fn problem(e: TokenizerError) -> Problem {
@@ -37,6 +39,27 @@ pub async fn tokenize(
     let counts: Vec<u32> = ids.iter().map(|v| v.len() as u32).collect();
     let input_tokens = counts.iter().map(|c| u64::from(*c)).sum();
     Ok(Json(TokenizeResponse { counts, input_tokens, ids: req.return_ids.then_some(ids), offsets }))
+}
+
+pub async fn truncate(
+    Extension(ctx): Extension<SecurityContext>,
+    Extension(service): Extension<Arc<TokenizerService>>,
+    Json(req): Json<TruncateRequest>,
+) -> Result<Json<TruncateResponse>, Problem> {
+    tracing::debug!(model = %req.model, texts = req.texts.len(), bytes = req.texts.iter().map(String::len).sum::<usize>(), "truncate");
+    let budgets = match req.max_tokens {
+        MaxTokens::All(b) => vec![b; req.texts.len()],
+        MaxTokens::PerText(v) if v.len() == req.texts.len() => v,
+        MaxTokens::PerText(_) => return Err(problem(TokenizerError::InvalidInput("max_tokens needs one budget per text".to_owned()))),
+    };
+    let r = service.truncate(&ctx, &req.model, &req.texts, &budgets, req.keep).await.map_err(problem)?;
+    let mut out = TruncateResponse { texts: Vec::with_capacity(r.len()), kept_tokens: Vec::with_capacity(r.len()), counts: Vec::with_capacity(r.len()) };
+    for (text, kept, count) in r {
+        out.texts.push(text);
+        out.kept_tokens.push(kept);
+        out.counts.push(count);
+    }
+    Ok(Json(out))
 }
 
 pub async fn count_tokens(

@@ -48,5 +48,19 @@ pub fn register_routes(mut router: Router, openapi: &dyn OpenApiRegistry, servic
         .standard_errors(openapi)
         .error_415(openapi)
         .register(router, openapi);
+    // POST /llm-gateway/v1/truncate - cut texts to a token budget (keep the head or the tail) at a character boundary
+    router = OperationBuilder::post("/llm-gateway/v1/truncate")
+        .operation_id("llm_gateway.truncate")
+        .summary("Cut texts to a token budget of a model's vocabulary, keeping their first or last tokens")
+        .tag("LLM Gateway")
+        .authenticated()
+        .require_license_features::<License>([])
+        .json_request::<dto::TruncateRequest>(openapi, "Texts, the model whose vocabulary applies, the budget and which end to keep")
+        .allow_content_types(&["application/json"])
+        .handler(handlers::truncate)
+        .json_response_with_schema::<dto::TruncateResponse>(openapi, http::StatusCode::OK, "The kept texts, their tokens and the full counts")
+        .standard_errors(openapi)
+        .error_415(openapi)
+        .register(router, openapi);
     router.layer(Extension(service))
 }

@@ -7,8 +7,8 @@ use std::sync::Arc;
 use async_trait::async_trait;
 use bytes::Bytes;
 use llm_gateway_sdk::{
-    ChatTemplate, CountTokensRequest, EncodeBatchRequest, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1, Usage,
-    VocabRef,
+    ChatTemplate, CountTokensRequest, EncodeBatchRequest, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1,
+    TruncateKeep, Usage, VocabRef,
 };
 use modkit::client_hub::{ClientHub, ClientScope};
 use modkit::plugins::{choose_plugin_instance, GtsPluginSelector};
@@ -90,6 +90,24 @@ impl TokenizerClient for TokenizerService {
             let spans = (a..b).map(|k| [u64::from(starts[k]), if k + 1 < b { u64::from(starts[k + 1]) } else { len }]).collect();
             (r.ids[a..b].to_vec(), spans)
         }).collect())
+    }
+
+    async fn truncate(&self, ctx: &SecurityContext, model: &str, texts: &[String], max_tokens: &[u32], keep: TruncateKeep)
+        -> Result<Vec<(String, u32, u32)>, TokenizerError> {
+        // the plugin does the work: the trait's default cuts on the host from token starts, the GPU plugin cuts on the device
+        if max_tokens.len() != texts.len() {
+            return Err(TokenizerError::InvalidInput("one token budget per text".to_owned()));
+        }
+        let (bytes, offsets) = pack_texts(texts);
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false };
+        let r = self.plugin().await?.truncate_batch(ctx, req, max_tokens, keep).await?;
+        texts.iter().enumerate().map(|(i, t)| {
+            let cut = r.cut[i] as usize;
+            // a cut is always a character boundary (include/cfbpe.h); get() refuses anything else instead of panicking
+            let kept = match keep { TruncateKeep::Head => t.get(..cut), TruncateKeep::Tail => t.get(cut..) }
+                .ok_or_else(|| TokenizerError::Internal(format!("the plugin cut text {i} inside a character")))?;
+            Ok((kept.to_owned(), r.kept[i], r.counts[i]))
+        }).collect()
     }
 
     async fn encode_with_special(&self, ctx: &SecurityContext, model: &str, texts: &[String], special: &SpecialTokens)
