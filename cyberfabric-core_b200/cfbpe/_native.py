@@ -29,6 +29,7 @@ EXPORTS = [
     "cfbpe_vocab_set_specials", "cfbpe_encode_batch_special", "cfbpe_encode_batch_special_device",
     "cfbpe_encode_batch_starts", "cfbpe_encode_batch_starts_device",
     "cfbpe_truncate_batch", "cfbpe_truncate_batch_device",
+    "cfbpe_chunk_batch", "cfbpe_chunk_batch_device",
 ]
 
 
@@ -112,6 +113,11 @@ def load():
     L.cfbpe_truncate_batch.argtypes = [vp, C.c_uint32, u8p, vp, u8p, vp, C.c_uint32, vp, vp, vp]
     L.cfbpe_truncate_batch_device.restype = C.c_int
     L.cfbpe_truncate_batch_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.cfbpe_chunk_batch.restype = C.c_int
+    L.cfbpe_chunk_batch.argtypes = [vp, C.c_uint32, u8p, vp, u8p, C.c_uint32, C.c_uint32, vp, C.c_uint64, vp, vp]
+    L.cfbpe_chunk_batch_device.restype = C.c_int
+    L.cfbpe_chunk_batch_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, C.c_uint32, C.c_uint32, vp, C.c_uint64, vp, vp,
+                                           C.POINTER(C.c_uint64), vp]
     L.cfbpe_vocab_set_specials.restype = C.c_int
     L.cfbpe_vocab_set_specials.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, vp, vp]
     L.cfbpe_encode_batch_special.restype = C.c_int
@@ -312,6 +318,37 @@ class Context:
                                                 bud.ctypes.data, mode, outs[0].ctypes.data, outs[1].ctypes.data, outs[2].ctypes.data))
         return outs[0][:n], outs[1][:n], outs[2][:n]
 
+    @staticmethod
+    def chunk_bound(offsets: np.ndarray, chunk_tokens: int, overlap_tokens: int = 0) -> int:
+        """chunks a batch can have at most (include/cfbpe.h, cfbpe_chunk_batch): the chunk formula with c = each prompt's byte length"""
+        ln = np.diff(np.asarray(offsets, dtype=np.int64))
+        step = chunk_tokens - overlap_tokens
+        if chunk_tokens < 1 or step < 1:
+            return 0
+        return int((ln > 0).sum() + ((np.maximum(ln - chunk_tokens, 0) + step - 1) // step).sum())
+
+    def chunk_batch(self, data: np.ndarray, offsets: np.ndarray, chunk_tokens: int, overlap_tokens: int = 0, vocab_ids=None,
+                    out_counts=None):
+        """cfbpe_chunk_batch: (spans, chunk_offsets, counts).  spans: uint32 [chunks, 2], (begin, end) of every chunk within its
+        prompt; prompt i's chunks are spans[chunk_offsets[i] .. chunk_offsets[i + 1]] (uint64, n + 1); counts: uint32 tokens a
+        prompt.  chunk_cap is the byte bound (chunk_bound), so the call never needs a second try."""
+        n = self._check_inputs(data, offsets, vocab_ids)
+        if not (isinstance(chunk_tokens, (int, np.integer)) and isinstance(overlap_tokens, (int, np.integer))
+                and 0 <= int(chunk_tokens) <= 0xFFFFFFFF and 0 <= int(overlap_tokens) <= 0xFFFFFFFF):
+            raise NativeError(EINVAL, "chunk_tokens and overlap_tokens must be integers in 0 .. 2^32 - 1")
+        cap = self.chunk_bound(offsets, int(chunk_tokens), int(overlap_tokens))
+        spans = np.empty((max(cap, 1), 2), dtype=np.uint32)
+        coffs = np.zeros(n + 1, dtype=np.uint64)
+        if out_counts is None:
+            out_counts = np.empty(max(n, 1), dtype=np.uint32)
+        elif not isinstance(out_counts, np.ndarray) or out_counts.dtype != np.uint32 or out_counts.size < n or not out_counts.flags.c_contiguous:
+            raise NativeError(EINVAL, "out_counts must be a C-contiguous uint32 array with one entry per prompt")
+        vid = None if vocab_ids is None else vocab_ids.ctypes.data
+        self._check(load().cfbpe_chunk_batch(self._h, n, data.ctypes.data if data.size else None, offsets.ctypes.data, vid,
+                                             int(chunk_tokens), int(overlap_tokens), spans.ctypes.data, cap, coffs.ctypes.data,
+                                             out_counts.ctypes.data))
+        return spans[:int(coffs[n])], coffs, out_counts[:n]
+
     def count_batch(self, data: np.ndarray, offsets: np.ndarray, vocab_ids=None, out_counts=None):
         n = self._check_inputs(data, offsets, vocab_ids)
         if out_counts is None:
@@ -369,6 +406,16 @@ class Context:
         may be None).  Asynchronous: errors come from the next synchronising call or device_status."""
         self._check(load().cfbpe_truncate_batch_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_budgets,
                                                        mode, d_out_cut, d_out_kept, d_out_counts, stream))
+
+    def chunk_batch_device(self, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, chunk_tokens, overlap_tokens, d_out_spans,
+                           chunk_cap, d_out_chunk_offsets, d_out_counts, stream=0, sync=True):
+        """cfbpe_chunk_batch_device on raw device pointers (d_out_spans: room for chunk_cap pairs of uint32; d_out_chunk_offsets:
+        n_prompts + 1 uint64; d_out_counts: n_prompts uint32 or None); the chunk count when sync, else fully asynchronous"""
+        nc = C.c_uint64(0)
+        rc = load().cfbpe_chunk_batch_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, chunk_tokens, overlap_tokens,
+                                             d_out_spans, chunk_cap, d_out_chunk_offsets, d_out_counts, C.byref(nc) if sync else None, stream)
+        self._check(rc)
+        return nc.value if sync else None
 
     # ---- special tokens
     @staticmethod

@@ -162,6 +162,50 @@ def truncate_cuts(data: np.ndarray, offsets: np.ndarray, id_offsets: np.ndarray,
 
 
 @dataclass
+class ChunkBatchResponse:
+    """every prompt cut into chunks of at most N tokens (TokenizerPluginClient.chunk_batch)"""
+    spans: np.ndarray            # uint32 [chunks, 2]: (begin, end) of every chunk within its prompt, always character boundaries
+    chunk_offsets: np.ndarray    # uint64 [n + 1]: prompt i's chunks are spans[chunk_offsets[i] .. chunk_offsets[i + 1]]
+    counts: np.ndarray           # uint32: tokens of every whole prompt
+
+
+def _chunk_args(chunk_tokens, overlap_tokens) -> Tuple[int, int]:
+    ok = all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in (chunk_tokens, overlap_tokens))
+    if not ok or not 1 <= int(chunk_tokens) <= 0xFFFFFFFF or not 0 <= int(overlap_tokens) < int(chunk_tokens):
+        raise InvalidInput("chunk size must be an integer in 1 .. 2^32 - 1 and the overlap an integer in 0 .. chunk size - 1")
+    return int(chunk_tokens), int(overlap_tokens)
+
+
+def chunk_spans(data: np.ndarray, offsets: np.ndarray, id_offsets: np.ndarray, starts: np.ndarray, chunk_tokens: int,
+                overlap_tokens: int = 0) -> Tuple[np.ndarray, np.ndarray]:
+    """The chunking contract (include/cfbpe.h, cfbpe_chunk_batch) from every token's start: (spans uint32 [chunks, 2], chunk
+    offsets uint64 [n + 1]).  Windows of N = chunk_tokens tokens start every N - overlap_tokens tokens until one reaches the last
+    token; chunk k covers tokens [a, e) and its bytes are [F(a), F(e)), F(j) = the character start at or before token j's start,
+    F(c) = the prompt's length."""
+    n = len(offsets) - 1
+    step = chunk_tokens - overlap_tokens
+    spans, coffs = [], np.zeros(n + 1, dtype=np.uint64)
+    for i in range(n):
+        o, ln = int(offsets[i]), int(offsets[i + 1]) - int(offsets[i])
+        st = starts[int(id_offsets[i]):int(id_offsets[i + 1])].astype(np.int64)
+        c = len(st)
+
+        def floor(j):
+            if j >= c:
+                return ln
+            x = int(st[j])
+            while 0 < x < ln and data[o + x] & 0xC0 == 0x80:
+                x -= 1
+            return x
+        k = 0 if c == 0 else 1 if c <= chunk_tokens else 1 + (c - chunk_tokens + step - 1) // step
+        for q in range(k):
+            a = q * step
+            spans.append((floor(a), floor(min(a + chunk_tokens, c))))
+        coffs[i + 1] = coffs[i] + k
+    return (np.array(spans, dtype=np.uint32).reshape(-1, 2), coffs)
+
+
+@dataclass
 class CountTokensRequest:
     vocab: VocabRef
     bytes: np.ndarray
@@ -305,6 +349,19 @@ class TokenizerPluginClient:
             raise ServiceUnavailable("the tokenizer plugin does not return token starts")
         cut, kept = truncate_cuts(req.bytes, req.offsets, r.offsets, r.starts, bud, tail)
         return TruncateBatchResponse(cut, kept, np.asarray(r.counts[:n], dtype=np.uint32))
+
+    def chunk_batch(self, ctx: SecurityContext, req: EncodeBatchRequest, chunk_tokens: int, overlap_tokens: int = 0) -> ChunkBatchResponse:
+        """Cut every prompt of `req` into chunks of at most chunk_tokens tokens that overlap by overlap_tokens, at character
+        boundaries of the whole prompt's encoding -- include/cfbpe.h, cfbpe_chunk_batch.  This default works on any plugin:
+        encode_batch with token starts, then the cuts on the host."""
+        n_tok, overlap = _chunk_args(chunk_tokens, overlap_tokens)
+        n = len(req.offsets) - 1
+        r = self.encode_batch(ctx, EncodeBatchRequest(req.vocab, req.bytes, req.offsets, req.vocabs_per_prompt, req.vocab_index,
+                                                      with_starts=True))
+        if r.starts is None:
+            raise ServiceUnavailable("the tokenizer plugin does not return token starts")
+        spans, coffs = chunk_spans(req.bytes, req.offsets, r.offsets, r.starts, n_tok, overlap)
+        return ChunkBatchResponse(spans, coffs, np.asarray(r.counts[:n], dtype=np.uint32))
 
 
 GTS_PLUGIN_SCHEMA = "gts.x.core.modkit.plugin.v1~x.llmgw.tokenizer.plugin.v1~"
@@ -535,6 +592,18 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
             raise _map_native(e) from e
         return TruncateBatchResponse(cut, kept, counts)
 
+    def chunk_batch(self, ctx: SecurityContext, req: EncodeBatchRequest, chunk_tokens: int, overlap_tokens: int = 0) -> ChunkBatchResponse:
+        """the device path (cfbpe_chunk_batch): the chunks are cut where the ids and starts are; only the spans, chunk offsets and
+        counts come back"""
+        n_tok, overlap = _chunk_args(chunk_tokens, overlap_tokens)
+        self._check_arrays(req)
+        vid = self._vocab_ids(req)
+        try:
+            spans, coffs, counts = self.ctx.chunk_batch(req.bytes, req.offsets, n_tok, overlap, vid)
+        except N.NativeError as e:
+            raise _map_native(e) from e
+        return ChunkBatchResponse(spans, coffs, counts)
+
     def close(self):
         self.ctx.close()
 
@@ -607,6 +676,19 @@ class LlmGatewayTokenizerService:
             b = data[int(offs[i]):int(offs[i + 1])].tobytes()
             c = int(r.cut[i])
             out.append(((b[c:] if tail else b[:c]).decode("utf-8"), int(r.kept[i]), int(r.counts[i])))
+        return out
+
+    def chunk(self, ctx: SecurityContext, model: str, texts: Sequence[str], max_tokens: int, overlap: int = 0) -> List[List[str]]:
+        """Split texts into chunks of at most max_tokens tokens that overlap by `overlap` tokens (a RAG splitter's chunk_size /
+        chunk_overlap, or an embedding endpoint's long inputs): per text, its chunk strings.  The cuts are at token boundaries of
+        the whole text's encoding, moved back to character boundaries, so every chunk is valid UTF-8; with no overlap the chunks
+        join back into the text.  Encoding a chunk again may give other tokens: BPE is not prefix-stable."""
+        data, offs = pack_texts(texts)
+        r = self._plugin().chunk_batch(ctx, EncodeBatchRequest(VocabRef(model), data, offs), max_tokens, overlap)
+        out = []
+        for i in range(len(texts)):
+            b = data[int(offs[i]):int(offs[i + 1])].tobytes()
+            out.append([b[int(x):int(y)].decode("utf-8") for x, y in r.spans[int(r.chunk_offsets[i]):int(r.chunk_offsets[i + 1])]])
         return out
 
     def count_tokens(self, ctx: SecurityContext, model: str, messages: Sequence[dict]) -> Usage:

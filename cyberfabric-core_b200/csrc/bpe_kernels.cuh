@@ -87,6 +87,8 @@ struct DeviceStatus {
     uint32_t bad_vocab;    // != 0: a prompt names a vocabulary id that is not loaded (device-path callers; the host paths check before)
     uint32_t defer_n;      // pieces K2b handed to K2c ...
     unsigned long long defer_parts;   // ... and their parts at hand-over
+    uint64_t n_chunks;     // chunk calls: chunks of this (sub-)batch (written by chunk_scan) ...
+    uint64_t chunk_end;    // ... and chunk_base + n_chunks, as tok_end for the tokens (kept last: the fields above keep their offsets)
 };
 
 // K2a's lists of the short pieces that need the merge loop, one per length class (worst-case capacities: a class with
@@ -1846,6 +1848,93 @@ truncate_long_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ ids,
     if (atomicAdd(&tv.kept[p], 1u) + 2 == parts) {            // the last of parts 1 .. parts - 1: every sum is in
         __threadfence();
         truncate_finish(b, T, ids, r0, t, tv, p, atomicAdd(&tv.cut[p], 0u));
+    }
+}
+
+// Chunking (pipeline.cuh, enqueue_emit): prompt p with c tokens is cut into windows of n tokens that start every step = n - overlap
+// tokens -- none for c = 0, one for c <= n, else 1 + ceil((c - n) / step), as LangChain's split_text_on_tokens.  Chunk k covers
+// tokens [a, e), a = k x step, e = min(a + n, c); its bytes are [F(a), F(e)), F(j) = the largest character start at or before the
+// start of token j (the starts of starts_emit), F(c) = len.  Both ends take the same snap, so the chunks are valid UTF-8 and, with
+// no overlap, tile the prompt.
+//   chunk_scan: one CTA, as tile_scan: every prompt's chunk count from out_offsets, their exclusive scan after *base (the chunks of
+//               the sub-batches before, nullable) into offsets[0 .. n_prompts], and the (sub-)batch's total into the status
+//               (n_chunks, chunk_end), where the next sub-batch of a pipelined call continues
+//   chunk_emit: a thread per chunk, the grid striding over the status's range.  It finds its prompt in offsets (binary search),
+//               reads two starts, moves each back over at most 3 continuation bytes and writes the pair; consecutive threads
+//               write consecutive pairs.  Chunks at or past cap are not written.
+struct ChunkView {
+    uint32_t n, step;           // chunk_tokens, chunk_tokens - overlap_tokens
+    uint64_t* offsets;          // out: the (sub-)batch's chunk offsets [n_prompts + 1], ranks in the call's chunk stream
+    const uint64_t* base;       // nullable: the chunks of the sub-batches before this one (the previous status's chunk_end)
+    uint32_t* begin;            // out: span begins ...
+    uint32_t* end;              // ... and ends.  stride 2 (end = begin + 1): the pairs of the caller's spans, chunk q at 2q;
+    uint32_t stride;            //   stride 1: two arrays, indexed by q minus the (sub-)batch's first chunk (a host call's staging)
+    uint64_t cap;               // chunks at or past cap are not written
+};
+__device__ __forceinline__ uint64_t chunk_count(uint64_t c, uint32_t n, uint32_t step) {
+    return c == 0 ? 0 : c <= n ? 1 : 1 + (c - n + step - 1) / step;
+}
+__device__ __forceinline__ uint64_t prompt_chunks(const uint64_t* __restrict__ out_offsets, const ChunkView& cv, uint32_t p) {
+    return chunk_count(out_offsets[p + 1] - out_offsets[p], cv.n, cv.step);
+}
+// the largest character start at or before x in s[0 .. len) (len for x >= len): at most 3 continuation bytes back
+__device__ __forceinline__ uint32_t char_floor(const uint8_t* s, uint32_t len, uint32_t x) {
+    if (x >= len) return len;
+    while (x > 0 && (s[x] & 0xC0u) == 0x80u) --x;
+    return x;
+}
+
+__global__ void __launch_bounds__(1024)
+chunk_scan_kernel(BatchView b, const uint64_t* __restrict__ out_offsets, ChunkView cv, DeviceStatus* status) {
+    __shared__ uint64_t s_warp[32];
+    const uint64_t base0 = cv.base ? *cv.base : 0;
+    const uint32_t n = b.n_prompts;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarps = (blockDim.x + 31) >> 5;
+    const uint32_t per = ((n + nwarps - 1) / nwarps + 31u) & ~31u;          // prompts per warp, a multiple of 32
+    const uint32_t lo = wid * per < n ? wid * per : n;
+    const uint32_t hi = lo + per < n ? lo + per : n;
+    uint64_t sum = 0;
+    for (uint32_t i = lo + lane; i < hi; i += 32) sum += prompt_chunks(out_offsets, cv, i);
+#pragma unroll
+    for (uint32_t d = 16; d; d >>= 1) sum += __shfl_xor_sync(kFull, sum, d);
+    if (lane == 0) s_warp[wid] = sum;
+    __syncthreads();
+    uint64_t carry = base0, total = 0;
+    for (uint32_t w = 0; w < nwarps; ++w) { const uint64_t v = s_warp[w]; if (w < wid) carry += v; total += v; }
+    for (uint32_t i0 = lo; i0 < hi; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        const uint64_t v = i < hi ? prompt_chunks(out_offsets, cv, i) : 0;
+        uint64_t x = v;
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) { const uint64_t o = __shfl_up_sync(kFull, x, d); if (lane >= d) x += o; }
+        if (i < hi) cv.offsets[i] = carry + x - v;
+        carry += __shfl_sync(kFull, x, 31);
+    }
+    if (threadIdx.x == 0) { cv.offsets[n] = base0 + total; status->n_chunks = total; status->chunk_end = base0 + total; }
+}
+
+__global__ void __launch_bounds__(256)
+chunk_emit_kernel(BatchView b, const uint64_t* __restrict__ out_offsets, const uint32_t* __restrict__ starts, ChunkView cv,
+                  const DeviceStatus* status) {
+    const uint64_t q1 = status->chunk_end, q0 = q1 - status->n_chunks;
+    const uint64_t lim = q1 < cv.cap ? q1 : cv.cap;
+    const bool pairs = cv.stride == 2 && (reinterpret_cast<uintptr_t>(cv.begin) & 7u) == 0;   // one 8-byte store a chunk
+    for (uint64_t q = q0 + static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; q < lim; q += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+        const uint32_t p = find_prompt(cv.offsets, b.n_prompts, q);
+        const uint64_t r0 = out_offsets[p], o = b.offsets[p];
+        const uint64_t c = out_offsets[p + 1] - r0;
+        const uint64_t a = (q - cv.offsets[p]) * cv.step, e = a + cv.n < c ? a + cv.n : c;
+        const uint32_t len = static_cast<uint32_t>(b.offsets[p + 1] - o);
+        const uint8_t* s = b.bytes + o;
+        const uint32_t lo = char_floor(s, len, starts[r0 + a]);
+        const uint32_t hi = e < c ? char_floor(s, len, starts[r0 + e]) : len;
+        if (pairs) {
+            *reinterpret_cast<uint2*>(cv.begin + 2 * q) = uint2{lo, hi};
+        } else {
+            const uint64_t j = cv.stride == 2 ? 2 * q : q - q0;
+            cv.begin[j] = lo;
+            cv.end[j] = hi;
+        }
     }
 }
 

@@ -134,6 +134,8 @@ struct Lane {
     uint32_t* d_out_starts = nullptr;    // host calls with token starts: [max_bytes + 1], allocated on the lane's first such call
     uint32_t* d_trunc = nullptr;         // host truncate calls: budgets, cuts, kept counts [3 x (max_prompts + 1)], allocated on the
                                          // lane's first such call
+    uint64_t* d_chunk_offs = nullptr;    // host chunk calls: chunk offsets in the layout of d_out_offsets, then the shard chunk totals
+                                         // of a multi-device call [CFBPE_MAX_DEVICES]; allocated on the lane's first such call
     Workspace ws{};
     DeviceStatus* h_status = nullptr;  // pinned
     ProfEvents prof{};
@@ -390,6 +392,41 @@ int download_cuts(cfbpe_ctx* ctx, Lane* ln, const TruncateArgs& t, uint32_t p0, 
     return CFBPE_OK;
 }
 
+// A host chunk call (cfbpe_chunk_batch): n tokens a chunk, a new chunk every step tokens; spans (room for cap chunks) and chunk
+// offsets out.  The ids and starts it needs go to the lane's buffers and are never downloaded.  sub_end (nullable, a shard of a
+// multi-device call): gets every sub-batch's chunk_end (shard-local ranks), for the downloads after the shards' totals are known.
+struct ChunkArgs { uint32_t n, step; uint32_t* spans; uint64_t cap; uint64_t* offsets; uint64_t* sub_end; };
+
+// the lane's chunk-offset buffer (host chunk calls), allocated on its first such call: a context that never chunks keeps the
+// footprint it had.  The caller has selected the lane's device.
+int ensure_chunk_lane(cfbpe_ctx* ctx, Lane* ln) {
+    if (ln->d_chunk_offs) return CFBPE_OK;
+    if (dmalloc(&ln->d_chunk_offs, lane_offsets_alloc(ctx->max_prompts, kMaxPipeChunks) + CFBPE_MAX_DEVICES) != cudaSuccess) {
+        cudaGetLastError(); ln->d_chunk_offs = nullptr;
+        return fail(ctx, CFBPE_ENOMEM, "no device memory for the chunk offsets");
+    }
+    return CFBPE_OK;
+}
+uint64_t* lane_chunk_totals(cfbpe_ctx* ctx, Lane* ln) { return ln->d_chunk_offs + lane_offsets_alloc(ctx->max_prompts, kMaxPipeChunks); }
+// a host call's chunks of the (sub-)batch with workspace w and offsets at q0: the offsets to the lane's buffer, the spans staged
+// in w's per-byte scratch, which is dead once the ids are out (begins in ids_by_pos, ends in dense.by_piece: a (sub-)batch has
+// no more chunks than tokens and no more tokens than bytes); base: the previous sub-batch's chunk_end, or nullptr
+ChunkView lane_chunk_view(Lane* ln, const Workspace& w, uint64_t q0, const uint64_t* base, const ChunkArgs& c) {
+    return ChunkView{c.n, c.step, ln->d_chunk_offs + q0, base, w.ids_by_pos, w.dense.by_piece, 1u, UINT64_MAX};
+}
+// chunks [first, first + count) of the call, staged by lane_chunk_view in w, to their (begin, end) pairs in spans
+int download_spans(cfbpe_ctx* ctx, const Workspace& w, uint32_t* spans, uint64_t first, uint64_t count, cudaStream_t s) {
+    if (!count) return CFBPE_OK;
+    CK(cudaMemcpy2DAsync(spans + 2 * first, 2 * sizeof(uint32_t), w.ids_by_pos, sizeof(uint32_t), sizeof(uint32_t), count, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpy2DAsync(spans + 2 * first + 1, 2 * sizeof(uint32_t), w.dense.by_piece, sizeof(uint32_t), sizeof(uint32_t), count, cudaMemcpyDeviceToHost, s));
+    return CFBPE_OK;
+}
+// the call's `need` chunks exceed chunk_cap; the host learns it in offsets[n]
+int fail_chunk_nospace(cfbpe_ctx* ctx, uint64_t need, uint64_t* offsets, uint32_t n) {
+    if (offsets) offsets[n] = need;
+    return fail(ctx, CFBPE_ENOSPC, "chunk_cap too small: need " + std::to_string(need) + " chunks");
+}
+
 // an asynchronous device-path call may still own the lane's workspace: wait for it (the caller has selected the lane's device)
 int wait_for_device_call(cfbpe_ctx* ctx, Lane* ln) {
     if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }
@@ -414,10 +451,13 @@ int upload_batch(cfbpe_ctx* ctx, Lane* ln, uint32_t n, const uint8_t* bytes, con
 // defer != nullptr (a shard of a multi-device call): nothing is downloaded here -- ids, offsets and counts stay in the lane's device
 // buffers (dense, shard-local ranks: sub-batch k's offsets at d_out_offsets + sub_batch_offsets_at(p_k, k)) and *defer gets the
 // shard's token total.  trunc (nullable): a truncate call; its cuts and kept counts are final (per prompt, prompt-relative) and
-// are downloaded under `defer` too.
+// are downloaded under `defer` too.  chunk (nullable): a chunk call; chunk offsets chain across the sub-batches on the device as
+// token ranks do (DeviceStatus::chunk_end), so sub-batch k's tile_scan waits for k - 1's whole back stage rather than its scan.
+// Under `defer` its offsets and spans stay on the device and chunk->sub_end gets every sub-batch's chunk_end.
 int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, int G, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
                        const uint8_t* vocab_ids, uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
-                       bool want_ids, uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out, const TruncateArgs* trunc) {
+                       bool want_ids, uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out, const TruncateArgs* trunc,
+                       const ChunkArgs* chunk) {
     // ---- cut
     uint32_t cut[kMaxPipeChunks + 1];
     const int nc = plan_sub_batches(offsets, n, total, ctx->pipe_chunk, kMaxPipeChunks, cut);
@@ -490,10 +530,13 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (trace) CK(cudaEventRecord(ln->trace[k][7], ss));
         if (k) CK(cudaStreamWaitEvent(ss, prev->ev_chain[k - 1], 0));    // token ranks chain through DeviceStatus::tok_end: only the scan waits
         enqueue_scan(b, w, ss, static_cast<ProfEvents*>(nullptr), k ? &prev->d_status_arr[k - 1].tok_end : nullptr);   // (G > 1: a peer pointer)
-        CK(cudaEventRecord(ln->ev_chain[k], ss));
+        if (!chunk) CK(cudaEventRecord(ln->ev_chain[k], ss));
         const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, p0) : TruncateView{};
+        const ChunkView cv = chunk ? lane_chunk_view(ln, w, q0, k ? &prev->d_status_arr[k - 1].chunk_end : nullptr, *chunk) : ChunkView{};
         enqueue_emit(b, w, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets + q0, ln->d_out_counts + p0,
-                     ss, static_cast<ProfEvents*>(nullptr), out_starts ? ln->d_out_starts : nullptr, &dv->vs, trunc ? &tv : nullptr);
+                     ss, static_cast<ProfEvents*>(nullptr), (out_starts || chunk) ? ln->d_out_starts : nullptr, &dv->vs, trunc ? &tv : nullptr,
+                     chunk ? &cv : nullptr);
+        if (chunk) CK(cudaEventRecord(ln->ev_chain[k], ss));       // (the chunk scan read the previous chunk_end: the chain ends here)
         CK(cudaGetLastError());
         status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr + k, ln->h_status_arr + k);
         CK(cudaEventRecord(ln->ev_done[k], ss));
@@ -501,7 +544,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
     }
     // ---- trail the kernels with the downloads
     int err = CFBPE_OK;
-    uint64_t tok_total = 0;
+    uint64_t tok_total = 0, chunk_total = 0;
     for (int k = 0; k < nc; ++k) {
         Lane* const ln = lns[k % G];
         if (G > 1) CK(cudaSetDevice(dvs[k % G]->device));
@@ -513,8 +556,17 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         const uint64_t base = st.tok_end - st.n_tokens;
         tok_total = st.tok_end;
         if (!err && trunc) { const int rc = download_cuts(ctx, ln, *trunc, p0, nk, ds); if (rc) return rc; }
+        if (chunk) { chunk_total = st.chunk_end; if (chunk->sub_end) chunk->sub_end[k] = st.chunk_end; }
         if (err || defer) continue;
         if (no_copy) continue;
+        if (chunk) {
+            const uint64_t q0 = sub_batch_offsets_at(p0, k);
+            CK(cudaMemcpyAsync(chunk->offsets + p0, ln->d_chunk_offs + q0, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
+            if (st.chunk_end <= chunk->cap) {
+                const Workspace w = slice_workspace(ln->ws, offsets[p0], offsets[p1] - offsets[p0], static_cast<uint32_t>(k));
+                if (const int rc = download_spans(ctx, w, chunk->spans, st.chunk_end - st.n_chunks, st.n_chunks, ds)) return rc;
+            }
+        }
         if (want_ids && out_ids && st.tok_end <= out_cap && st.n_tokens)
             CK(cudaMemcpyAsync(out_ids + base, ln->d_out_ids + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (out_starts && st.tok_end <= out_cap && st.n_tokens)      // (prompt-relative: the same ranks and base as the ids)
@@ -545,6 +597,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
     if (err) return err;
     if (defer) { *defer = tok_total; if (cut_out) { std::memcpy(cut_out, cut, sizeof(uint32_t) * (nc + 1)); *nc_out = nc; } return CFBPE_OK; }
     if (want_ids && tok_total > out_cap) return fail_nospace(ctx, tok_total, out_offsets, n);
+    if (chunk && chunk_total > chunk->cap) return fail_chunk_nospace(ctx, chunk_total, chunk->offsets, n);
     return CFBPE_OK;
 }
 
@@ -552,18 +605,22 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
 // defer / cut_out / nc_out: see run_host_pipelined; the one-shot path under `defer` leaves everything on the device as ONE sub-batch.
 // out_starts != nullptr: the tokens' starts too (in ln->d_out_starts, beside the ids; under `defer` it is only a flag).
 // trunc != nullptr: a truncate call (the ids stay in the lane; the cuts and kept counts are downloaded, under `defer` too).
+// chunk != nullptr: a chunk call (the ids and starts stay in the lane; the chunk offsets and spans are downloaded, except under
+// `defer`, where chunk->sub_end[0] gets the chunk total).
 int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
              uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
-             uint64_t* defer = nullptr, uint32_t* cut_out = nullptr, int* nc_out = nullptr, const TruncateArgs* trunc = nullptr) {
+             uint64_t* defer = nullptr, uint32_t* cut_out = nullptr, int* nc_out = nullptr, const TruncateArgs* trunc = nullptr,
+             const ChunkArgs* chunk = nullptr) {
     CK(cudaSetDevice(dv->device));
     int rc = wait_for_device_call(ctx, ln);
-    if (!rc && out_starts) rc = ensure_starts_lane(ctx, ln);
+    if (!rc && (out_starts || chunk)) rc = ensure_starts_lane(ctx, ln);
     if (!rc && trunc) rc = ensure_truncate_lane(ctx, ln);
+    if (!rc && chunk) rc = ensure_chunk_lane(ctx, ln);
     if (rc) return rc;
     const bool profiling = ctx->profiling.load();
     if (!profiling && total >= ctx->pipe_min && n >= 2)
         return run_host_pipelined(ctx, &dv, &ln, 1, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                                  defer, cut_out, nc_out, trunc);
+                                  defer, cut_out, nc_out, trunc, chunk);
     cudaStream_t s = ln->stream;
     ProfEvents* prof = profiling ? &ln->prof : nullptr;
     if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); }
@@ -574,9 +631,11 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     if (prof) cudaEventRecord(prof->h2d[1], s);
 
     const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, 0) : TruncateView{};
+    const ChunkView cv = chunk ? lane_chunk_view(ln, ln->ws, 0, nullptr, *chunk) : ChunkView{};
     enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets,
                    ln->d_out_counts, static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, out_starts ? ln->d_out_starts : nullptr, trunc ? &tv : nullptr);
+                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, (out_starts || chunk) ? ln->d_out_starts : nullptr, trunc ? &tv : nullptr,
+                   chunk ? &cv : nullptr);
     CK(cudaGetLastError());
     if (prof) cudaEventRecord(prof->d2h[0], s);
     CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
@@ -584,11 +643,21 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     if (!defer) {
         if (out_offsets) CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
         if (out_counts && n) CK(cudaMemcpyAsync(out_counts, ln->d_out_counts, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        if (chunk) CK(cudaMemcpyAsync(chunk->offsets, ln->d_chunk_offs, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     }
     CK(cudaStreamSynchronize(s));
     const DeviceStatus st = *ln->h_status;
     if ((rc = fail_status(ctx, st))) return rc;
-    if (defer) { *defer = st.n_tokens; if (cut_out) { cut_out[0] = 0; cut_out[1] = n; *nc_out = 1; } return CFBPE_OK; }
+    if (defer) {
+        *defer = st.n_tokens;
+        if (cut_out) { cut_out[0] = 0; cut_out[1] = n; *nc_out = 1; }
+        if (chunk && chunk->sub_end) chunk->sub_end[0] = st.chunk_end;
+        return CFBPE_OK;
+    }
+    if (chunk) {
+        if (st.chunk_end > chunk->cap) return fail_chunk_nospace(ctx, st.chunk_end, chunk->offsets, n);
+        if ((rc = download_spans(ctx, ln->ws, chunk->spans, 0, st.chunk_end, s))) return rc;
+    }
     if (want_ids) {
         if (st.n_tokens > out_cap) return fail_nospace(ctx, st.n_tokens, out_offsets, n);
         if (out_ids && st.n_tokens) CK(cudaMemcpyAsync(out_ids, ln->d_out_ids, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
@@ -723,7 +792,7 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
 struct SpecialArgs { const uint8_t* const* modes; uint32_t* bad; };
 int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
                      uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
-                     const SpecialArgs* special = nullptr, const TruncateArgs* trunc = nullptr) {
+                     const SpecialArgs* special = nullptr, const TruncateArgs* trunc = nullptr, const ChunkArgs* chunk = nullptr) {
     const uint32_t G = static_cast<uint32_t>(ctx->devs.size());
     std::vector<uint32_t> lo(G + 1, 0);
     for (uint32_t d = 1; d < G; ++d) {      // first prompt whose start is >= d * total / G
@@ -735,7 +804,8 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     lo[G] = n;
     for (uint32_t d = 0; d < G; ++d)
         if (offsets[lo[d + 1]] - offsets[lo[d]] > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "a device's shard exceeds max_batch_bytes (one prompt is too large to balance)");
-    struct Shard { int rc = CFBPE_OK; std::string err; uint64_t tokens = 0; std::vector<uint64_t> local_offs; uint32_t cut[kMaxPipeChunks + 1]; int nc = 0; uint32_t bad[2] = {}; };
+    struct Shard { int rc = CFBPE_OK; std::string err; uint64_t tokens = 0; std::vector<uint64_t> local_offs; uint32_t cut[kMaxPipeChunks + 1]; int nc = 0; uint32_t bad[2] = {};
+                   uint64_t chunk_end[kMaxPipeChunks] = {}; };
     std::vector<Shard> sh(G);
     std::vector<std::unique_ptr<LaneLock>> locks(G);
     for (uint32_t d = 0; d < G; ++d) locks[d].reset(new LaneLock(ctx->devs[d].get()));
@@ -754,9 +824,10 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
                 s.cut[0] = 0; s.cut[1] = nd; s.nc = 1;
             } else {
                 const TruncateArgs shard_trunc = trunc ? truncate_from(*trunc, p0) : TruncateArgs{};
+                const ChunkArgs shard_chunk = chunk ? ChunkArgs{chunk->n, chunk->step, nullptr, UINT64_MAX, nullptr, s.chunk_end} : ChunkArgs{};
                 s.rc = run_lane(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
                                 nullptr, out_starts, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc,
-                                trunc ? &shard_trunc : nullptr);
+                                trunc ? &shard_trunc : nullptr, chunk ? &shard_chunk : nullptr);
             }
             if (s.rc) s.err = tl_err;
         });
@@ -785,6 +856,10 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     uint64_t grand = 0;
     for (uint32_t d = 0; d < G; ++d) grand += sh[d].tokens;
     const bool fits = !want_ids || grand <= out_cap;
+    // a chunk call: every shard's chunk total is on the host already (its last sub-batch's chunk_end, shard-local)
+    std::vector<uint64_t> chunk_tot(G, 0), chunk_base(G + 1, 0);
+    for (uint32_t d = 0; d < G && chunk; ++d) { chunk_tot[d] = sh[d].nc ? sh[d].chunk_end[sh[d].nc - 1] : 0; chunk_base[d + 1] = chunk_base[d] + chunk_tot[d]; }
+    const bool chunks_fit = !chunk || chunk_base[G] <= chunk->cap;
     {
         std::vector<std::thread> th;
         for (uint32_t d = 0; d < G; ++d) th.emplace_back([&, d]() {
@@ -795,6 +870,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             ck(cudaSetDevice(ctx->devs[d]->device), "cudaSetDevice");
             cudaStream_t st = ln->stream;
             ck(cudaMemcpyAsync(ln->h_totals, ln->d_totals, sizeof(uint64_t) * G, cudaMemcpyDeviceToHost, st), "totals download");
+            if (chunk) ck(cudaMemcpyAsync(lane_chunk_totals(ctx, ln), chunk_tot.data(), sizeof(uint64_t) * G, cudaMemcpyHostToDevice, st), "chunk totals upload");
             for (int k = 0; k < s.nc; ++k) {
                 const uint32_t q0 = s.cut[k], nk = s.cut[k + 1] - s.cut[k];
                 const bool last = (k + 1 == s.nc) && (d + 1 == G);
@@ -804,6 +880,20 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
                 rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(src, cnt, ln->d_totals, d);
                 if (out_offsets) ck(cudaMemcpyAsync(out_offsets + p0 + q0, src, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st), "offsets download");
                 if (out_counts && nk) ck(cudaMemcpyAsync(out_counts + p0 + q0, ln->d_out_counts + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "counts download");
+                if (chunk) {      // chunk offsets: rebased as the token offsets, by the chunk totals of the shards before; spans: prompt-relative
+                    uint64_t* csrc = ln->d_chunk_offs + sub_batch_offsets_at(q0, k);
+                    rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(csrc, cnt, lane_chunk_totals(ctx, ln), d);
+                    ck(cudaMemcpyAsync(chunk->offsets + p0 + q0, csrc, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st), "chunk offsets download");
+                    const uint64_t c0 = k ? s.chunk_end[k - 1] : 0, c1 = s.chunk_end[k];
+                    if (chunks_fit && c1 > c0) {
+                        const uint64_t o0 = s.local_offs[q0];
+                        const Workspace w = slice_workspace(ln->ws, o0, s.local_offs[q0 + nk] - o0, static_cast<uint32_t>(k));
+                        ck(cudaMemcpy2DAsync(chunk->spans + 2 * (chunk_base[d] + c0), 2 * sizeof(uint32_t), w.ids_by_pos, sizeof(uint32_t), sizeof(uint32_t),
+                                             c1 - c0, cudaMemcpyDeviceToHost, st), "span begins download");
+                        ck(cudaMemcpy2DAsync(chunk->spans + 2 * (chunk_base[d] + c0) + 1, 2 * sizeof(uint32_t), w.dense.by_piece, sizeof(uint32_t), sizeof(uint32_t),
+                                             c1 - c0, cudaMemcpyDeviceToHost, st), "span ends download");
+                    }
+                }
             }
             ck(cudaStreamSynchronize(st), "stream sync");
             uint64_t base = 0;
@@ -816,21 +906,23 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     }
     for (uint32_t d = 0; d < G; ++d) if (rcs[d]) return fail(ctx, rcs[d], errs[d]);
     if (!fits) return fail_nospace(ctx, grand, out_offsets, n);
+    if (!chunks_fit) return fail_chunk_nospace(ctx, chunk_base[G], chunk->offsets, n);
     return CFBPE_OK;
 }
 
-// shared body of encode_batch / encode_batch_starts / count_batch / truncate_batch (host buffers); out_starts: NULL but for
-// encode_batch_starts; trunc: NULL but for truncate_batch (which emits the ids into the lane, out_ids NULL, out_cap unlimited)
+// shared body of encode_batch / encode_batch_starts / count_batch / truncate_batch / chunk_batch (host buffers); out_starts: NULL
+// but for encode_batch_starts; trunc: NULL but for truncate_batch, chunk: NULL but for chunk_batch (both emit the ids into the lane,
+// out_ids NULL, out_cap unlimited)
 int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
              uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
-             const TruncateArgs* trunc = nullptr) {
+             const TruncateArgs* trunc = nullptr, const ChunkArgs* chunk = nullptr) {
     tl_err.clear();
     std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
     uint64_t total = 0;
     int rc = validate_batch(ctx, n, offsets, vocab_ids, &total);
     if (rc) return rc;
     if (total && !bytes) return fail(ctx, CFBPE_EINVAL, "bytes is NULL");
-    if (want_ids && !trunc && (!out_offsets || (!out_ids && out_cap))) return fail(ctx, CFBPE_EINVAL, "output pointer is NULL");
+    if (want_ids && !trunc && !chunk && (!out_offsets || (!out_ids && out_cap))) return fail(ctx, CFBPE_EINVAL, "output pointer is NULL");
     if (ctx->devs.size() > 1 && n >= ctx->devs.size() && !ctx->profiling.load()) {
         // Two ways over several devices.  When every device can hold the whole batch (and the devices see each other's memory):
         // the sub-batches of ONE pipelined call go round-robin over the devices -- uploads, kernels and downloads of all devices
@@ -845,20 +937,22 @@ int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* o
                 lns[g] = locks[g]->ln;
                 CK(cudaSetDevice(dvs[g]->device));
                 rc = wait_for_device_call(ctx, lns[g]);
-                if (!rc && out_starts) rc = ensure_starts_lane(ctx, lns[g]);
+                if (!rc && (out_starts || chunk)) rc = ensure_starts_lane(ctx, lns[g]);
                 if (!rc && trunc) rc = ensure_truncate_lane(ctx, lns[g]);
+                if (!rc && chunk) rc = ensure_chunk_lane(ctx, lns[g]);
                 if (rc) return rc;
             }
             return run_host_pipelined(ctx, dvs, lns, G, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                                      nullptr, nullptr, nullptr, trunc);
+                                      nullptr, nullptr, nullptr, trunc, chunk);
         }
-        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total, nullptr, trunc);
+        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total, nullptr, trunc,
+                                chunk);
     }
     if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds max_batch_bytes of this context");
     DeviceCtx* dv = ctx->devs[0].get();
     LaneLock lk(dv);
     return run_lane(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                    nullptr, nullptr, nullptr, trunc);
+                    nullptr, nullptr, nullptr, trunc, chunk);
 }
 
 
@@ -940,6 +1034,7 @@ void destroy_lane(Lane* ln) {
     free_special_lane(ln);
     cudaFree(ln->d_bytes); cudaFree(ln->d_offsets); cudaFree(ln->d_vocab_ids);
     cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts); cudaFree(ln->d_out_starts); cudaFree(ln->d_trunc);
+    cudaFree(ln->d_chunk_offs);
     for_each_ws_buffer(ln->ws, [](auto*& p, WsKind) { cudaFree(p); });
     cudaFree(ln->ws.status);
     cudaFree(ln->d_dec_sums); cudaFree(ln->d_dec_base); cudaFree(ln->d_totals);
@@ -1189,6 +1284,26 @@ int run_device_truncate(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_byt
     });
 }
 
+// shared body of chunk_batch_device: the ids, offsets and starts go to the lane's buffers (max_batch_bytes ids fit); the status
+// carries the chunk count where device_call and cfbpe_device_status look for the id count, so ENOSPC is checked against chunk_cap
+int run_device_chunk(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                     const uint8_t* d_vocab_ids, uint32_t chunk_tokens, uint32_t overlap_tokens, uint32_t* d_out_spans, uint64_t chunk_cap,
+                     uint64_t* d_out_chunk_offsets, uint32_t* d_out_counts, uint64_t* n_chunks, void* stream) {
+    return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_chunk_offsets, true, chunk_cap, n_chunks, stream, true,
+                       [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents* prof) {
+        if (const int rc = ensure_starts_lane(ctx, ln)) return rc;
+        const ChunkView cv{chunk_tokens, chunk_tokens - overlap_tokens, d_out_chunk_offsets, nullptr, d_out_spans, d_out_spans + 1, 2u, chunk_cap};
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets, d_out_counts,
+                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
+                       ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, ln->d_out_starts, nullptr, &cv);
+        CK(cudaGetLastError());
+        static_assert(offsetof(DeviceStatus, chunk_end) == offsetof(DeviceStatus, n_chunks) + sizeof(uint64_t) &&
+                      offsetof(DeviceStatus, tok_end) == offsetof(DeviceStatus, n_tokens) + sizeof(uint64_t), "count, then end");
+        CK(cudaMemcpyAsync(&ln->ws.status->n_tokens, &ln->ws.status->n_chunks, 2 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+        return CFBPE_OK;
+    });
+}
+
 }  // namespace
 
 // Every entry point that selects a device puts the caller's current device back on return: the library is a guest in the host
@@ -1380,6 +1495,17 @@ int cfbpe_truncate_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* byte
     return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, nullptr, nullptr, UINT64_MAX, nullptr, out_counts, true, &t);
 }
 
+int cfbpe_chunk_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                      uint32_t chunk_tokens, uint32_t overlap_tokens, uint32_t* out_spans, uint64_t chunk_cap, uint64_t* out_chunk_offsets,
+                      uint32_t* out_counts) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (const char* e = chunk_args_error(chunk_tokens, overlap_tokens, out_spans, out_chunk_offsets)) return fail(ctx, CFBPE_EINVAL, e);
+    const ChunkArgs c{chunk_tokens, chunk_tokens - overlap_tokens, out_spans, chunk_cap, out_chunk_offsets, nullptr};
+    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, nullptr, nullptr, UINT64_MAX, nullptr, out_counts, true, nullptr, &c);
+}
+
 int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, const uint64_t* id_offsets,
                        const uint8_t* vocab_ids, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets) {
     DeviceGuard restore_device;
@@ -1462,6 +1588,17 @@ int cfbpe_truncate_batch_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_
     if (const char* e = truncate_args_error(d_budgets, mode, d_out_cut, d_out_kept)) return fail(ctx, CFBPE_EINVAL, e);
     return run_device_truncate(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_budgets, mode, d_out_cut, d_out_kept, d_out_counts,
                                stream);
+}
+
+int cfbpe_chunk_batch_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                             const uint8_t* d_vocab_ids, uint32_t chunk_tokens, uint32_t overlap_tokens, uint32_t* d_out_spans, uint64_t chunk_cap,
+                             uint64_t* d_out_chunk_offsets, uint32_t* d_out_counts, uint64_t* n_chunks, void* stream) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (const char* e = chunk_args_error(chunk_tokens, overlap_tokens, d_out_spans, d_out_chunk_offsets)) return fail(ctx, CFBPE_EINVAL, e);
+    return run_device_chunk(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, chunk_tokens, overlap_tokens, d_out_spans, chunk_cap,
+                            d_out_chunk_offsets, d_out_counts, n_chunks, stream);
 }
 
 int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* ids) {

@@ -133,6 +133,14 @@ inline const char* truncate_args_error(const uint32_t* budgets, uint32_t mode, c
     return nullptr;
 }
 
+// the checks of a chunk call's own arguments (cfbpe_chunk_batch and its device form): the error, or nullptr
+inline const char* chunk_args_error(uint32_t chunk_tokens, uint32_t overlap_tokens, const uint32_t* spans, const uint64_t* chunk_offsets) {
+    if (chunk_tokens == 0) return "chunk_tokens must be at least 1";
+    if (overlap_tokens >= chunk_tokens) return "overlap_tokens must be less than chunk_tokens";
+    if (!spans || !chunk_offsets) return "out_spans and out_chunk_offsets are required";
+    return nullptr;
+}
+
 // K2b CTAs per SM (long_grid = 4 x SM count).  8 x 128 threads x 64 registers is the whole register file of an SM: the
 // short-piece kernels on the other stream then wait for K2b instead of running beside it.
 #ifndef CFBPE_LONG_CTAS
@@ -253,10 +261,13 @@ inline void enqueue_scan(const BatchView& b, const Workspace& w, Stream stream, 
 // The dense-id tile arrays are free once the ids are out (the tiles of 2048 tokens are no more than the 2 KiB piece tiles).
 // trunc (nullable; only with out_ids, and then vs too): every prompt's cut to its token budget, from the ids where they are
 // (truncate_kernel, and truncate_long_kernel for the prompts with more ids to sum than one warp takes).
+// chunk (nullable; only with out_starts): every prompt's chunks of chunk->n tokens, from the starts (chunk_scan, then chunk_emit
+// over a grid of at most kChunkEmitCtas CTAs; a (sub-)batch has no more chunks than bytes).
+constexpr uint32_t kChunkEmitCtas = 1024;
 template <typename Stream, typename Prof>
 inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
                          uint32_t* out_counts, Stream stream, Prof* prof, uint32_t* out_starts = nullptr, const VocabSet* vs = nullptr,
-                         const TruncateView* trunc = nullptr) {
+                         const TruncateView* trunc = nullptr, const ChunkView* chunk = nullptr) {
     CFBPE_MARK(prof, K_EMIT, stream, true);
     if (b.total_bytes && out_ids) {
         CFBPE_LAUNCH(emit_compact_kernel, n_scan_tiles(b.total_bytes), 256, stream, w.tok_bits, w.piece_bits, n_flag_words(b.total_bytes), w.tile_base,
@@ -280,25 +291,34 @@ inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_i
             CFBPE_LAUNCH(truncate_long_kernel, static_cast<unsigned>((n_chunks + 7) / 8), 256, stream, b, *vs, out_ids, out_offsets, *trunc);
         }
     }
+    if (out_ids && out_starts && chunk) {
+        CFBPE_LAUNCH(chunk_scan_kernel, 1u, 1024, stream, b, out_offsets, *chunk, w.status);
+        if (b.total_bytes) {
+            const uint64_t ctas = (b.total_bytes + 255) / 256;
+            CFBPE_LAUNCH(chunk_emit_kernel, static_cast<unsigned>(ctas < kChunkEmitCtas ? ctas : kChunkEmitCtas), 256, stream,
+                         b, out_offsets, static_cast<const uint32_t*>(out_starts), *chunk, static_cast<const DeviceStatus*>(w.status));
+        }
+    }
 }
 template <typename Stream, typename Prof>
 inline void enqueue_back(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
                          uint32_t* out_counts, Stream stream, Prof* prof, const uint64_t* token_base, uint32_t* out_starts = nullptr,
-                         const VocabSet* vs = nullptr, const TruncateView* trunc = nullptr) {
+                         const VocabSet* vs = nullptr, const TruncateView* trunc = nullptr, const ChunkView* chunk = nullptr) {
     enqueue_count(b, w, stream, prof);
     enqueue_scan(b, w, stream, prof, token_base);
-    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs, trunc);
+    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs, trunc, chunk);
 }
 
 // The whole path.  `aux` / `aux2` are streams of their own for the two long-piece kernels (pass the main stream to run everything
 // in order); CFBPE_FORK / CFBPE_JOIN order them.  out_ids may be nullptr (count only); out_starts (nullable, with out_ids): the
-// tokens' byte offsets within their prompts; trunc (nullable, with out_ids): the prompts' cuts to their token budgets.  Everything
-// is asynchronous.
+// tokens' byte offsets within their prompts; trunc (nullable, with out_ids): the prompts' cuts to their token budgets; chunk
+// (nullable, with out_starts): the prompts' chunks.  Everything is asynchronous.
 template <typename Stream, typename Prof, typename Ev>
 inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTables& uc, const Workspace& w,
                            uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
                            uint32_t long_grid, Stream stream, Stream aux, Stream aux2, Ev ev_fork, Ev ev_join, Ev ev_join2, Prof* prof,
-                           const uint64_t* token_base = nullptr, uint32_t* out_starts = nullptr, const TruncateView* trunc = nullptr) {
+                           const uint64_t* token_base = nullptr, uint32_t* out_starts = nullptr, const TruncateView* trunc = nullptr,
+                           const ChunkView* chunk = nullptr) {
     enqueue_split(b, vs, uc, w, stream, prof, long_grid / 4);
     CFBPE_FORK(stream, aux2, ev_fork);
     enqueue_list(b, vs, w, long_grid, aux2, prof);
@@ -307,7 +327,7 @@ inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTable
     enqueue_short(b, vs, w, long_grid, stream, prof);
     CFBPE_JOIN(stream, aux, ev_join);
     CFBPE_JOIN(stream, aux2, ev_join2);
-    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base, out_starts, &vs, trunc);
+    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base, out_starts, &vs, trunc, chunk);
 }
 
 }  // namespace cfbpe

@@ -197,6 +197,30 @@ CFBPE_API int cfbpe_truncate_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uin
                                    const uint8_t *vocab_ids, const uint32_t *budgets, uint32_t mode, uint32_t *out_cut,
                                    uint32_t *out_kept, uint32_t *out_counts);
 
+/* Cut every prompt into chunks of at most chunk_tokens = N tokens that overlap by overlap_tokens = S (N >= 1, S < N; step
+ * s = N - S): the chunk_size / chunk_overlap windows of a RAG splitter or of an embedding endpoint's long inputs.  For prompt i with
+ * bytes b, ids t_0 .. t_{c-1} (cfbpe_encode_batch) and token starts x_j (cfbpe_encode_batch_starts; x_c = len(b)):
+ *   chunks: 0 if c = 0, 1 if c <= N, else 1 + ceil((c - N) / s) -- LangChain's split_text_on_tokens: windows start at token 0, s,
+ *           2s, ... and stop at the first that reaches the last token;
+ *   chunk k covers tokens [a, e), a = k x s, e = min(a + N, c), and its text is b[F(a) .. F(e)): F(j) = the largest character
+ *           start <= x_j (the snap of CFBPE_TRUNCATE_HEAD), F(c) = len(b).
+ * Both ends take the same snap, so every chunk is valid UTF-8; with S = 0 the chunks tile the prompt (each ends where the next
+ * begins, the first begins at 0, the last ends at len(b)); chunk 0 ends where cfbpe_truncate_batch(HEAD, budget N) cuts.  A chunk
+ * is empty only when N is smaller than the number of byte tokens one character was split into (so N <= 3).  The boundaries are
+ * those of the WHOLE prompt's encoding, as for truncation: encoding a chunk again may give other ids.
+ * out_spans: 2 entries a chunk (begin, end; relative to the prompt), room for chunk_cap chunks; prompt i's chunks are
+ * out_chunk_offsets[i] .. out_chunk_offsets[i + 1] (n_prompts + 1 entries).  CFBPE_ENOSPC when the chunks exceed chunk_cap
+ * (out_chunk_offsets[n_prompts] = the chunks needed; no span is written).  Sum over the prompts of the chunk formula with c = the
+ * prompt's byte length always fits, because c <= len: a caller can size out_spans once and never retry.  out_counts[i] = c, as
+ * cfbpe_count_batch (may be NULL).  Errors: chunk_tokens = 0, overlap_tokens >= chunk_tokens, a NULL out_spans or a NULL
+ * out_chunk_offsets is CFBPE_EINVAL; the rest as cfbpe_count_batch.  The ids and starts stay on the device.  Costs: the lane's
+ * token-start buffer (4 bytes per byte of max_batch_bytes, as cfbpe_encode_batch_starts) and 8 bytes per prompt of max_prompts
+ * for the chunk offsets, allocated on the lane's first such call (CFBPE_ENOMEM if that fails). */
+CFBPE_API int cfbpe_chunk_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
+                                const uint8_t *vocab_ids, uint32_t chunk_tokens, uint32_t overlap_tokens,
+                                uint32_t *out_spans /* 2 per chunk: begin, end; prompt-relative */, uint64_t chunk_cap,
+                                uint64_t *out_chunk_offsets /* n_prompts + 1 */, uint32_t *out_counts /* may be NULL */);
+
 /* Decode (SURVEY.md section 8(f) item 2; tiktoken CoreBPE.decode_bytes): out_bytes = the concatenation of the tokens' bytes.
  * ids: the packed token ids of n_seqs sequences, id_offsets[n_seqs + 1] their boundaries (in ids), vocab_ids[n_seqs] or NULL.
  * out_offsets[n_seqs + 1]: byte boundaries of the decoded sequences in out_bytes.  CFBPE_ENOSPC if out_cap is too small
@@ -266,6 +290,16 @@ CFBPE_API int cfbpe_encode_batch_starts_device(cfbpe_ctx *ctx, uint32_t n_prompt
 CFBPE_API int cfbpe_truncate_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
                                           const uint64_t *d_offsets, const uint8_t *d_vocab_ids, const uint32_t *d_budgets, uint32_t mode,
                                           uint32_t *d_out_cut, uint32_t *d_out_kept, uint32_t *d_out_counts, void *stream);
+/* cfbpe_chunk_batch on device-resident buffers, enqueued on `stream` as cfbpe_encode_batch_device (d_bytes readable for 32 bytes
+ * past total_bytes).  d_out_spans (room for chunk_cap chunks), d_out_chunk_offsets and d_out_counts (may be NULL) are device
+ * memory.  n_chunks (host, may be NULL) is written after an internal stream sync, and then CFBPE_ENOSPC is returned when the
+ * chunks exceed chunk_cap; with n_chunks == NULL the call is fully asynchronous, d_out_chunk_offsets[n_prompts] holds the total,
+ * and CFBPE_ENOSPC, malformed UTF-8 and an unloaded vocabulary are reported by the next call that synchronises (or
+ * cfbpe_device_status).  Chunks at or past chunk_cap are not written. */
+CFBPE_API int cfbpe_chunk_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
+                                       const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t chunk_tokens,
+                                       uint32_t overlap_tokens, uint32_t *d_out_spans, uint64_t chunk_cap,
+                                       uint64_t *d_out_chunk_offsets, uint32_t *d_out_counts, uint64_t *n_chunks, void *stream);
 /* Synchronise `stream` and return the status word of the last device call (0, CFBPE_EILSEQ, CFBPE_ENOSPC). */
 CFBPE_API int cfbpe_device_status(cfbpe_ctx *ctx, void *stream);
 

@@ -91,6 +91,12 @@ extern "C" {
     pub fn cfbpe_truncate_batch_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64, d_offsets: *const u64,
                                        d_vocab_ids: *const u8, d_budgets: *const u32, mode: u32, d_out_cut: *mut u32, d_out_kept: *mut u32,
                                        d_out_counts: *mut u32, stream: *mut c_void) -> c_int;
+    pub fn cfbpe_chunk_batch(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64, vocab_ids: *const u8,
+                             chunk_tokens: u32, overlap_tokens: u32, out_spans: *mut u32, chunk_cap: u64, out_chunk_offsets: *mut u64,
+                             out_counts: *mut u32) -> c_int;
+    pub fn cfbpe_chunk_batch_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64, d_offsets: *const u64,
+                                    d_vocab_ids: *const u8, chunk_tokens: u32, overlap_tokens: u32, d_out_spans: *mut u32, chunk_cap: u64,
+                                    d_out_chunk_offsets: *mut u64, d_out_counts: *mut u32, n_chunks: *mut u64, stream: *mut c_void) -> c_int;
     pub fn cfbpe_decode_batch(ctx: *mut cfbpe_ctx, n_seqs: u32, ids: *const u32, id_offsets: *const u64,
                               vocab_ids: *const u8, out_bytes: *mut u8, out_cap: u64, out_offsets: *mut u64) -> c_int;
     pub fn cfbpe_encode_batch_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64,
@@ -133,6 +139,22 @@ pub struct Truncated {
     pub cut: Vec<u32>,
     pub kept: Vec<u32>,
     pub counts: Vec<u32>,
+}
+
+/// Result of [`Ctx::chunk_batch`]: every chunk's `[begin, end)` byte span within its prompt (always character boundaries), prompt
+/// i's chunks at `spans[chunk_offsets[i] .. chunk_offsets[i + 1]]`, and the tokens of every whole prompt.
+#[derive(Debug, Default)]
+pub struct Chunked {
+    pub spans: Vec<[u32; 2]>,
+    pub chunk_offsets: Vec<u64>,
+    pub counts: Vec<u32>,
+}
+
+/// The most chunks a batch can have (`include/cfbpe.h`, `cfbpe_chunk_batch`): the chunk formula with c = each prompt's byte length.
+pub fn chunk_bound(offsets: &[u64], chunk_tokens: u32, overlap_tokens: u32) -> u64 {
+    let step = u64::from(chunk_tokens.saturating_sub(overlap_tokens).max(1));
+    offsets.windows(2).map(|w| w[1] - w[0]).filter(|&len| len > 0)
+        .map(|len| 1 + len.saturating_sub(u64::from(chunk_tokens)).div_ceil(step)).sum()
 }
 
 /// Safe owner of one `cfbpe_ctx`.  The context is internally synchronised (header: "safe to call concurrently from several
@@ -324,6 +346,28 @@ impl Ctx {
         for v in [&mut out.cut, &mut out.kept, &mut out.counts] {
             v.truncate(n as usize);
         }
+        Ok(out)
+    }
+
+    /// Cut every prompt into chunks of at most `chunk_tokens` tokens that overlap by `overlap_tokens`, at character boundaries of
+    /// the whole prompt's encoding.  The output is sized by [`chunk_bound`], so the call never retries; only the spans, chunk offsets
+    /// and counts leave the device.
+    pub fn chunk_batch(&self, bytes: &[u8], offsets: &[u64], vocab_ids: Option<&[u8]>, chunk_tokens: u32, overlap_tokens: u32)
+        -> Result<Chunked, NativeError> {
+        let n = Self::check_inputs(bytes.len(), offsets, vocab_ids)?;
+        let cap = chunk_bound(offsets, chunk_tokens, overlap_tokens);
+        let mut spans = vec![[0u32; 2]; (cap as usize).max(1)];
+        let mut out = Chunked { spans: Vec::new(), chunk_offsets: vec![0; n as usize + 1], counts: vec![0; (n as usize).max(1)] };
+        // SAFETY: spans holds cap pairs, chunk_offsets n + 1 entries, counts at least n; none is retained.
+        let rc = unsafe {
+            cfbpe_chunk_batch(self.0.as_ptr(), n, bytes.as_ptr(), offsets.as_ptr(), vocab_ids.map_or(std::ptr::null(), <[u8]>::as_ptr),
+                              chunk_tokens, overlap_tokens, spans.as_mut_ptr().cast::<u32>(), cap, out.chunk_offsets.as_mut_ptr(),
+                              out.counts.as_mut_ptr())
+        };
+        self.check(rc)?;
+        spans.truncate(out.chunk_offsets[n as usize] as usize);
+        out.spans = spans;
+        out.counts.truncate(n as usize);
         Ok(out)
     }
 

@@ -6,7 +6,7 @@ use std::sync::Arc;
 use async_trait::async_trait;
 use cfbpe_sys::{Ctx, NativeError};
 use llm_gateway_sdk::{
-    CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens, TokenizerError,
+    ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens, TokenizerError,
     TokenizerPluginClient, TruncateBatchResponse, TruncateKeep, VocabRef,
 };
 use modkit_security::SecurityContext;
@@ -162,6 +162,22 @@ impl TokenizerPluginClient for Service {
             .map_err(|e| TokenizerError::Internal(e.to_string()))?
             .map_err(map_native)?;
         Ok(TruncateBatchResponse { cut: out.cut, kept: out.kept, counts: out.counts })
+    }
+
+    /// The device path (`cfbpe_chunk_batch`): the chunks are cut from the token starts where they are; no id or start leaves the device.
+    async fn chunk_batch(&self, _ctx: &SecurityContext, req: EncodeBatchRequest, chunk_tokens: u32, overlap_tokens: u32)
+        -> Result<ChunkBatchResponse, TokenizerError> {
+        if chunk_tokens == 0 || overlap_tokens >= chunk_tokens {
+            return Err(TokenizerError::InvalidInput("the chunk size must be at least 1 and the overlap less than it".to_owned()));
+        }
+        let n = req.offsets.len().saturating_sub(1);
+        let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
+        let native = self.native.clone();
+        let out = tokio::task::spawn_blocking(move || native.chunk_batch(&req.bytes, &req.offsets, vid.as_deref(), chunk_tokens, overlap_tokens))
+            .await
+            .map_err(|e| TokenizerError::Internal(e.to_string()))?
+            .map_err(map_native)?;
+        Ok(ChunkBatchResponse { spans: out.spans, chunk_offsets: out.chunk_offsets, counts: out.counts })
     }
 
     /// The device path: scan, cut and splice run as CUDA kernels (`cfbpe_encode_batch_special`).  The caller's special tokens

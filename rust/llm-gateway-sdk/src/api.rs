@@ -21,6 +21,12 @@ pub trait TokenizerClient: Send + Sync {
     async fn truncate(&self, ctx: &SecurityContext, model: &str, texts: &[String], max_tokens: &[u32], keep: TruncateKeep)
         -> Result<Vec<(String, u32, u32)>, TokenizerError>;
 
+    /// Split texts into chunks of at most `max_tokens` tokens that overlap by `overlap` tokens (a RAG splitter's chunk_size /
+    /// chunk_overlap, an embedding endpoint's long inputs): per text, its chunks.  The cuts are at character boundaries, so every
+    /// chunk is valid UTF-8; with no overlap the chunks join back into the text.
+    async fn chunk(&self, ctx: &SecurityContext, model: &str, texts: &[String], max_tokens: u32, overlap: u32)
+        -> Result<Vec<Vec<String>>, TokenizerError>;
+
     /// tiktoken's `encode(text, allowed_special = …, disallowed_special = …)`.
     async fn encode_with_special(&self, ctx: &SecurityContext, model: &str, texts: &[String], special: &SpecialTokens)
         -> Result<Vec<Vec<u32>>, TokenizerError>;

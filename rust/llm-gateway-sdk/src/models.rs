@@ -88,6 +88,36 @@ pub fn truncate_cut(prompt: &[u8], starts: &[u32], budget: u32, keep: TruncateKe
     }
 }
 
+/// Every prompt of a batch cut into chunks of at most N tokens (`include/cfbpe.h`, `cfbpe_chunk_batch`).  Windows of N tokens start
+/// every N - overlap tokens until one reaches the last token; chunk k covers tokens [a, e) and its bytes are [F(a), F(e)), F(j) =
+/// the character start at or before token j's start, F(c) = the prompt's length.  With no overlap the chunks tile the prompt.
+#[derive(Debug, Clone, Default, Serialize, Deserialize)]
+pub struct ChunkBatchResponse {
+    /// `[begin, end)` of every chunk within its prompt (always character boundaries: every chunk is valid UTF-8)
+    pub spans: Vec<[u32; 2]>,
+    /// prompt i's chunks are `spans[chunk_offsets[i] .. chunk_offsets[i + 1]]` (n + 1 entries)
+    pub chunk_offsets: Vec<u64>,
+    /// tokens of every whole prompt
+    pub counts: Vec<u32>,
+}
+
+/// The chunking contract on the host, from every token's start (`EncodeBatchResponse::starts`): the `[begin, end)` spans of prompt
+/// `prompt` (its UTF-8 bytes), whose tokens start at `starts`.  `chunk_tokens` >= 1, `overlap_tokens` < `chunk_tokens`.
+pub fn chunk_spans(prompt: &[u8], starts: &[u32], chunk_tokens: u32, overlap_tokens: u32) -> Vec<[u32; 2]> {
+    let (c, len) = (starts.len(), prompt.len());
+    let (n, step) = (chunk_tokens as usize, (chunk_tokens - overlap_tokens) as usize);
+    let floor = |j: usize| -> u32 {
+        if j >= c {
+            return len as u32;
+        }
+        let mut x = starts[j] as usize;
+        while x > 0 && x < len && prompt[x] & 0xC0 == 0x80 { x -= 1; }
+        x as u32
+    };
+    let k = if c == 0 { 0 } else if c <= n { 1 } else { 1 + (c - n).div_ceil(step) };
+    (0..k).map(|q| [floor(q * step), floor((q * step + n).min(c))]).collect()
+}
+
 #[derive(Debug, Clone)]
 pub struct CountTokensRequest {
     pub vocab: VocabRef,

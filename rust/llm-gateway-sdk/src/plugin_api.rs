@@ -4,7 +4,7 @@ use async_trait::async_trait;
 use modkit_security::SecurityContext;
 
 use crate::error::TokenizerError;
-use crate::models::{truncate_cut, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens,
+use crate::models::{chunk_spans, truncate_cut, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens,
                     TruncateBatchResponse, TruncateKeep, VocabRef};
 
 /// Each plugin registers this trait with a scoped `ClientHub` entry using its GTS instance id as the scope.  Clients are
@@ -44,6 +44,30 @@ pub trait TokenizerPluginClient: Send + Sync {
             let (cut, kept) = truncate_cut(prompt, &starts[enc.offsets[i] as usize..enc.offsets[i + 1] as usize], budgets[i], keep);
             out.cut.push(cut);
             out.kept.push(kept);
+        }
+        Ok(out)
+    }
+
+    /// Cut every prompt of the batch into chunks of at most `chunk_tokens` tokens that overlap by `overlap_tokens`, at character
+    /// boundaries of the whole prompt's encoding (`ChunkBatchResponse`).  The default works on any plugin that returns token
+    /// starts: one `encode_batch` with `with_starts`, then the cuts on the host.  `gpu-bpe-tokenizer-plugin` overrides it with the
+    /// device call, which downloads no ids and no starts.
+    async fn chunk_batch(&self, ctx: &SecurityContext, req: EncodeBatchRequest, chunk_tokens: u32, overlap_tokens: u32)
+        -> Result<ChunkBatchResponse, TokenizerError> {
+        if chunk_tokens == 0 || overlap_tokens >= chunk_tokens {
+            return Err(TokenizerError::InvalidInput("the chunk size must be at least 1 and the overlap less than it".to_owned()));
+        }
+        let n = req.offsets.len().saturating_sub(1);
+        let bytes = req.bytes.clone();
+        let offsets = req.offsets.clone();
+        let enc = self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, ..req }).await?;
+        let starts = enc.starts.ok_or_else(|| TokenizerError::ServiceUnavailable("the tokenizer plugin does not return token starts".to_owned()))?;
+        let mut out = ChunkBatchResponse { spans: Vec::new(), chunk_offsets: Vec::with_capacity(n + 1), counts: enc.counts };
+        out.chunk_offsets.push(0);
+        for i in 0..n {
+            let prompt = &bytes[offsets[i] as usize..offsets[i + 1] as usize];
+            out.spans.extend(chunk_spans(prompt, &starts[enc.offsets[i] as usize..enc.offsets[i + 1] as usize], chunk_tokens, overlap_tokens));
+            out.chunk_offsets.push(out.spans.len() as u64);
         }
         Ok(out)
     }

@@ -1,4 +1,5 @@
-//! REST DTOs of `POST /llm-gateway/v1/tokenize`, `POST /llm-gateway/v1/count-tokens` and `POST /llm-gateway/v1/truncate`.
+//! REST DTOs of `POST /llm-gateway/v1/tokenize`, `POST /llm-gateway/v1/count-tokens`, `POST /llm-gateway/v1/truncate` and
+//! `POST /llm-gateway/v1/chunk`.
 
 use schemars::JsonSchema;
 use serde::{Deserialize, Serialize};
@@ -59,6 +60,30 @@ pub struct TruncateResponse {
     pub texts: Vec<String>,
     /// tokens of every text's encoding wholly inside the kept text: the budget, or one to three fewer when the cut moved
     pub kept_tokens: Vec<u32>,
+    /// token count of every whole text, as `counts` of `/tokenize`
+    pub counts: Vec<u32>,
+}
+
+#[derive(Debug, Deserialize, JsonSchema)]
+#[serde(deny_unknown_fields)]
+pub struct ChunkRequest {
+    /// canonical model id or vocabulary name
+    pub model: String,
+    /// texts to split (one entry per document)
+    pub texts: Vec<String>,
+    /// the most tokens a chunk holds (>= 1)
+    pub max_tokens: u32,
+    /// tokens consecutive chunks share (< max_tokens); default 0
+    #[serde(default)]
+    pub overlap: u32,
+}
+
+#[derive(Debug, Serialize, JsonSchema)]
+pub struct ChunkResponse {
+    /// every text's chunks, cut at token boundaries of its whole encoding moved to character boundaries (valid UTF-8)
+    pub chunks: Vec<Vec<String>>,
+    /// every chunk's `[begin, end)` byte span in its text's UTF-8, in the order of `chunks`
+    pub spans: Vec<Vec<[u32; 2]>>,
     /// token count of every whole text, as `counts` of `/tokenize`
     pub counts: Vec<u32>,
 }

@@ -8,7 +8,7 @@ use modkit_errors::Problem;
 use modkit_security::SecurityContext;
 
 use crate::api::rest::dto::{
-    ChatTemplateDto, CountTokensRequest, CountTokensResponse, MaxTokens, TokenizeRequest, TokenizeResponse, TruncateRequest, TruncateResponse,
+    ChatTemplateDto, ChunkRequest, ChunkResponse, CountTokensRequest, CountTokensResponse, MaxTokens, TokenizeRequest, TokenizeResponse, TruncateRequest, TruncateResponse,
 };
 use crate::domain::service::TokenizerService;
 
@@ -57,6 +57,22 @@ pub async fn truncate(
     for (text, kept, count) in r {
         out.texts.push(text);
         out.kept_tokens.push(kept);
+        out.counts.push(count);
+    }
+    Ok(Json(out))
+}
+
+pub async fn chunk(
+    Extension(ctx): Extension<SecurityContext>,
+    Extension(service): Extension<Arc<TokenizerService>>,
+    Json(req): Json<ChunkRequest>,
+) -> Result<Json<ChunkResponse>, Problem> {
+    tracing::debug!(model = %req.model, texts = req.texts.len(), bytes = req.texts.iter().map(String::len).sum::<usize>(), "chunk");
+    let r = service.chunk_with_spans(&ctx, &req.model, &req.texts, req.max_tokens, req.overlap).await.map_err(problem)?;
+    let mut out = ChunkResponse { chunks: Vec::with_capacity(r.len()), spans: Vec::with_capacity(r.len()), counts: Vec::with_capacity(r.len()) };
+    for (chunks, spans, count) in r {
+        out.chunks.push(chunks);
+        out.spans.push(spans);
         out.counts.push(count);
     }
     Ok(Json(out))

@@ -62,5 +62,19 @@ pub fn register_routes(mut router: Router, openapi: &dyn OpenApiRegistry, servic
         .standard_errors(openapi)
         .error_415(openapi)
         .register(router, openapi);
+    // POST /llm-gateway/v1/chunk - split texts into chunks of at most N tokens, optionally overlapping, at character boundaries
+    router = OperationBuilder::post("/llm-gateway/v1/chunk")
+        .operation_id("llm_gateway.chunk")
+        .summary("Split texts into chunks of at most N tokens of a model's vocabulary, with an optional overlap")
+        .tag("LLM Gateway")
+        .authenticated()
+        .require_license_features::<License>([])
+        .json_request::<dto::ChunkRequest>(openapi, "Texts, the model whose vocabulary applies, the chunk size and the overlap")
+        .allow_content_types(&["application/json"])
+        .handler(handlers::chunk)
+        .json_response_with_schema::<dto::ChunkResponse>(openapi, http::StatusCode::OK, "The chunks, their byte spans and the full counts")
+        .standard_errors(openapi)
+        .error_415(openapi)
+        .register(router, openapi);
     router.layer(Extension(service))
 }

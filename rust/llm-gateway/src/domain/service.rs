@@ -58,6 +58,22 @@ impl TokenizerService {
             .ok_or_else(|| TokenizerError::ServiceUnavailable(format!("tokenizer plugin {instance_id} is not registered yet")))
     }
 
+    /// Per text: its chunks, their `[begin, end)` spans in its UTF-8 and its token count (`POST /llm-gateway/v1/chunk`).  The plugin
+    /// does the work: the trait's default cuts on the host from token starts, the GPU plugin cuts on the device.
+    pub async fn chunk_with_spans(&self, ctx: &SecurityContext, model: &str, texts: &[String], max_tokens: u32, overlap: u32)
+        -> Result<Vec<(Vec<String>, Vec<[u32; 2]>, u32)>, TokenizerError> {
+        let (bytes, offsets) = pack_texts(texts);
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false };
+        let r = self.plugin().await?.chunk_batch(ctx, req, max_tokens, overlap).await?;
+        texts.iter().enumerate().map(|(i, t)| {
+            let spans = r.spans[r.chunk_offsets[i] as usize..r.chunk_offsets[i + 1] as usize].to_vec();
+            // a span always ends on character boundaries (include/cfbpe.h); get() refuses anything else instead of panicking
+            let chunks = spans.iter().map(|&[b, e]| t.get(b as usize..e as usize).map(str::to_owned)
+                .ok_or_else(|| TokenizerError::Internal(format!("the plugin cut text {i} inside a character")))).collect::<Result<Vec<_>, _>>()?;
+            Ok((chunks, spans, r.counts[i]))
+        }).collect()
+    }
+
     /// the `TextContent.text` parts of a request's messages (`schemas/core/message.v1.schema.json`)
     fn text_parts(messages: &[Value]) -> Vec<String> {
         messages
@@ -108,6 +124,11 @@ impl TokenizerClient for TokenizerService {
                 .ok_or_else(|| TokenizerError::Internal(format!("the plugin cut text {i} inside a character")))?;
             Ok((kept.to_owned(), r.kept[i], r.counts[i]))
         }).collect()
+    }
+
+    async fn chunk(&self, ctx: &SecurityContext, model: &str, texts: &[String], max_tokens: u32, overlap: u32)
+        -> Result<Vec<Vec<String>>, TokenizerError> {
+        Ok(self.chunk_with_spans(ctx, model, texts, max_tokens, overlap).await?.into_iter().map(|(chunks, _, _)| chunks).collect())
     }
 
     async fn encode_with_special(&self, ctx: &SecurityContext, model: &str, texts: &[String], special: &SpecialTokens)
