@@ -14,9 +14,11 @@ def build(force=False):
     if not force and os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in deps):
         return SO
     os.makedirs(os.path.dirname(SO), exist_ok=True)
+    tmp = SO + ".%d.tmp" % os.getpid()       # another process may be loading SO: it sees the old library or the whole new one
     cmd = ["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-fvisibility=hidden", "-fno-omit-frame-pointer",
-           "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas", "-DCFBPE_SIM=1", "-o", SO] + srcs
+           "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas", "-DCFBPE_SIM=1", "-o", tmp] + srcs
     subprocess.check_call(cmd)
+    os.replace(tmp, SO)
     return SO
 
 

@@ -1,7 +1,8 @@
 // sim_harness.cpp -- runs the product's CUDA kernels on the CPU SIMT emulator (tests/simt/cusim.h).
 // TEST INFRASTRUCTURE: built by tests/simt/build.py into tests/simt/_build/libcfbpe_sim.so and
-// loaded only by the non-GPU tests.  The table builder (csrc/vocab.cpp) and the kernels
-// (csrc/bpe_kernels.cuh, csrc/pipeline.cuh) are the product sources, compiled unchanged.
+// loaded only by the non-GPU tests, through tests/simt/simlib.py.  The table builder (csrc/vocab.cpp), the kernels
+// (csrc/bpe_kernels.cuh, csrc/pipeline.cuh, csrc/specials.cuh) and the special-token host code (csrc/specials.h) are the
+// product sources, compiled unchanged.
 #include "cusim.h"
 
 #define CFBPE_LAUNCH(kernel, grid, block, stream, ...) cusim::launch((grid), (block), [&] { kernel(__VA_ARGS__); })
@@ -16,7 +17,10 @@
 #include <type_traits>
 #include <vector>
 
+template <typename T> inline T atomicAnd(T* p, T v) { T o = *p; *p = o & v; return o; }   // (specials.cuh's; not in cusim.h)
+
 #include "../../cyberfabric-core_b200/csrc/pipeline.cuh"
+#include "../../cyberfabric-core_b200/csrc/specials.cuh"
 #include "../../cyberfabric-core_b200/csrc/pretok_ctx.h"
 #include "../../cyberfabric-core_b200/csrc/subbatch.h"
 #include "../../cyberfabric-core_b200/csrc/unicode_tables.h"
@@ -29,6 +33,7 @@ struct SimVocab {
     std::vector<uint8_t> blob;
     TablesHeader hdr;
 };
+struct SimSpecials { std::vector<uint32_t> words; };
 
 static UcTables uc_tables() {
     static uint16_t fsm[kNumPatterns * kPretokTableSize];
@@ -57,6 +62,29 @@ struct SimWorkspace {
     }
     SimWorkspace(const SimWorkspace&) = delete;
     SimWorkspace& operator=(const SimWorkspace&) = delete;
+};
+
+// The VocabSet of a call over built vocabularies, unloaded slots aliasing slot 0 as the library's install_blob makes them, and,
+// when the call has prompts (offsets != nullptr), its batch: the bytes copied with the 64 bytes of padding the kernels read into.
+struct SimBatch {
+    VocabSet vs{};
+    std::vector<uint8_t> padded;
+    BatchView b{};
+    SimBatch(void* const* vocabs, uint32_t n_vocabs, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids) {
+        for (uint32_t i = 0; i < n_vocabs && i < kMaxVocabs; ++i) {
+            SimVocab* v = static_cast<SimVocab*>(vocabs[i]);
+            vs.v[i] = make_view(v->blob.data(), v->hdr);
+        }
+        for (uint32_t i = n_vocabs; i < kMaxVocabs && n_vocabs; ++i) vs.v[i] = vs.v[0];
+        vs.loaded_mask = n_vocabs >= 32 ? 0xFFFFFFFFu : ((1u << n_vocabs) - 1u);
+        if (!offsets) return;
+        const uint64_t total = offsets[n_prompts];
+        padded.assign(bytes, bytes + total);
+        padded.resize(total + 64);
+        b = BatchView{padded.data(), offsets, vocab_ids, n_prompts, total};
+    }
+    SimBatch(const SimBatch&) = delete;
+    SimBatch& operator=(const SimBatch&) = delete;
 };
 
 extern "C" __attribute__((visibility("default"))) uint32_t sim_ctx_count(uint32_t cased) { static SplitTablesHost st; build_split_tables(&st); return st.n_ctx[cased & 1]; }
@@ -118,8 +146,6 @@ __attribute__((visibility("default"))) uint32_t sim_pair_lookup(void* vp, uint32
 
 // K1 only: piece-start bits (n_words+2 words) for a packed batch; patterns[] per vocab id
 static unsigned long long fixups_seen = 0, resumes_seen = 0;
-static int legacy_split = 0;
-__attribute__((visibility("default"))) void sim_use_legacy_split(int on) { legacy_split = on; }
 __attribute__((visibility("default"))) unsigned long long sim_split_fixups(int reset) { const unsigned long long v = fixups_seen; if (reset) fixups_seen = 0; return v; }
 __attribute__((visibility("default"))) int sim_split(const uint32_t* patterns, uint32_t n_patterns, uint32_t n_prompts,
                                                      const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
@@ -137,18 +163,13 @@ __attribute__((visibility("default"))) int sim_split(const uint32_t* patterns, u
         UcTables uc = uc_tables();
         std::vector<SplitFix> fix(total / 16 + 2);
         const uint32_t fix_cap = static_cast<uint32_t>(fix.size());
-        if (legacy_split) {
-            const uint64_t n_chunks = (total + kSplitChunk - 1) / kSplitChunk;
-            cusim::launch(static_cast<unsigned>((n_chunks + 255) / 256), 256, [&] { pretok_split_kernel(b, vs, uc, piece_bits, &st, fix.data(), fix_cap); });
-        } else {
-            std::vector<uint32_t> pstart(nw + 2), bprompt((total >> kPromptBlockShift) + 2);
-            cusim::launch(static_cast<unsigned>((static_cast<uint64_t>(n_prompts) + 1 + 255) / 256), 256, [&] { prompt_map_kernel(b, vs, pstart.data(), bprompt.data(), &st); });
-            const uint64_t n_blocks16 = (total + 15) / 16;
-            const uint32_t n_tiles = static_cast<uint32_t>((n_blocks16 + kSplitWarpOwned - 1) / kSplitWarpOwned);
-            const uint32_t n_tabs = vocab_ids ? kNumPatterns : 1u;
-            cusim::launch(n_tiles < 17 ? 1u : 2u, kSplitCta,      // fewer warps than tiles: the persistent loop runs
-                          [&] { pretok_split16_kernel(b, vs, uc, pstart.data(), bprompt.data(), piece_bits, &st, fix.data(), fix_cap, n_tabs, n_tiles); });
-        }
+        std::vector<uint32_t> pstart(nw + 2), bprompt((total >> kPromptBlockShift) + 2);
+        cusim::launch(static_cast<unsigned>((static_cast<uint64_t>(n_prompts) + 1 + 255) / 256), 256, [&] { prompt_map_kernel(b, vs, pstart.data(), bprompt.data(), &st); });
+        const uint64_t n_blocks16 = (total + 15) / 16;
+        const uint32_t n_tiles = static_cast<uint32_t>((n_blocks16 + kSplitWarpOwned - 1) / kSplitWarpOwned);
+        const uint32_t n_tabs = vocab_ids ? kNumPatterns : 1u;
+        cusim::launch(n_tiles < 17 ? 1u : 2u, kSplitCta,      // fewer warps than tiles: the persistent loop runs
+                      [&] { pretok_split16_kernel(b, vs, uc, pstart.data(), bprompt.data(), piece_bits, &st, fix.data(), fix_cap, n_tabs, n_tiles); });
         cusim::launch(2u, 256, [&] { pretok_fixup_kernel(b, vs, uc, piece_bits, &st, fix.data(), fix_cap); });
         fixups_seen += st.fix_n;
         resumes_seen += cfbpe::dbg_counters()[3] + cfbpe::dbg_counters()[4];
@@ -156,26 +177,19 @@ __attribute__((visibility("default"))) int sim_split(const uint32_t* patterns, u
     return st.bad_utf8 ? CFBPE_EILSEQ : 0;
 }
 
-// the whole path (K1..K3) on host memory
+// the whole path (K1..K3) on host memory, one pass as run_lane without pipelining: cfbpe_encode_batch, or with a non-NULL
+// out_starts (room for out_cap entries) cfbpe_encode_batch_starts
 __attribute__((visibility("default"))) int sim_encode_batch(void* const* vocabs, uint32_t n_vocabs, uint32_t n_prompts,
                                                             const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
-                                                            uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
+                                                            uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets,
                                                             uint32_t* out_counts, uint64_t* n_long_out) {
-    const uint64_t total = offsets[n_prompts];
-    std::vector<uint8_t> padded(bytes, bytes + total); padded.resize(total + 64);
-    BatchView b{padded.data(), offsets, vocab_ids, n_prompts, total};
-    VocabSet vs{};
-    for (uint32_t i = 0; i < n_vocabs && i < kMaxVocabs; ++i) {
-        SimVocab* v = static_cast<SimVocab*>(vocabs[i]);
-        vs.v[i] = make_view(v->blob.data(), v->hdr);
-    }
-    SimWorkspace ws(total);
-    vs.loaded_mask = n_vocabs >= 32 ? 0xFFFFFFFFu : ((1u << n_vocabs) - 1u);
+    SimBatch c(vocabs, n_vocabs, n_prompts, bytes, offsets, vocab_ids);
+    SimWorkspace ws(c.b.total_bytes);
     int* prof = nullptr;
-    enqueue_encode(b, vs, uc_tables(), ws.w, out_ids, out_cap, out_offsets, out_counts, 4u, 0, 0, 0, 0, 0, 0, prof);
+    enqueue_encode(c.b, c.vs, uc_tables(), ws.w, out_ids, out_cap, out_offsets, out_counts, 4u, 0, 0, 0, 0, 0, 0, prof, nullptr, out_starts);
     if (n_long_out) *n_long_out = static_cast<uint64_t>(ws.st.n_long) + ws.st.n_big;
     if (const int rc = status_error(ws.st).code) return rc;
-    if (out_ids && ws.st.n_tokens > out_cap) return CFBPE_ENOSPC;
+    if (out_ids && ws.st.n_tokens > out_cap) { out_offsets[n_prompts] = ws.st.n_tokens; return CFBPE_ENOSPC; }
     return 0;
 }
 
@@ -214,27 +228,150 @@ __attribute__((visibility("default"))) int sim_plan_sub_batches(const uint64_t* 
     return plan_sub_batches(offsets, n, offsets[n], chunk, max_chunks, cut);
 }
 
-// the decode path (ids -> bytes) on host memory; returns the number of decoded bytes in out_offsets[n_seqs]
-__attribute__((visibility("default"))) int sim_decode_batch(void* const* vocabs, uint32_t n_vocabs, uint32_t n_seqs, const uint32_t* ids,
-                                                            const uint64_t* id_offsets, const uint8_t* vocab_ids, uint8_t* out, uint64_t out_cap,
-                                                            uint64_t* out_offsets) {
-    VocabSet vs{};
-    for (uint32_t i = 0; i < n_vocabs && i < kMaxVocabs; ++i) {
-        SimVocab* v = static_cast<SimVocab*>(vocabs[i]);
-        vs.v[i] = make_view(v->blob.data(), v->hdr);
-    }
+// the decode path (ids -> bytes) on host memory, with the vocabularies' special tables when specials is not NULL (a NULL
+// entry: no table); returns the number of decoded bytes in out_offsets[n_seqs]
+__attribute__((visibility("default"))) int sim_decode_batch(void* const* vocabs, void* const* specials, uint32_t n_vocabs, uint32_t n_seqs,
+                                                            const uint32_t* ids, const uint64_t* id_offsets, const uint8_t* vocab_ids,
+                                                            uint8_t* out, uint64_t out_cap, uint64_t* out_offsets) {
+    const SimBatch c(vocabs, n_vocabs, 0, nullptr, nullptr, nullptr);
+    SpecialSet sp{};
+    for (uint32_t i = 0; specials && i < n_vocabs && i < kMaxVocabs; ++i)
+        if (const SimSpecials* t = static_cast<const SimSpecials*>(specials[i])) sp.v[i] = make_special_view(t->words.data(), t->words);
     const uint64_t n_ids = id_offsets[n_seqs];
     DecodeView d{ids, id_offsets, vocab_ids, n_seqs, n_ids};
     const uint32_t n_tiles = static_cast<uint32_t>((n_ids + kDecodeTile - 1) / kDecodeTile);
     std::vector<uint32_t> lens(n_ids + 1), sums(n_tiles + 1);
     std::vector<uint64_t> base(n_tiles + 1);
     DeviceStatus st{};
-    if (n_tiles) cusim::launch(n_tiles, 256, [&] { decode_len_kernel(d, vs, lens.data(), sums.data(), &st); });
+    if (n_tiles) cusim::launch(n_tiles, 256, [&] { decode_len_kernel(d, c.vs, lens.data(), sums.data(), &st, sp); });
     cusim::launch(1u, n_tiles ? 1024u : 32u, [&] { tile_scan_kernel(sums.data(), n_tiles, base.data(), &st, nullptr); });
     if (st.bad_utf8) return CFBPE_EINVAL;
-    if (n_tiles) cusim::launch(n_tiles, 256, [&] { decode_copy_kernel(d, vs, lens.data(), base.data(), out, out_cap); });
+    if (n_tiles) cusim::launch(n_tiles, 256, [&] { decode_copy_kernel(d, c.vs, lens.data(), base.data(), out, out_cap, sp); });
     cusim::launch(static_cast<unsigned>((static_cast<uint64_t>(n_seqs) + 1 + 255) / 256), 256, [&] { decode_offsets_kernel(d, lens.data(), base.data(), out_offsets, &st); });
     return st.tok_end > out_cap ? CFBPE_ENOSPC : 0;
+}
+
+// the table cfbpe_vocab_set_specials builds (rc 0 or CFBPE_EINVAL with a message); n == 0 gives an empty table
+__attribute__((visibility("default"))) void* sim_specials_build(uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* ids,
+                                                                int* rc, char* err, size_t errcap) {
+    SimSpecials* t = new SimSpecials();
+    std::string e;
+    *rc = build_special_table(n, bytes, offsets, ids, t->words, e);
+    if (*rc) { if (err && errcap) std::snprintf(err, errcap, "%s", e.c_str()); delete t; return nullptr; }
+    return t;
+}
+__attribute__((visibility("default"))) void sim_specials_free(void* t) { delete static_cast<SimSpecials*>(t); }
+
+// the special set of a call (fill_special_set, as the library's special_set) over the host tables
+static int sim_special_set(void* const* specials, uint32_t n_vocabs, const uint8_t* const* modes, SpecialSet* sp, bool* scan) {
+    const uint32_t* words[kMaxVocabs] = {};
+    SpecialView views[kMaxVocabs] = {};
+    for (uint32_t v = 0; v < n_vocabs && v < kMaxVocabs; ++v) {
+        const SimSpecials* t = static_cast<const SimSpecials*>(specials[v]);
+        if (!t || t->words.empty()) continue;
+        words[v] = t->words.data();
+        views[v] = make_special_view(t->words.data(), t->words);
+    }
+    uint32_t bad[2];
+    return fill_special_set(words, views, modes, sp, scan, bad);
+}
+
+// cfbpe_encode_batch_special on host memory: the special set (fill_special_set) and the reading of the scan
+// (special_scan_result) are the library's host code; between them the scan, then the ordinary path on the prompts as they are
+// (no kept match) or on the stretches followed by the splice, as enqueue_special_call in csrc/cfbpe.cu runs them.  out_bad[2];
+// *n_stretches_out: the stretches of the ordinary pass (n_prompts when the call took the fast path)
+__attribute__((visibility("default"))) int sim_encode_batch_special(void* const* vocabs, void* const* specials, uint32_t n_vocabs,
+                                                                    const uint8_t* const* modes, uint32_t n_prompts, const uint8_t* bytes,
+                                                                    const uint64_t* offsets, const uint8_t* vocab_ids, uint32_t* out_ids,
+                                                                    uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
+                                                                    uint32_t max_prompts, uint32_t* out_bad, uint64_t* n_stretches_out) {
+    SimBatch c(vocabs, n_vocabs, n_prompts, bytes, offsets, vocab_ids);
+    const uint64_t total = c.b.total_bytes, mp = max_prompts;
+    SimWorkspace ws(total);
+    std::vector<uint32_t> kept_n(mp + 1), st_id(mp + 1), ord_ids(total + 1), ord_counts(mp + 1);
+    std::vector<uint64_t> kept_base(mp + 1), st_off(mp + 2), st_base(mp + 1), ord_offsets(mp + 2);
+    std::vector<uint8_t> st_vocab(mp + 1);
+    SpecialStatus ss{};
+    const SpecialWork sw{kept_n.data(), kept_base.data(), st_off.data(), st_vocab.data(), st_id.data(), st_base.data(), &ss};
+    SpecialSet sp;
+    bool scan = false;
+    if (const int rc = sim_special_set(specials, n_vocabs, modes, &sp, &scan)) return rc;
+    uint64_t n_str = n_prompts;
+    if (scan) {
+        enqueue_special_scan(c.b, sp, ws.w, sw, 0);
+        const SpecialScanResult r = special_scan_result(ss, n_prompts, max_prompts);
+        if (r.disallowed) {
+            if (out_bad) { out_bad[0] = r.prompt; out_bad[1] = r.index; }
+            return CFBPE_EBADMSG;
+        }
+        if (!r.fits) return CFBPE_EINVAL;
+        n_str = r.n_stretches;
+    }
+    if (n_stretches_out) *n_stretches_out = n_str;
+    int* prof = nullptr;
+    uint64_t n_tokens;
+    if (n_str == n_prompts) {
+        enqueue_encode(c.b, c.vs, uc_tables(), ws.w, out_ids, out_cap, out_offsets, out_counts, 4u, 0, 0, 0, 0, 0, 0, prof);
+        n_tokens = ws.st.n_tokens;
+    } else {
+        enqueue_encode_special(c.b, sp, c.vs, uc_tables(), ws.w, sw, static_cast<uint32_t>(n_str), ord_ids.data(), total + 1, ord_offsets.data(),
+                               ord_counts.data(), out_ids, out_cap, out_offsets, out_counts, 4u, 0, 0, 0, 0, 0, 0, prof);
+        n_tokens = ss.fin.n_tokens;
+    }
+    if (const int rc = status_error(ws.st).code) return rc;
+    if (out_ids && n_tokens > out_cap) { out_offsets[n_prompts] = n_tokens; return CFBPE_ENOSPC; }
+    return 0;
+}
+
+// cfbpe_truncate_batch on host memory (one pass, as run_lane without pipelining): the ids go to a scratch buffer of one id a
+// byte, as they go to the lane's buffer; out_counts may be NULL
+__attribute__((visibility("default"))) int sim_truncate_batch(void* const* vocabs, uint32_t n_vocabs, uint32_t n_prompts,
+                                                              const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                                                              const uint32_t* budgets, uint32_t mode, uint32_t* out_cut, uint32_t* out_kept,
+                                                              uint32_t* out_counts) {
+    if (truncate_args_error(budgets, mode, out_cut, out_kept)) return CFBPE_EINVAL;
+    SimBatch c(vocabs, n_vocabs, n_prompts, bytes, offsets, vocab_ids);
+    const uint64_t total = c.b.total_bytes;
+    SimWorkspace ws(total);
+    std::vector<uint32_t> ids(total + 1, 0xDEADBEEF);
+    std::vector<uint64_t> offs(static_cast<uint64_t>(n_prompts) + 1);
+    std::vector<uint32_t> counts(static_cast<uint64_t>(n_prompts) + 1);
+    const TruncateView tv{budgets, mode == CFBPE_TRUNCATE_TAIL ? 1u : 0u, out_cut, out_kept};
+    int* prof = nullptr;
+    enqueue_encode(c.b, c.vs, uc_tables(), ws.w, ids.data(), total + 1, offs.data(), counts.data(), 4u, 0, 0, 0, 0, 0, 0, prof, nullptr, nullptr, &tv);
+    if (const int rc = status_error(ws.st).code) return rc;
+    if (out_counts) std::copy(counts.begin(), counts.begin() + n_prompts, out_counts);
+    return 0;
+}
+
+// cfbpe_chunk_batch on host memory (one pass, as run_lane without pipelining): the ids and starts go to scratch buffers of one
+// entry a byte, as they go to the lane's buffers.  device_form = 0: the spans stage in the workspace's ids_by_pos / dense.by_piece
+// and are copied out when they fit, as a host call does; 1: they go straight to out_spans (pairs, chunks at or past chunk_cap not
+// written), as cfbpe_chunk_batch_device does.  out_counts may be NULL.
+__attribute__((visibility("default"))) int sim_chunk_batch(void* const* vocabs, uint32_t n_vocabs, uint32_t n_prompts, const uint8_t* bytes,
+                                                           const uint64_t* offsets, const uint8_t* vocab_ids, uint32_t chunk_tokens,
+                                                           uint32_t overlap_tokens, uint32_t* out_spans, uint64_t chunk_cap,
+                                                           uint64_t* out_chunk_offsets, uint32_t* out_counts, int device_form) {
+    if (chunk_args_error(chunk_tokens, overlap_tokens, out_spans, out_chunk_offsets)) return CFBPE_EINVAL;
+    SimBatch c(vocabs, n_vocabs, n_prompts, bytes, offsets, vocab_ids);
+    const uint64_t total = c.b.total_bytes;
+    SimWorkspace ws(total);
+    std::vector<uint32_t> ids(total + 1, 0xDEADBEEF), starts(total + 1, 0xDEADBEEF);
+    std::vector<uint64_t> offs(static_cast<uint64_t>(n_prompts) + 1);
+    std::vector<uint32_t> counts(static_cast<uint64_t>(n_prompts) + 1);
+    const uint32_t step = chunk_tokens - overlap_tokens;
+    const ChunkView cv = device_form ? ChunkView{chunk_tokens, step, out_chunk_offsets, nullptr, out_spans, out_spans + 1, 2u, chunk_cap}
+                                     : ChunkView{chunk_tokens, step, out_chunk_offsets, nullptr, ws.w.ids_by_pos, ws.w.dense.by_piece, 1u, UINT64_MAX};
+    int* prof = nullptr;
+    enqueue_encode(c.b, c.vs, uc_tables(), ws.w, ids.data(), total + 1, offs.data(), counts.data(), 4u, 0, 0, 0, 0, 0, 0, prof, nullptr, starts.data(),
+                   nullptr, &cv);
+    if (const int rc = status_error(ws.st).code) return rc;
+    if (out_counts) std::copy(counts.begin(), counts.begin() + n_prompts, out_counts);
+    if (ws.st.chunk_end != out_chunk_offsets[n_prompts] || ws.st.n_chunks != ws.st.chunk_end) return CFBPE_EIO;
+    if (ws.st.chunk_end > chunk_cap) return CFBPE_ENOSPC;
+    if (!device_form)
+        for (uint64_t q = 0; q < ws.st.chunk_end; ++q) { out_spans[2 * q] = ws.w.ids_by_pos[q]; out_spans[2 * q + 1] = ws.w.dense.by_piece[q]; }
+    return 0;
 }
 
 }  // extern "C"

@@ -1,4 +1,4 @@
-"""ctypes binding of the SIMT-emulator harness (test infrastructure)."""
+"""ctypes binding of the SIMT-emulator harness (test infrastructure; tests/simt/sim_harness.cpp)."""
 import ctypes as C
 import os
 import sys
@@ -8,6 +8,8 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import build as _build  # noqa: E402
 
+EINVAL, ENOENT, ENOSPC, EILSEQ, EBADMSG = -22, -2, -28, -84, -74
+ORDINARY, ALLOW, DISALLOW = 0, 1, 2             # special-token modes
 _lib = None
 
 
@@ -27,9 +29,22 @@ def lib():
         L.sim_split.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sim_encode_batch.restype = C.c_int
         L.sim_encode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+                                       C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sim_decode_batch.restype = C.c_int
-        L.sim_decode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        L.sim_decode_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_uint64, C.c_void_p]
+        L.sim_specials_build.restype = C.c_void_p
+        L.sim_specials_build.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_char_p, C.c_size_t]
+        L.sim_specials_free.argtypes = [C.c_void_p]
+        L.sim_encode_batch_special.restype = C.c_int
+        L.sim_encode_batch_special.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]
+        L.sim_truncate_batch.restype = C.c_int
+        L.sim_truncate_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]
+        L.sim_chunk_batch.restype = C.c_int
+        L.sim_chunk_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
+                                      C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int]
         L.sim_plan_sub_batches.restype = C.c_int
         L.sim_plan_sub_batches.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.c_int, C.c_void_p]
         L.sim_split_fixups.restype = C.c_ulonglong
@@ -94,6 +109,32 @@ class SimVocab:
         return lib().sim_pair_lookup(self._h, l, r)
 
 
+class Specials:
+    """the special-token table of one vocabulary ({str or bytes: id}, order = special index)"""
+
+    def __init__(self, specials):
+        toks = [t.encode("utf-8") if isinstance(t, str) else bytes(t) for t in specials]
+        self.tokens = toks
+        offs = np.zeros(len(toks) + 1, dtype=np.uint64)
+        if toks:
+            offs[1:] = np.cumsum([len(t) for t in toks])
+        data = np.frombuffer(b"".join(toks) + b"\0", dtype=np.uint8).copy()
+        ids = np.asarray([int(v) for v in specials.values()] + [0], dtype=np.uint32)
+        rc = C.c_int(0)
+        err = C.create_string_buffer(256)
+        self._h = lib().sim_specials_build(len(toks), data.ctypes.data, offs.ctypes.data, ids.ctypes.data, C.byref(rc), err, 256)
+        self.rc, self.err = rc.value, err.value.decode()
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            lib().sim_specials_free(self._h)
+
+
+def _handles(objs):
+    """the C array of the SimVocab / Specials handles (None: a NULL entry)"""
+    return (C.c_void_p * len(objs))(*[None if o is None else o._h for o in objs])
+
+
 def pack(prompts):
     """list[bytes] -> (uint8 array, uint64 offsets)"""
     offs = np.zeros(len(prompts) + 1, dtype=np.uint64)
@@ -111,8 +152,7 @@ def split(patterns, prompts, vocab_ids=None):
     bits = np.zeros(nw + 2, dtype=np.uint32)
     pats = np.asarray(patterns, dtype=np.uint32)
     vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
-    dbuf = np.concatenate([data, np.zeros(8, np.uint8)])
-    rc = lib().sim_split(pats.ctypes.data, len(pats), len(prompts), dbuf.ctypes.data, offs.ctypes.data,
+    rc = lib().sim_split(pats.ctypes.data, len(pats), len(prompts), data.ctypes.data, offs.ctypes.data,
                          None if vid is None else vid.ctypes.data, bits.ctypes.data)
     flags = np.unpackbits(bits.view(np.uint8), bitorder="little")[:total]
     out = []
@@ -124,35 +164,102 @@ def split(patterns, prompts, vocab_ids=None):
     return rc, out
 
 
-def encode_batch(vocabs, prompts, vocab_ids=None, out_cap=None):
+def encode_batch(vocabs, prompts, vocab_ids=None, out_cap=None, starts=None):
+    """(rc, ids, offsets, counts, long pieces); starts: an array of out_cap entries that receives the token starts, or None"""
     data, offs = pack(prompts)
     total = int(offs[-1])
     cap = total + 1 if out_cap is None else out_cap
     ids = np.zeros(max(cap, 1), dtype=np.uint32)
     out_off = np.zeros(len(prompts) + 1, dtype=np.uint64)
     counts = np.zeros(max(len(prompts), 1), dtype=np.uint32)
-    vh = (C.c_void_p * len(vocabs))(*[v._h for v in vocabs])
     vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
     nlong = C.c_uint64(0)
-    dbuf = np.concatenate([data, np.zeros(8, np.uint8)])
-    rc = lib().sim_encode_batch(vh, len(vocabs), len(prompts), dbuf.ctypes.data, offs.ctypes.data,
-                                None if vid is None else vid.ctypes.data, ids.ctypes.data, cap,
-                                out_off.ctypes.data, counts.ctypes.data, C.byref(nlong))
+    rc = lib().sim_encode_batch(_handles(vocabs), len(vocabs), len(prompts), data.ctypes.data, offs.ctypes.data,
+                                None if vid is None else vid.ctypes.data, ids.ctypes.data,
+                                None if starts is None else starts.ctypes.data, cap, out_off.ctypes.data, counts.ctypes.data,
+                                C.byref(nlong))
     return rc, ids, out_off, counts[:len(prompts)], nlong.value
 
 
-def decode_batch(vocabs, ids, id_offsets, vocab_ids=None, out_cap=None):
-    """the decode kernels on the emulator: (rc, bytes uint8, byte offsets uint64 n+1)"""
+def encode_starts(vocabs, prompts, vocab_ids=None, out_cap=None):
+    """encode with token starts: (rc, ids, starts, offsets, counts)"""
+    cap = sum(len(p) for p in prompts) + 1 if out_cap is None else out_cap
+    starts = np.full(max(cap, 1), 0xFFFFFFFF, dtype=np.uint32)
+    rc, ids, out_off, counts, _ = encode_batch(vocabs, prompts, vocab_ids, cap, starts)
+    n_tok = int(out_off[-1])
+    return rc, ids[:n_tok], starts[:n_tok], out_off, counts
+
+
+def encode_batch_special(vocabs, specials, prompts, modes=None, vocab_ids=None, out_cap=None, max_prompts=1 << 20, counts_only=False):
+    """(rc, per-prompt id lists, counts, bad (prompt, index), n_stretches, offsets)"""
+    data, offs = pack(prompts)
+    total = int(offs[-1])
+    cap = total + 1 if out_cap is None else out_cap
+    ids = np.zeros(max(cap, 1), dtype=np.uint32)
+    out_off = np.zeros(len(prompts) + 1, dtype=np.uint64)
+    counts = np.zeros(max(len(prompts), 1), dtype=np.uint32)
+    keep = [None if m is None else np.ascontiguousarray(m, dtype=np.uint8) for m in (modes or [])]
+    marr = (C.c_void_p * 8)(*([None if m is None else m.ctypes.data for m in keep] + [None] * (8 - len(keep)))) if modes is not None else None
+    vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
+    bad = np.zeros(2, dtype=np.uint32)
+    nst = C.c_uint64(0)
+    rc = lib().sim_encode_batch_special(_handles(vocabs), _handles(specials), len(vocabs), marr, len(prompts), data.ctypes.data,
+                                        offs.ctypes.data, None if vid is None else vid.ctypes.data,
+                                        None if counts_only else ids.ctypes.data, cap, out_off.ctypes.data, counts.ctypes.data,
+                                        max_prompts, bad.ctypes.data, C.byref(nst))
+    out = None
+    if rc == 0 and not counts_only:
+        out = [ids[int(out_off[i]):int(out_off[i + 1])].tolist() for i in range(len(prompts))]
+    return rc, out, counts[:len(prompts)].tolist(), (int(bad[0]), int(bad[1])), nst.value, out_off
+
+
+def truncate(vocabs, prompts, budgets, mode, vocab_ids=None, null=None):
+    """(rc, cut, kept, counts); null: the name of an argument to pass as NULL"""
+    data, offs = pack(prompts)
+    n = len(prompts)
+    bud = np.ascontiguousarray(np.broadcast_to(np.asarray(budgets, dtype=np.uint64), (n,)).astype(np.uint32)) if n else np.zeros(1, np.uint32)
+    cut = np.full(max(n, 1), 0xFFFFFFFF, dtype=np.uint32)
+    kept = np.full(max(n, 1), 0xFFFFFFFF, dtype=np.uint32)
+    counts = np.zeros(max(n, 1), dtype=np.uint32)
+    vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
+    rc = lib().sim_truncate_batch(_handles(vocabs), len(vocabs), n, data.ctypes.data, offs.ctypes.data,
+                                  None if vid is None else vid.ctypes.data, None if null == "budgets" else bud.ctypes.data, mode,
+                                  None if null == "cut" else cut.ctypes.data, None if null == "kept" else kept.ctypes.data,
+                                  counts.ctypes.data)
+    return rc, cut[:n], kept[:n], counts[:n]
+
+
+def chunk(vocabs, prompts, n_tok, overlap, vocab_ids=None, cap=None, device_form=False, null=None):
+    """(rc, spans [cap, 2], chunk offsets [n + 1], counts); cap: the byte bound by default; null: an argument to pass as NULL"""
+    data, offs = pack(prompts)
+    n = len(prompts)
+    if cap is None:
+        ln = np.array([len(p) for p in prompts], dtype=np.int64)
+        step = max(n_tok - overlap, 1)
+        cap = int((ln > 0).sum() + ((np.maximum(ln - n_tok, 0) + step - 1) // step).sum())
+    spans = np.full((max(cap, 1), 2), 0xFFFFFFFF, dtype=np.uint32)
+    coffs = np.full(n + 1, 0xFFFFFFFFFFFFFFFF, dtype=np.uint64)
+    counts = np.zeros(max(n, 1), dtype=np.uint32)
+    vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
+    rc = lib().sim_chunk_batch(_handles(vocabs), len(vocabs), n, data.ctypes.data, offs.ctypes.data, None if vid is None else vid.ctypes.data,
+                               n_tok, overlap, None if null == "spans" else spans.ctypes.data, cap,
+                               None if null == "offsets" else coffs.ctypes.data, counts.ctypes.data, int(device_form))
+    return rc, spans, coffs, counts[:n]
+
+
+def decode_batch(vocabs, ids, id_offsets, vocab_ids=None, out_cap=None, specials=None):
+    """the decode kernels on the emulator: (rc, bytes uint8, byte offsets uint64 n+1); specials: the vocabularies' Specials
+    tables (None entries allowed), or None"""
     ids = np.ascontiguousarray(ids, dtype=np.uint32)
     id_offsets = np.ascontiguousarray(id_offsets, dtype=np.uint64)
     n = len(id_offsets) - 1
     cap = int(out_cap) if out_cap is not None else int(len(ids)) * 260 + 64
     out = np.zeros(max(cap, 1), dtype=np.uint8)
     out_off = np.zeros(n + 1, dtype=np.uint64)
-    vh = (C.c_void_p * len(vocabs))(*[v._h for v in vocabs])
     vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
-    rc = lib().sim_decode_batch(vh, len(vocabs), n, ids.ctypes.data, id_offsets.ctypes.data,
-                                None if vid is None else vid.ctypes.data, out.ctypes.data, cap, out_off.ctypes.data)
+    rc = lib().sim_decode_batch(_handles(vocabs), None if specials is None else _handles(specials), len(vocabs), n, ids.ctypes.data,
+                                id_offsets.ctypes.data, None if vid is None else vid.ctypes.data, out.ctypes.data, cap,
+                                out_off.ctypes.data)
     return rc, out[:int(out_off[n])] if rc == 0 else out[:0], out_off
 
 

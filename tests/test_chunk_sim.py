@@ -1,10 +1,7 @@
 """Chunking (chunk_scan / chunk_emit, csrc/bpe_kernels.cuh) on the CPU SIMT emulator, against a reference built here from live
 tiktoken 0.12.0: encode_ordinary, the tokens' byte lengths and the snap of include/cfbpe.h (cfbpe_chunk_batch)."""
 import base64
-import ctypes as C
-import os
 import random
-import sys
 
 import numpy as np
 import pytest
@@ -12,58 +9,7 @@ import pytest
 import fuzzgen
 import simlib
 from conftest import COMBOS, golden_cases
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "simt"))
-import build_chunk  # noqa: E402
-
-EINVAL, ENOENT, ENOSPC, EILSEQ = -22, -2, -28, -84
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = C.CDLL(build_chunk.build())
-        L.sim_vocab_build.restype = C.c_void_p
-        L.sim_vocab_build.argtypes = [C.c_char_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]
-        L.sim_vocab_free.argtypes = [C.c_void_p]
-        L.sim_chunk_batch.restype = C.c_int
-        L.sim_chunk_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
-                                      C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int]
-        _lib = L
-    return _lib
-
-
-class Vocab:
-    def __init__(self, file_bytes, pattern, max_ranks):
-        err = C.create_string_buffer(256)
-        self._h = lib().sim_vocab_build(file_bytes, len(file_bytes), 0, pattern, max_ranks, err, 256)
-        if not self._h:
-            raise ValueError(err.value.decode())
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            lib().sim_vocab_free(self._h)
-
-
-def chunk(vocabs, prompts, n_tok, overlap, vocab_ids=None, cap=None, device_form=False, null=None):
-    """(rc, spans [cap, 2], chunk offsets [n + 1], counts); cap: the byte bound by default; null: an argument to pass as NULL"""
-    data, offs = simlib.pack(prompts)
-    n = len(prompts)
-    if cap is None:
-        ln = np.array([len(p) for p in prompts], dtype=np.int64)
-        step = max(n_tok - overlap, 1)
-        cap = int((ln > 0).sum() + ((np.maximum(ln - n_tok, 0) + step - 1) // step).sum())
-    spans = np.full((max(cap, 1), 2), 0xFFFFFFFF, dtype=np.uint32)
-    coffs = np.full(n + 1, 0xFFFFFFFFFFFFFFFF, dtype=np.uint64)
-    counts = np.zeros(max(n, 1), dtype=np.uint32)
-    vh = (C.c_void_p * len(vocabs))(*[v._h for v in vocabs])
-    vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
-    dbuf = np.concatenate([data, np.zeros(8, np.uint8)])
-    rc = lib().sim_chunk_batch(vh, len(vocabs), n, dbuf.ctypes.data, offs.ctypes.data, None if vid is None else vid.ctypes.data,
-                               n_tok, overlap, None if null == "spans" else spans.ctypes.data, cap,
-                               None if null == "offsets" else coffs.ctypes.data, counts.ctypes.data, int(device_form))
-    return rc, spans, coffs, counts[:n]
+from simlib import EILSEQ, EINVAL, ENOENT, ENOSPC, chunk
 
 
 def is_cont(b):
@@ -103,7 +49,7 @@ def encs(tekken_bytes):
 
 @pytest.fixture(scope="module")
 def vocabs(tekken_bytes):
-    return {pat: Vocab(tekken_bytes, pat, n) for pat, n in COMBOS}
+    return {pat: simlib.SimVocab(tekken_bytes, 0, pat, n) for pat, n in COMBOS}
 
 
 def check(encs, vocabs, prompts, n_tok, overlap, pats, vocab_ids=None, device_form=False):

@@ -2,10 +2,7 @@
 prefix sum of the byte lengths of the prompt's tokens before it, the ids / offsets / counts are those of the plain path, and the
 starts give live tiktoken 0.12.0's `decode_with_offsets` under its own byte -> character rule."""
 import base64
-import ctypes as C
-import os
 import random
-import sys
 
 import numpy as np
 import pytest
@@ -13,66 +10,11 @@ import pytest
 import fuzzgen
 import simlib
 from conftest import COMBOS, golden_cases
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "simt"))
-import build_starts  # noqa: E402
-
-ENOSPC = -28
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = C.CDLL(build_starts.build())
-        L.sim_vocab_build.restype = C.c_void_p
-        L.sim_vocab_build.argtypes = [C.c_char_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]
-        L.sim_vocab_free.argtypes = [C.c_void_p]
-        L.sim_encode_batch_starts.restype = C.c_int
-        L.sim_encode_batch_starts.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                              C.c_uint64, C.c_void_p, C.c_void_p]
-        _lib = L
-    return _lib
-
-
-class Vocab:
-    def __init__(self, file_bytes, pattern, max_ranks):
-        err = C.create_string_buffer(256)
-        self._h = lib().sim_vocab_build(file_bytes, len(file_bytes), 0, pattern, max_ranks, err, 256)
-        if not self._h:
-            raise ValueError(err.value.decode())
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            lib().sim_vocab_free(self._h)
-
-
-def encode_starts(vocabs, prompts, vocab_ids=None, out_cap=None):
-    """(rc, ids, starts, offsets, counts)"""
-    data, offs = simlib.pack(prompts)
-    total = int(offs[-1])
-    cap = total + 1 if out_cap is None else out_cap
-    ids = np.zeros(max(cap, 1), dtype=np.uint32)
-    starts = np.full(max(cap, 1), 0xFFFFFFFF, dtype=np.uint32)
-    out_off = np.zeros(len(prompts) + 1, dtype=np.uint64)
-    counts = np.zeros(max(len(prompts), 1), dtype=np.uint32)
-    vh = (C.c_void_p * len(vocabs))(*[v._h for v in vocabs])
-    vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
-    dbuf = np.concatenate([data, np.zeros(8, np.uint8)])
-    rc = lib().sim_encode_batch_starts(vh, len(vocabs), len(prompts), dbuf.ctypes.data, offs.ctypes.data,
-                                       None if vid is None else vid.ctypes.data, ids.ctypes.data, starts.ctypes.data, cap,
-                                       out_off.ctypes.data, counts.ctypes.data)
-    n_tok = int(out_off[-1])
-    return rc, ids[:n_tok], starts[:n_tok], out_off, counts[:len(prompts)]
+from simlib import ENOSPC, encode_starts
 
 
 @pytest.fixture(scope="module")
 def vocabs(tekken_bytes):
-    return {pat: Vocab(tekken_bytes, pat, n) for pat, n in COMBOS}
-
-
-@pytest.fixture(scope="module")
-def plain_vocabs(tekken_bytes):
     return {pat: simlib.SimVocab(tekken_bytes, 0, pat, n) for pat, n in COMBOS}
 
 
@@ -82,11 +24,11 @@ def tok_lens(tekken_bytes):
     return np.array([len(base64.b64decode(l.split()[0])) for l in tekken_bytes.splitlines()], dtype=np.int64)
 
 
-def check(vocabs, plain, lens, prompts, vocab_ids=None):
+def check(vocabs, lens, prompts, vocab_ids=None):
     """starts obey the prefix-sum rule; ids, offsets and counts equal the plain path's"""
     rc, ids, starts, off, counts = encode_starts(vocabs, prompts, vocab_ids)
     assert rc == 0
-    prc, pids, poff, pcounts, _ = simlib.encode_batch(plain, prompts, vocab_ids=vocab_ids)
+    prc, pids, poff, pcounts, _ = simlib.encode_batch(vocabs, prompts, vocab_ids=vocab_ids)
     assert prc == 0
     assert np.array_equal(off, poff)
     assert np.array_equal(ids, pids[:int(poff[-1])])
@@ -101,12 +43,12 @@ def check(vocabs, plain, lens, prompts, vocab_ids=None):
 
 
 @pytest.mark.parametrize("pat,n_ranks", COMBOS)
-def test_golden_cases_starts_and_parity(golden, vocabs, plain_vocabs, tok_lens, pat, n_ranks):
+def test_golden_cases_starts_and_parity(golden, vocabs, tok_lens, pat, n_ranks):
     cases = golden_cases(golden)
-    check([vocabs[pat]], [plain_vocabs[pat]], tok_lens, cases)
+    check([vocabs[pat]], tok_lens, cases)
 
 
-def test_layouts(vocabs, plain_vocabs, tok_lens):
+def test_layouts(vocabs, tok_lens):
     rng = random.Random(11)
     words = [s.encode() for s in fuzzgen.fuzz_strings(3, 400, max_atoms=4)]
     prompts = [w for w in words[:300]]                        # many prompts inside one 1 KiB window, empty ones among them
@@ -125,19 +67,19 @@ def test_layouts(vocabs, plain_vocabs, tok_lens):
     prompts.append(long_one.encode())                         # several windows; pieces > 32 B and > 256 B (ids by position)
     prompts += [b"", b"tail"]
     for pat in (0, 3):
-        check([vocabs[pat]], [plain_vocabs[pat]], tok_lens, prompts)
+        check([vocabs[pat]], tok_lens, prompts)
 
 
-def test_empty_prompts_only_and_edges(vocabs, plain_vocabs, tok_lens):
-    check([vocabs[0]], [plain_vocabs[0]], tok_lens, [b"", b"", b""])
-    check([vocabs[0]], [plain_vocabs[0]], tok_lens, [b"", b"a", b"", b"", b"bc", b""])
-    check([vocabs[0]], [plain_vocabs[0]], tok_lens, [b"x" * 1024, b"y" * 1023, b"", b"z"])
+def test_empty_prompts_only_and_edges(vocabs, tok_lens):
+    check([vocabs[0]], tok_lens, [b"", b"", b""])
+    check([vocabs[0]], tok_lens, [b"", b"a", b"", b"", b"bc", b""])
+    check([vocabs[0]], tok_lens, [b"x" * 1024, b"y" * 1023, b"", b"z"])
 
 
-def test_mixed_vocabulary_batch(vocabs, plain_vocabs, tok_lens):
+def test_mixed_vocabulary_batch(vocabs, tok_lens):
     prompts = [s.encode() for s in fuzzgen.fuzz_strings(31, 300, max_atoms=40)] + [s.encode() for s in fuzzgen.long_runs(2)[:40]]
     vid = np.array([i % 4 for i in range(len(prompts))], dtype=np.uint8)
-    check([vocabs[p] for p, _ in COMBOS], [plain_vocabs[p] for p, _ in COMBOS], tok_lens, prompts, vocab_ids=vid)
+    check([vocabs[p] for p, _ in COMBOS], tok_lens, prompts, vocab_ids=vid)
 
 
 def test_out_cap_too_small(vocabs):

@@ -2,10 +2,7 @@
 built here from live tiktoken 0.12.0: decode_bytes of the first / last k ids, moved to a character boundary (include/cfbpe.h,
 cfbpe_truncate_batch)."""
 import base64
-import ctypes as C
-import os
 import random
-import sys
 
 import numpy as np
 import pytest
@@ -13,57 +10,10 @@ import pytest
 import fuzzgen
 import simlib
 from conftest import COMBOS, golden_cases
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "simt"))
-import build_truncate  # noqa: E402
+from simlib import EILSEQ, EINVAL, ENOENT, truncate
 
 HEAD, TAIL = 0, 1
-EINVAL, ENOENT, EILSEQ = -22, -2, -84
 MAX_BUDGET = 2 ** 32 - 1
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = C.CDLL(build_truncate.build())
-        L.sim_vocab_build.restype = C.c_void_p
-        L.sim_vocab_build.argtypes = [C.c_char_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]
-        L.sim_vocab_free.argtypes = [C.c_void_p]
-        L.sim_truncate_batch.restype = C.c_int
-        L.sim_truncate_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
-                                         C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib = L
-    return _lib
-
-
-class Vocab:
-    def __init__(self, file_bytes, pattern, max_ranks):
-        err = C.create_string_buffer(256)
-        self._h = lib().sim_vocab_build(file_bytes, len(file_bytes), 0, pattern, max_ranks, err, 256)
-        if not self._h:
-            raise ValueError(err.value.decode())
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            lib().sim_vocab_free(self._h)
-
-
-def truncate(vocabs, prompts, budgets, mode, vocab_ids=None, null=None):
-    """(rc, cut, kept, counts); null: the name of an argument to pass as NULL"""
-    data, offs = simlib.pack(prompts)
-    n = len(prompts)
-    bud = np.ascontiguousarray(np.broadcast_to(np.asarray(budgets, dtype=np.uint64), (n,)).astype(np.uint32)) if n else np.zeros(1, np.uint32)
-    cut = np.full(max(n, 1), 0xFFFFFFFF, dtype=np.uint32)
-    kept = np.full(max(n, 1), 0xFFFFFFFF, dtype=np.uint32)
-    counts = np.zeros(max(n, 1), dtype=np.uint32)
-    vh = (C.c_void_p * len(vocabs))(*[v._h for v in vocabs])
-    vid = None if vocab_ids is None else np.ascontiguousarray(vocab_ids, dtype=np.uint8)
-    dbuf = np.concatenate([data, np.zeros(8, np.uint8)])
-    rc = lib().sim_truncate_batch(vh, len(vocabs), n, dbuf.ctypes.data, offs.ctypes.data, None if vid is None else vid.ctypes.data,
-                                  None if null == "budgets" else bud.ctypes.data, mode, None if null == "cut" else cut.ctypes.data,
-                                  None if null == "kept" else kept.ctypes.data, counts.ctypes.data)
-    return rc, cut[:n], kept[:n], counts[:n]
 
 
 def is_cont(b):
@@ -107,7 +57,7 @@ def encs(tekken_bytes):
 
 @pytest.fixture(scope="module")
 def vocabs(tekken_bytes):
-    return {pat: Vocab(tekken_bytes, pat, n) for pat, n in COMBOS}
+    return {pat: simlib.SimVocab(tekken_bytes, 0, pat, n) for pat, n in COMBOS}
 
 
 def budget_kinds(c, rng):
