@@ -43,6 +43,19 @@ def fuzz_strings(seed: int, count: int, max_atoms=24):
     return [fuzz_string(rng, max_atoms) for _ in range(count)]
 
 
+SCALAR_CONTEXTS = [lambda c: c, lambda c: "a" + c + "b", lambda c: " " + c + c + "'s", lambda c: "A" + c + "1",
+                   lambda c: "!" + c + "\n"]
+
+
+def every_scalar_value(context: int, per_prompt=16):
+    """all 1 112 064 Unicode scalar values (every code point but the surrogates), in order, each wrapped in one of the five
+    SCALAR_CONTEXTS (alone, between letters, doubled after a space with a contraction, between a capital and a digit,
+    after punctuation before a newline), per_prompt of them a prompt"""
+    f = SCALAR_CONTEXTS[context]
+    cps = [c for c in range(0x110000) if not 0xD800 <= c <= 0xDFFF]
+    return ["".join(f(chr(c)) for c in cps[i:i + per_prompt]) for i in range(0, len(cps), per_prompt)]
+
+
 def long_runs(seed: int):
     """adversarial long single-class runs and repeats"""
     rng = random.Random(seed)
