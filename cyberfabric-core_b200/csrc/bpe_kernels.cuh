@@ -477,8 +477,9 @@ __device__ __forceinline__ uint64_t next_set_bit(const uint32_t* __restrict__ bi
 constexpr uint32_t kPieceRange = 512;     // bytes of text per warp: 16 per lane
 constexpr uint32_t kPieceWarps = 4;       // warps per CTA
 
-// bytes [p, p+16) as four little-endian words, read with aligned 32-bit loads (p may be unaligned; the buffer is
-// readable up to 16 bytes past the last prompt byte)
+// bytes [p, p+16) as four little-endian words, read with aligned 32-bit loads (p may be unaligned): an aligned p reads
+// [p, p + 16), any other [p & ~3, (p & ~3) + 20), so the furthest byte read is p + 18.  Callers stay within the 32 readable
+// bytes past the last prompt byte (include/cfbpe.h); no result depends on the bytes read past a prompt's end
 __device__ __forceinline__ void load16(const uint8_t* __restrict__ p, uint32_t& w0, uint32_t& w1, uint32_t& w2, uint32_t& w3) {
     const uintptr_t addr = reinterpret_cast<uintptr_t>(p);
     const uint32_t* q = reinterpret_cast<const uint32_t*>(addr & ~static_cast<uintptr_t>(3));

@@ -111,7 +111,10 @@ inline Workspace slice_workspace(const Workspace& all, uint64_t o0, uint64_t len
 }
 
 // The lane's inputs and outputs of a pipelined host call.  Sub-batch k's bytes start on a 16-byte boundary (K1 reads 16 bytes a
-// lane with one load; the allocation leaves >= 16 bytes of readable padding after the last); its n_k + 1 offsets start at p0 + k.
+// lane with one load); its n_k + 1 offsets start at p0 + k.  Between the end of sub-batch k and the start of k + 1 lie 1 to 31
+// bytes (1 when o0 = 1 and o0 + len = 0 mod 16), so k's kernels read up to 32 bytes past its end into k + 1's bytes -- stale
+// data from an earlier call, or an upload in flight -- which no result depends on; the allocation leaves more than 32 bytes after
+// the last sub-batch.
 inline uint64_t sub_batch_bytes_at(uint64_t o0, uint32_t k) { return ((o0 + 15) & ~15ull) + 16ull * k; }
 inline uint64_t lane_bytes_alloc(uint64_t max_bytes, uint32_t max_chunks) { return max_bytes + 256 + 16ull * (max_chunks + 1); }
 inline uint64_t sub_batch_offsets_at(uint32_t p0, uint32_t k) { return static_cast<uint64_t>(p0) + k; }

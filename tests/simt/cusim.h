@@ -192,8 +192,9 @@ template <typename T> inline T from_u64(uint64_t u) { T v; std::memcpy(&v, &u, s
 #define __launch_bounds__(...)
 #define __shared__ static
 #define __align__(n) __attribute__((aligned(n)))
-struct uint4 { unsigned x, y, z, w; };
-struct uint2 { unsigned x, y; };
+// CUDA's alignment: a vector load from a misaligned address faults on the GPU; here the sanitizer build stops on it
+struct alignas(16) uint4 { unsigned x, y, z, w; };
+struct alignas(8) uint2 { unsigned x, y; };
 inline uint4 make_uint4(unsigned x, unsigned y, unsigned z, unsigned w) { uint4 v; v.x = x; v.y = y; v.z = z; v.w = w; return v; }
 #define threadIdx (cusim::B().cur->tid)
 #define blockIdx (cusim::B().bid)

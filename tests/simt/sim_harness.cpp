@@ -12,7 +12,13 @@
 #define CFBPE_FORK(main, aux, ev) ((void)0)
 #define CFBPE_JOIN(main, aux, ev) ((void)0)
 
+#include <sys/mman.h>
+#include <unistd.h>
+
 #include <algorithm>
+#include <cstdio>
+#include <cstdlib>
+#include <memory>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -64,11 +70,54 @@ struct SimWorkspace {
     SimWorkspace& operator=(const SimWorkspace&) = delete;
 };
 
+// Where every call puts its batch's bytes (sim_batch_layout; process-wide): the first prompt byte at an address = misalign
+// (mod 16), the fill repeated over the mapped bytes before it and over the padding after the last prompt byte, and a guard:
+//   kGuardNone    64 bytes of padding
+//   kGuardAfter   exactly 32 bytes of padding (what include/cfbpe.h asks of a caller), then a PROT_NONE page; the start
+//                 follows from the batch length, misalign is not used
+//   kGuardBefore  the first byte misalign bytes into a page whose predecessor is PROT_NONE; 64 bytes of padding
+// The default (misalign 0, fill one zero byte, no guard) is the layout every test had before layouts could be chosen.
+enum : uint32_t { kGuardNone = 0, kGuardAfter = 1, kGuardBefore = 2 };
+struct SimByteLayout {
+    uint32_t misalign = 0, guard = kGuardNone;
+    std::vector<uint8_t> fill{0};
+};
+static SimByteLayout g_layout;
+
+// a batch's bytes placed by g_layout, unmapped on destruction (an access to a guard page stops the process with SIGSEGV)
+struct SimBytes {
+    uint8_t* p = nullptr;              // the first prompt byte
+    void* map = nullptr;
+    size_t map_len = 0;
+    SimBytes(const uint8_t* bytes, uint64_t total) {
+        const size_t page = static_cast<size_t>(sysconf(_SC_PAGESIZE));
+        const SimByteLayout& L = g_layout;
+        const uint64_t pad = L.guard == kGuardAfter ? 32 : 64;
+        const uint64_t lead = L.guard == kGuardAfter ? 0 : L.misalign;
+        const size_t readable = (lead + total + pad + page - 1) / page * page;
+        map_len = readable + (L.guard == kGuardNone ? 0 : page);
+        map = mmap(nullptr, map_len, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0);
+        if (map == MAP_FAILED) { std::perror("mmap"); std::abort(); }
+        uint8_t* r = static_cast<uint8_t*>(map);                  // the readable region [r, r + readable)
+        if (L.guard == kGuardBefore) r += page;
+        p = L.guard == kGuardAfter ? r + readable - pad - total : r + lead;
+        const size_t n_fill = L.fill.size();
+        for (uint8_t* q = r; q < p; ++q) *q = L.fill[static_cast<size_t>(q - r) % n_fill];
+        if (total) std::memcpy(p, bytes, total);
+        for (uint64_t i = 0; i < pad; ++i) p[total + i] = L.fill[i % n_fill];
+        if (L.guard == kGuardAfter && mprotect(r + readable, page, PROT_NONE)) { std::perror("mprotect"); std::abort(); }
+        if (L.guard == kGuardBefore && mprotect(map, page, PROT_NONE)) { std::perror("mprotect"); std::abort(); }
+    }
+    ~SimBytes() { munmap(map, map_len); }
+    SimBytes(const SimBytes&) = delete;
+    SimBytes& operator=(const SimBytes&) = delete;
+};
+
 // The VocabSet of a call over built vocabularies, unloaded slots aliasing slot 0 as the library's install_blob makes them, and,
-// when the call has prompts (offsets != nullptr), its batch: the bytes copied with the 64 bytes of padding the kernels read into.
+// when the call has prompts (offsets != nullptr), its batch: the bytes placed by the current layout (SimBytes).
 struct SimBatch {
     VocabSet vs{};
-    std::vector<uint8_t> padded;
+    std::unique_ptr<SimBytes> bytes;
     BatchView b{};
     SimBatch(void* const* vocabs, uint32_t n_vocabs, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids) {
         for (uint32_t i = 0; i < n_vocabs && i < kMaxVocabs; ++i) {
@@ -79,9 +128,8 @@ struct SimBatch {
         vs.loaded_mask = n_vocabs >= 32 ? 0xFFFFFFFFu : ((1u << n_vocabs) - 1u);
         if (!offsets) return;
         const uint64_t total = offsets[n_prompts];
-        padded.assign(bytes, bytes + total);
-        padded.resize(total + 64);
-        b = BatchView{padded.data(), offsets, vocab_ids, n_prompts, total};
+        this->bytes = std::make_unique<SimBytes>(bytes, total);
+        b = BatchView{this->bytes->p, offsets, vocab_ids, n_prompts, total};
     }
     SimBatch(const SimBatch&) = delete;
     SimBatch& operator=(const SimBatch&) = delete;
@@ -91,6 +139,15 @@ extern "C" __attribute__((visibility("default"))) uint32_t sim_ctx_count(uint32_
 extern "C" __attribute__((visibility("default"))) uint32_t sim_prod_count(uint32_t pat) { static SplitTablesHost st; build_split_tables(&st); return st.n_prod[pat & 3]; }
 
 extern "C" {
+
+// the layout of every later call's batch (SimBytes): 0, or CFBPE_EINVAL for misalign > 15, an empty fill or an unknown guard
+__attribute__((visibility("default"))) int sim_batch_layout(uint32_t misalign, const uint8_t* fill, uint32_t fill_len, uint32_t guard) {
+    if (misalign > 15 || !fill || !fill_len || guard > kGuardBefore) return CFBPE_EINVAL;
+    g_layout.misalign = misalign;
+    g_layout.guard = guard;
+    g_layout.fill.assign(fill, fill + fill_len);
+    return 0;
+}
 
 __attribute__((visibility("default"))) void* sim_vocab_build(const uint8_t* file, size_t len, uint32_t format,
                                                              uint32_t pattern, uint32_t max_ranks, char* err, size_t errcap) {
@@ -144,6 +201,13 @@ __attribute__((visibility("default"))) uint32_t sim_pair_lookup(void* vp, uint32
     return pair_lookup(make_view(v->blob.data(), v->hdr), l, r);
 }
 
+// K1's bulk run scanners on n bytes placed by the current layout: ascii_digit_run_end (digits != 0) or same_byte_run_end(c) from
+// pos, bounded by pe
+__attribute__((visibility("default"))) uint64_t sim_run_end(uint32_t digits, const uint8_t* bytes, uint64_t n, uint64_t pos, uint64_t pe, uint32_t c) {
+    const SimBytes placed(bytes, n);
+    return digits ? ascii_digit_run_end(placed.p, pos, pe) : same_byte_run_end(placed.p, pos, pe, c);
+}
+
 // K1 only: piece-start bits (n_words+2 words) for a packed batch; patterns[] per vocab id
 static unsigned long long fixups_seen = 0, resumes_seen = 0;
 __attribute__((visibility("default"))) unsigned long long sim_split_fixups(int reset) { const unsigned long long v = fixups_seen; if (reset) fixups_seen = 0; return v; }
@@ -151,8 +215,8 @@ __attribute__((visibility("default"))) int sim_split(const uint32_t* patterns, u
                                                      const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
                                                      uint32_t* piece_bits) {
     const uint64_t total = offsets[n_prompts];
-    std::vector<uint8_t> padded(bytes, bytes + total); padded.resize(total + 64);
-    BatchView b{padded.data(), offsets, vocab_ids, n_prompts, total};
+    const SimBytes placed(bytes, total);
+    BatchView b{placed.p, offsets, vocab_ids, n_prompts, total};
     VocabSet vs{};
     for (uint32_t i = 0; i < n_patterns && i < kMaxVocabs; ++i) vs.v[i].pattern_id = patterns[i];
     DeviceStatus st{};

@@ -1,4 +1,5 @@
 """ctypes binding of the SIMT-emulator harness (test infrastructure; tests/simt/sim_harness.cpp)."""
+import contextlib
 import ctypes as C
 import os
 import sys
@@ -10,13 +11,17 @@ import build as _build  # noqa: E402
 
 EINVAL, ENOENT, ENOSPC, EILSEQ, EBADMSG = -22, -2, -28, -84, -74
 ORDINARY, ALLOW, DISALLOW = 0, 1, 2             # special-token modes
+GUARDS = {"none": 0, "after": 1, "before": 2}   # sim_batch_layout's guard pages
+SANITIZE_ENV = "CFBPE_SIM_SANITIZE"             # "1": this process loads the alignment-sanitizer build (build.py)
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_build.build())
+        L = C.CDLL(_build.build(sanitize=os.environ.get(SANITIZE_ENV) == "1"))
+        L.sim_batch_layout.restype = C.c_int
+        L.sim_batch_layout.argtypes = [C.c_uint32, C.c_char_p, C.c_uint32, C.c_uint32]
         L.sim_vocab_build.restype = C.c_void_p
         L.sim_vocab_build.argtypes = [C.c_char_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]
         L.sim_vocab_free.argtypes = [C.c_void_p]
@@ -25,6 +30,8 @@ def lib():
         L.sim_piece_lookup.argtypes = [C.c_void_p, C.c_char_p, C.c_uint32]
         L.sim_pair_lookup.restype = C.c_uint32
         L.sim_pair_lookup.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
+        L.sim_run_end.restype = C.c_uint64
+        L.sim_run_end.argtypes = [C.c_uint32, C.c_char_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32]
         L.sim_split.restype = C.c_int
         L.sim_split.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.sim_encode_batch.restype = C.c_int
@@ -59,6 +66,23 @@ def lib():
         L.sim_workspace_layout.argtypes = [C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p]
         _lib = L
     return _lib
+
+
+def set_batch_layout(misalign=0, fill=b"\0", guard="none"):
+    """where every later call puts its batch (sim_harness.cpp, SimBytes): the first prompt byte at an address = misalign (mod 16),
+    `fill` repeated over the bytes before it and the padding after the last prompt byte; guard "after": exactly 32 bytes of
+    padding, then an unmapped page (misalign not used); "before": an unmapped page just before the misalign leading bytes"""
+    assert lib().sim_batch_layout(misalign, bytes(fill), len(fill), GUARDS[guard]) == 0, (misalign, fill, guard)
+
+
+@contextlib.contextmanager
+def batch_layout(misalign=0, fill=b"\0", guard="none"):
+    """set_batch_layout for the calls in the block, then the default again (aligned, 64 zero bytes, no guard)"""
+    set_batch_layout(misalign, fill, guard)
+    try:
+        yield
+    finally:
+        set_batch_layout()
 
 
 def validate_blob(blob: np.ndarray):
@@ -142,6 +166,12 @@ def pack(prompts):
         offs[1:] = np.cumsum([len(p) for p in prompts], dtype=np.uint64)
     data = np.frombuffer(b"".join(prompts), dtype=np.uint8).copy() if prompts else np.zeros(0, np.uint8)
     return data, offs
+
+
+def run_end(data: bytes, pos, pe, byte=None):
+    """K1's bulk run scanners on data placed by the current layout: the end of the run of `byte` (same_byte_run_end) or, with
+    byte None, of ASCII digits (ascii_digit_run_end) that starts at pos, bounded by pe"""
+    return int(lib().sim_run_end(1 if byte is None else 0, bytes(data), len(data), pos, pe, 0 if byte is None else byte))
 
 
 def split(patterns, prompts, vocab_ids=None):
