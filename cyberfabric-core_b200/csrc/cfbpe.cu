@@ -4,12 +4,15 @@
 // computes runs the kernels of bpe_kernels.cuh on the device or returns an error.
 #include <cuda_runtime.h>
 
+#include <array>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/cfbpe.h"
@@ -33,21 +36,31 @@ static inline void prof_mark(ProfEvents* p, int idx, cudaStream_t s, bool begin)
 
 using namespace cfbpe;
 
+// Owners of a context's CUDA resources.  Each kind is released by its deleter and nowhere else; a deleter acts on the current
+// device, so ~Lane and ~DeviceCtx select theirs before their members go.
+struct DeviceFree { void operator()(void* p) const { cudaFree(p); } };
+struct HostFree { void operator()(void* p) const { cudaFreeHost(p); } };
+struct StreamDestroy { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+struct EventDestroy { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+template <typename T> using DevPtr = std::unique_ptr<T, DeviceFree>;    // device memory
+template <typename T> using HostPtr = std::unique_ptr<T, HostFree>;     // pinned host memory
+using Stream = std::unique_ptr<std::remove_pointer_t<cudaStream_t>, StreamDestroy>;
+using Event = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, EventDestroy>;
+
 struct ProfEvents {
-    cudaEvent_t ev[CFBPE_NUM_KERNELS][2];
-    cudaEvent_t h2d[2], d2h[2], total[2];
+    Event ev[CFBPE_NUM_KERNELS][2];
+    Event h2d[2], d2h[2], total[2];
     bool launched[CFBPE_NUM_KERNELS];
 };
 static inline void prof_mark(ProfEvents* p, int idx, cudaStream_t s, bool begin) {
     if (!p) return;
-    cudaEventRecord(p->ev[idx][begin ? 0 : 1], s);
+    cudaEventRecord(p->ev[idx][begin ? 0 : 1].get(), s);
     p->launched[idx] = true;
 }
 
 #include <dlfcn.h>
 
 #include <atomic>
-#include <memory>
 #include <shared_mutex>
 #include <thread>
 
@@ -77,90 +90,97 @@ constexpr uint64_t kPipeMinBytes = 4ull << 20;      // smaller calls run as one 
 // the buffers of special-token calls (cfbpe_encode_batch_special*), allocated on the lane's first such call: a context that
 // never uses special tokens keeps the footprint it had
 struct LaneSpecial {
-    bool ready = false;
-    uint32_t* kept_n = nullptr;           // [max_prompts] kept matches per prompt ...
-    uint64_t* kept_base = nullptr;        // ... and their exclusive scan
-    uint64_t* st_off = nullptr;           // [max_prompts + 1] stretch byte offsets
-    uint8_t* st_vocab = nullptr;          // [max_prompts] stretch vocabularies
-    uint32_t* st_id = nullptr;            // [max_prompts] special id of a stretch, or kSpText
-    uint64_t* st_base = nullptr;          // [max_prompts] first output id of a stretch
-    uint64_t* fin_offsets = nullptr;      // host calls: the prompts' offsets [max_prompts + 1] ...
-    uint32_t* fin_counts = nullptr;       // ... and counts [max_prompts]
-    uint8_t* modes = nullptr;             // [CFBPE_MAX_VOCABS][kMaxSpecials] the call's mode bytes
-    SpecialStatus* status = nullptr;
-    SpecialStatus* h_status = nullptr;    // pinned
+    DevPtr<uint32_t> kept_n;              // [max_prompts] kept matches per prompt ...
+    DevPtr<uint64_t> kept_base;           // ... and their exclusive scan
+    DevPtr<uint64_t> st_off;              // [max_prompts + 1] stretch byte offsets
+    DevPtr<uint8_t> st_vocab;             // [max_prompts] stretch vocabularies
+    DevPtr<uint32_t> st_id;               // [max_prompts] special id of a stretch, or kSpText
+    DevPtr<uint64_t> st_base;             // [max_prompts] first output id of a stretch
+    DevPtr<uint64_t> fin_offsets;         // host calls: the prompts' offsets [max_prompts + 1] ...
+    DevPtr<uint32_t> fin_counts;          // ... and counts [max_prompts]
+    DevPtr<uint8_t> modes;                // [CFBPE_MAX_VOCABS][kMaxSpecials] the call's mode bytes
+    DevPtr<SpecialStatus> status;
+    HostPtr<SpecialStatus> h_status;      // pinned
 };
 
 struct Lane {
     std::mutex mu;                        // held for the duration of a call
     int device = 0;
     uint64_t max_bytes = 0;
-    cudaStream_t stream = nullptr;       // compute
-    cudaStream_t h2d_stream = nullptr;   // pipelined host calls: uploads run ahead of the kernels ...
-    cudaStream_t d2h_stream = nullptr;   // ... and downloads trail them
-    uint32_t* d_dec_sums = nullptr;      // decode: bytes per tile of kDecodeTile tokens ...
-    uint64_t* d_dec_base = nullptr;      // ... and their exclusive scan
-    cudaStream_t aux_stream = nullptr;   // the long-piece kernel runs here, next to the short-piece kernel
-    cudaStream_t aux2_stream = nullptr;  // ... and the big-piece kernel here, next to both
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_join2 = nullptr;
-    cudaStream_t side2[kSideStreams] = {};       // pipelined host calls: the big-piece kernel of sub-batch k
-    cudaEvent_t ev_list[kMaxPipeChunks] = {};
-    cudaEvent_t ev_ws = nullptr;         // recorded at the end of an asynchronous device-path call: the workspace is busy until then
+    Stream stream;                       // compute
+    Stream h2d_stream;                   // pipelined host calls: uploads run ahead of the kernels ...
+    Stream d2h_stream;                   // ... and downloads trail them
+    DevPtr<uint32_t> d_dec_sums;         // decode: bytes per tile of kDecodeTile tokens ...
+    DevPtr<uint64_t> d_dec_base;         // ... and their exclusive scan
+    Stream aux_stream;                   // the long-piece kernel runs here, next to the short-piece kernel
+    Stream aux2_stream;                  // ... and the big-piece kernel here, next to both
+    Event ev_fork, ev_join, ev_join2;
+    Stream side2[kSideStreams];          // pipelined host calls: the big-piece kernel of sub-batch k
+    Event ev_list[kMaxPipeChunks];
+    Event ev_ws;                         // recorded at the end of an asynchronous device-path call: the workspace is busy until then
     bool ws_pending = false;             // ... and whether one is outstanding
     uint64_t dev_out_cap = 0;            // out_cap of the last device-path call (cfbpe_device_status reports ENOSPC against it)
     bool dev_want_ids = false;
-    cudaEvent_t ev_scan[kMaxPipeChunks] = {};
-    cudaStream_t front[kFrontStreams] = {};   // front streams 1.. of a pipelined host call (0 = stream)
-    cudaStream_t pool[kPrioLevels][kPoolSlots] = {};   // CFBPE_PIPE_PRIO=1|2 (experiment): streams by priority level
+    Event ev_scan[kMaxPipeChunks];
+    Stream front[kFrontStreams];         // front streams 1.. of a pipelined host call (0 = stream)
+    Stream pool[kPrioLevels][kPoolSlots];   // CFBPE_PIPE_PRIO=1|2 (experiment): streams by priority level
     int prio_mode = 0, prio_levels = 1;
-    cudaStream_t side[kSideStreams] = {};  // long-piece tails + emit of sub-batch k overlap the front of k+1
-    cudaEvent_t ev_front[kMaxPipeChunks] = {};
-    cudaEvent_t ev_h2d[kMaxPipeChunks] = {};
-    cudaEvent_t ev_done[kMaxPipeChunks] = {};
-    cudaEvent_t ev_chain[kMaxPipeChunks] = {};   // tile_scan of sub-batch k done: the next sub-batch's scan may read tok_end
-    cudaEvent_t (*trace)[kTracePoints] = nullptr;           // CFBPE_PIPE_TRACE=1: timed events per sub-batch (h2d, split, short, long, back, d2h) + [nc][0] = start
-    DeviceStatus* d_status_arr = nullptr; // one status per sub-batch
-    DeviceStatus* h_status_arr = nullptr; // pinned
-    uint64_t* h_offs_stage = nullptr;     // pinned: sub-batch-local offsets
-    uint64_t* h_totals = nullptr;         // pinned: the all-gathered token totals of a multi-device call [CFBPE_MAX_DEVICES]
-    uint64_t* d_totals = nullptr;         // device: the same
+    Stream side[kSideStreams];           // long-piece tails + emit of sub-batch k overlap the front of k+1
+    Event ev_front[kMaxPipeChunks];
+    Event ev_h2d[kMaxPipeChunks];
+    Event ev_done[kMaxPipeChunks];
+    Event ev_chain[kMaxPipeChunks];      // tile_scan of sub-batch k done: the next sub-batch's scan may read tok_end
+    std::vector<std::array<Event, kTracePoints>> trace;   // CFBPE_PIPE_TRACE=1: timed events per sub-batch (h2d, split, short, long, back, d2h) + [nc][0] = start
+    DevPtr<DeviceStatus> d_status_arr;   // one status per sub-batch
+    HostPtr<DeviceStatus> h_status_arr;  // pinned
+    HostPtr<uint64_t> h_offs_stage;      // pinned: sub-batch-local offsets
+    HostPtr<uint64_t> h_totals;          // pinned: the all-gathered token totals of a multi-device call [CFBPE_MAX_DEVICES]
+    DevPtr<uint64_t> d_totals;           // device: the same
     // inputs / outputs of the host API
-    uint8_t* d_bytes = nullptr;
-    uint64_t* d_offsets = nullptr;
-    uint8_t* d_vocab_ids = nullptr;
-    uint32_t* d_out_ids = nullptr;
-    uint64_t* d_out_offsets = nullptr;
-    uint32_t* d_out_counts = nullptr;
-    uint32_t* d_out_starts = nullptr;    // host calls with token starts: [max_bytes + 1], allocated on the lane's first such call
-    uint32_t* d_trunc = nullptr;         // host truncate calls: budgets, cuts, kept counts [3 x (max_prompts + 1)], allocated on the
+    DevPtr<uint8_t> d_bytes;
+    DevPtr<uint64_t> d_offsets;
+    DevPtr<uint8_t> d_vocab_ids;
+    DevPtr<uint32_t> d_out_ids;
+    DevPtr<uint64_t> d_out_offsets;
+    DevPtr<uint32_t> d_out_counts;
+    DevPtr<uint32_t> d_out_starts;       // host calls with token starts: [max_bytes + 1], allocated on the lane's first such call
+    DevPtr<uint32_t> d_trunc;            // host truncate calls: budgets, cuts, kept counts [3 x (max_prompts + 1)], allocated on the
                                          // lane's first such call
-    uint64_t* d_chunk_offs = nullptr;    // host chunk calls: chunk offsets in the layout of d_out_offsets, then the shard chunk totals
+    DevPtr<uint64_t> d_chunk_offs;       // host chunk calls: chunk offsets in the layout of d_out_offsets, then the shard chunk totals
                                          // of a multi-device call [CFBPE_MAX_DEVICES]; allocated on the lane's first such call
-    Workspace ws{};
-    DeviceStatus* h_status = nullptr;  // pinned
+    Workspace ws{};                      // the kernels' view: its sized buffers are released by ~Lane, its status is d_status
+    DevPtr<DeviceStatus> d_status;
+    HostPtr<DeviceStatus> h_status;      // pinned
     ProfEvents prof{};
     LaneSpecial sp;
+
+    ~Lane() {                            // the members' deleters run after this body, on the lane's device
+        cudaSetDevice(device);
+        for_each_ws_buffer(ws, [](auto*& p, WsKind) { cudaFree(p); });
+    }
 };
 
-struct DeviceVocab { uint8_t* d_blob = nullptr; };
+struct DeviceVocab { DevPtr<uint8_t> d_blob; };
 
 struct DeviceCtx {
     int device = 0;
     int index = 0;                        // position in cfbpe_ctx::devs (= NCCL rank)
     int sm_count = 0;                     // set from the device's properties; 0 until then
-    uint8_t* d_uc1 = nullptr;
-    uint8_t* d_uc2 = nullptr;
-    uint8_t* d_ascii = nullptr;
-    uint16_t* d_fsm = nullptr;
-    uint8_t* d_split_tables = nullptr;   // SplitTablesHost: class bytes, 16-wide transition tables, context + product automata (pretok_ctx.h)
+    DevPtr<uint8_t> d_uc1;
+    DevPtr<uint8_t> d_uc2;
+    DevPtr<uint8_t> d_ascii;
+    DevPtr<uint16_t> d_fsm;
+    DevPtr<uint8_t> d_split_tables;      // SplitTablesHost: class bytes, 16-wide transition tables, context + product automata (pretok_ctx.h)
     UcTables uc{};
     DeviceVocab vocabs[CFBPE_MAX_VOCABS];
     VocabSet vs{};
-    uint32_t* d_specials[CFBPE_MAX_VOCABS] = {};   // each vocabulary's special-token table (specials.h), or nullptr
+    DevPtr<uint32_t> d_specials[CFBPE_MAX_VOCABS];   // each vocabulary's special-token table (specials.h), or empty
     SpecialSet specials{};                          // their views (modes NULL): what decode reads
     std::vector<std::unique_ptr<Lane>> lanes;
     std::atomic<uint32_t> next_lane{0};
     void* comm = nullptr;                 // ncclComm_t of this device in the context's communicator
+
+    ~DeviceCtx() { cudaSetDevice(device); }   // the members' deleters run after this body, on this device
 };
 
 struct HostVocab { bool loaded = false; std::vector<uint8_t> h_blob; TablesHeader hdr{}; };
@@ -215,6 +235,34 @@ int fail(cfbpe_ctx*, int code, const std::string& msg) {
 
 template <typename T>
 cudaError_t dmalloc(T** p, uint64_t count) { return cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T)); }
+// fill an owner: count elements of T on the current device (dmalloc) or in pinned host memory (hmalloc), a stream, an event; the
+// owner stays empty when the call fails
+template <typename T>
+cudaError_t dmalloc(DevPtr<T>& p, uint64_t count) {
+    T* raw = nullptr;
+    const cudaError_t e = dmalloc(&raw, count);
+    p.reset(e == cudaSuccess ? raw : nullptr);
+    return e;
+}
+template <typename T>
+cudaError_t hmalloc(HostPtr<T>& p, uint64_t count) {
+    void* raw = nullptr;
+    const cudaError_t e = cudaMallocHost(&raw, count * sizeof(T));
+    p.reset(e == cudaSuccess ? static_cast<T*>(raw) : nullptr);
+    return e;
+}
+cudaError_t make_stream(Stream& s, int priority) {
+    cudaStream_t raw = nullptr;
+    const cudaError_t e = cudaStreamCreateWithPriority(&raw, cudaStreamNonBlocking, priority);
+    s.reset(e == cudaSuccess ? raw : nullptr);
+    return e;
+}
+cudaError_t make_event(Event& ev, unsigned flags) {
+    cudaEvent_t raw = nullptr;
+    const cudaError_t e = cudaEventCreateWithFlags(&raw, flags);
+    ev.reset(e == cudaSuccess ? raw : nullptr);
+    return e;
+}
 
 // the error a pass's status reports (status_error), or CFBPE_OK
 int fail_status(cfbpe_ctx* ctx, const DeviceStatus& st) {
@@ -267,8 +315,7 @@ void clear_specials(cfbpe_ctx* ctx, uint32_t vocab_id) {
         if (dv->d_specials[vocab_id]) {
             cudaSetDevice(dv->device);
             cudaDeviceSynchronize();          // a device-path call may still read the table
-            cudaFree(dv->d_specials[vocab_id]);
-            dv->d_specials[vocab_id] = nullptr;
+            dv->d_specials[vocab_id].reset();
         }
     }
 }
@@ -278,30 +325,29 @@ void clear_specials(cfbpe_ctx* ctx, uint32_t vocab_id) {
 // file was parsed once, the tables crossed PCIe once.
 int install_blob(cfbpe_ctx* ctx, uint32_t vocab_id, std::vector<uint8_t>&& blob) {
     const size_t G = ctx->devs.size();
-    std::vector<uint8_t*> nb(G, nullptr);
-    auto cleanup = [&]() { for (size_t d = 0; d < G; ++d) { cudaSetDevice(ctx->devs[d]->device); cudaFree(nb[d]); } };
+    std::vector<DevPtr<uint8_t>> nb(G);      // the new tables, one a device: released on return unless installed
     for (size_t d = 0; d < G; ++d) {
         cudaSetDevice(ctx->devs[d]->device);
-        if (cudaMalloc(reinterpret_cast<void**>(&nb[d]), blob.size()) != cudaSuccess) {
-            cleanup(); cudaGetLastError();
+        if (dmalloc(nb[d], blob.size()) != cudaSuccess) {
+            cudaGetLastError();
             return fail(ctx, CFBPE_ENOMEM, "no device memory for the vocabulary tables");
         }
     }
     cudaSetDevice(ctx->devs[0]->device);
-    cudaError_t e = cudaMemcpy(nb[0], blob.data(), blob.size(), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { cleanup(); return fail(ctx, CFBPE_EIO, std::string("table upload: ") + cudaGetErrorString(e)); }
+    cudaError_t e = cudaMemcpy(nb[0].get(), blob.data(), blob.size(), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return fail(ctx, CFBPE_EIO, std::string("table upload: ") + cudaGetErrorString(e));
     if (G > 1) {
         const NcclApi& nc = ctx->nccl;
         int rc = nc.GroupStart();
         for (size_t d = 0; d < G && rc == 0; ++d) {
             cudaSetDevice(ctx->devs[d]->device);
-            cudaStream_t st = ctx->devs[d]->lanes[0]->stream;
-            rc = nc.Broadcast(nb[0], nb[d], blob.size(), kNcclChar, 0, ctx->devs[d]->comm, st);
+            cudaStream_t st = ctx->devs[d]->lanes[0]->stream.get();
+            rc = nc.Broadcast(nb[0].get(), nb[d].get(), blob.size(), kNcclChar, 0, ctx->devs[d]->comm, st);
         }
         const int rc2 = nc.GroupEnd();
         if (rc == 0) rc = rc2;
-        for (size_t d = 0; d < G; ++d) { cudaSetDevice(ctx->devs[d]->device); if (cudaStreamSynchronize(ctx->devs[d]->lanes[0]->stream) != cudaSuccess && rc == 0) rc = -1; }
-        if (rc != 0) { cleanup(); return fail(ctx, CFBPE_EIO, std::string("ncclBroadcast of the vocabulary tables: ") + (rc > 0 ? nc.GetErrorString(rc) : "stream error")); }
+        for (size_t d = 0; d < G; ++d) { cudaSetDevice(ctx->devs[d]->device); if (cudaStreamSynchronize(ctx->devs[d]->lanes[0]->stream.get()) != cudaSuccess && rc == 0) rc = -1; }
+        if (rc != 0) return fail(ctx, CFBPE_EIO, std::string("ncclBroadcast of the vocabulary tables: ") + (rc > 0 ? nc.GetErrorString(rc) : "stream error"));
     }
     clear_specials(ctx, vocab_id);           // a new vocabulary starts without special tokens
     HostVocab& hv = ctx->vocabs[vocab_id];
@@ -313,9 +359,9 @@ int install_blob(cfbpe_ctx* ctx, uint32_t vocab_id, std::vector<uint8_t>&& blob)
         DeviceCtx* dv = ctx->devs[d].get();
         cudaSetDevice(dv->device);
         DeviceVocab& v = dv->vocabs[vocab_id];
-        if (v.d_blob) { cudaDeviceSynchronize(); cudaFree(v.d_blob); }   // kernels of a device-path call on any stream may still read the old tables
-        v.d_blob = nb[d];
-        dv->vs.v[vocab_id] = make_view(v.d_blob, hv.hdr);
+        if (v.d_blob) cudaDeviceSynchronize();   // kernels of a device-path call on any stream may still read the old tables
+        v.d_blob = std::move(nb[d]);
+        dv->vs.v[vocab_id] = make_view(v.d_blob.get(), hv.hdr);
         dv->vs.loaded_mask = ctx->loaded_mask;
         // slots that are not loaded alias a loaded one: a bad vocabulary id handed in by a device-path caller is reported
         // (DeviceStatus::bad_vocab -> CFBPE_ENOENT) instead of dereferencing a null table
@@ -330,13 +376,13 @@ void fill_profile(Lane* ln, uint64_t n_bytes) {
     for (int k = 0; k < CFBPE_NUM_KERNELS; ++k) {
         if (!ln->prof.launched[k]) continue;
         float ms = 0;
-        if (cudaEventElapsedTime(&ms, ln->prof.ev[k][0], ln->prof.ev[k][1]) == cudaSuccess) p.kernel_ms[k] = ms;
+        if (cudaEventElapsedTime(&ms, ln->prof.ev[k][0].get(), ln->prof.ev[k][1].get()) == cudaSuccess) p.kernel_ms[k] = ms;
         p.kernel_launches[k] = (k == K_EMIT) ? 2 : 1;   // emit_compact + prompt_offsets
     }
     float ms = 0;
-    if (cudaEventElapsedTime(&ms, ln->prof.h2d[0], ln->prof.h2d[1]) == cudaSuccess) p.h2d_ms = ms;
-    if (cudaEventElapsedTime(&ms, ln->prof.d2h[0], ln->prof.d2h[1]) == cudaSuccess) p.d2h_ms = ms;
-    if (cudaEventElapsedTime(&ms, ln->prof.total[0], ln->prof.total[1]) == cudaSuccess) p.total_ms = ms;
+    if (cudaEventElapsedTime(&ms, ln->prof.h2d[0].get(), ln->prof.h2d[1].get()) == cudaSuccess) p.h2d_ms = ms;
+    if (cudaEventElapsedTime(&ms, ln->prof.d2h[0].get(), ln->prof.d2h[1].get()) == cudaSuccess) p.d2h_ms = ms;
+    if (cudaEventElapsedTime(&ms, ln->prof.total[0].get(), ln->prof.total[1].get()) == cudaSuccess) p.total_ms = ms;
     p.n_tokens = ln->h_status->n_tokens;
     p.n_long_pieces = static_cast<uint64_t>(ln->h_status->n_long) + ln->h_status->n_big;
     p.n_bytes = n_bytes;
@@ -349,15 +395,21 @@ void fill_profile(Lane* ln, uint64_t n_bytes) {
     tl_profile_ready = true;
 }
 
-// the lane's buffer of token starts (host calls of cfbpe_encode_batch_starts), allocated on its first such call: a context that never
-// asks for starts keeps the footprint it had.  The caller has selected the lane's device.
-int ensure_starts_lane(cfbpe_ctx* ctx, Lane* ln) {
-    if (ln->d_out_starts) return CFBPE_OK;
-    if (dmalloc(&ln->d_out_starts, ln->max_bytes + 1) != cudaSuccess) {
-        cudaGetLastError(); ln->d_out_starts = nullptr;
-        return fail(ctx, CFBPE_ENOMEM, "no device memory for the token starts");
-    }
-    return CFBPE_OK;
+// A lane buffer that only some calls use, allocated on the lane's first such call: a context that never makes one keeps the
+// footprint it had.  The caller has selected the lane's device.
+template <typename T>
+int ensure_lane_buffer(cfbpe_ctx* ctx, DevPtr<T>& p, uint64_t count, const char* what) {
+    if (p || dmalloc(p, count) == cudaSuccess) return CFBPE_OK;
+    cudaGetLastError();
+    return fail(ctx, CFBPE_ENOMEM, std::string("no device memory for ") + what);
+}
+// the lane buffers of a call with token starts (cfbpe_encode_batch_starts, chunk calls), of a truncate call, of a host chunk call
+int ensure_call_buffers(cfbpe_ctx* ctx, Lane* ln, bool starts, bool trunc, bool chunk) {
+    const uint64_t mp = ctx->max_prompts;
+    int rc = starts ? ensure_lane_buffer(ctx, ln->d_out_starts, ln->max_bytes + 1, "the token starts") : CFBPE_OK;
+    if (!rc && trunc) rc = ensure_lane_buffer(ctx, ln->d_trunc, 3 * (mp + 1), "the truncate buffers");
+    if (!rc && chunk) rc = ensure_lane_buffer(ctx, ln->d_chunk_offs, lane_offsets_alloc(mp, kMaxPipeChunks) + CFBPE_MAX_DEVICES, "the chunk offsets");
+    return rc;
 }
 
 // A host truncate call (cfbpe_truncate_batch): budgets in, cuts and kept counts out, one per prompt of the call.  The ids it needs go to
@@ -365,23 +417,13 @@ int ensure_starts_lane(cfbpe_ctx* ctx, Lane* ln) {
 struct TruncateArgs { const uint32_t* budgets; uint32_t tail; uint32_t* cut; uint32_t* kept; };
 TruncateArgs truncate_from(const TruncateArgs& t, uint32_t p0) { return TruncateArgs{t.budgets + p0, t.tail, t.cut + p0, t.kept + p0}; }
 
-// the lane's truncate buffers (host truncate calls), allocated on its first such call: a context that never truncates keeps the
-// footprint it had.  The caller has selected the lane's device.
-int ensure_truncate_lane(cfbpe_ctx* ctx, Lane* ln) {
-    if (ln->d_trunc) return CFBPE_OK;
-    if (dmalloc(&ln->d_trunc, 3 * (static_cast<uint64_t>(ctx->max_prompts) + 1)) != cudaSuccess) {
-        cudaGetLastError(); ln->d_trunc = nullptr;
-        return fail(ctx, CFBPE_ENOMEM, "no device memory for the truncate buffers");
-    }
-    return CFBPE_OK;
-}
 // prompts p0 .. of the call in the lane's truncate buffers (a sub-batch's prompts keep their index in the call)
 TruncateView lane_truncate_view(cfbpe_ctx* ctx, Lane* ln, uint32_t tail, uint32_t p0) {
     const uint64_t m = static_cast<uint64_t>(ctx->max_prompts) + 1;
-    return TruncateView{ln->d_trunc + p0, tail, ln->d_trunc + m + p0, ln->d_trunc + 2 * m + p0};
+    return TruncateView{ln->d_trunc.get() + p0, tail, ln->d_trunc.get() + m + p0, ln->d_trunc.get() + 2 * m + p0};
 }
 int upload_budgets(cfbpe_ctx* ctx, Lane* ln, const TruncateArgs& t, uint32_t p0, uint32_t n, cudaStream_t s) {
-    if (n) CK(cudaMemcpyAsync(ln->d_trunc + p0, t.budgets + p0, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    if (n) CK(cudaMemcpyAsync(ln->d_trunc.get() + p0, t.budgets + p0, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     return CFBPE_OK;
 }
 int download_cuts(cfbpe_ctx* ctx, Lane* ln, const TruncateArgs& t, uint32_t p0, uint32_t n, cudaStream_t s) {
@@ -397,22 +439,12 @@ int download_cuts(cfbpe_ctx* ctx, Lane* ln, const TruncateArgs& t, uint32_t p0, 
 // multi-device call): gets every sub-batch's chunk_end (shard-local ranks), for the downloads after the shards' totals are known.
 struct ChunkArgs { uint32_t n, step; uint32_t* spans; uint64_t cap; uint64_t* offsets; uint64_t* sub_end; };
 
-// the lane's chunk-offset buffer (host chunk calls), allocated on its first such call: a context that never chunks keeps the
-// footprint it had.  The caller has selected the lane's device.
-int ensure_chunk_lane(cfbpe_ctx* ctx, Lane* ln) {
-    if (ln->d_chunk_offs) return CFBPE_OK;
-    if (dmalloc(&ln->d_chunk_offs, lane_offsets_alloc(ctx->max_prompts, kMaxPipeChunks) + CFBPE_MAX_DEVICES) != cudaSuccess) {
-        cudaGetLastError(); ln->d_chunk_offs = nullptr;
-        return fail(ctx, CFBPE_ENOMEM, "no device memory for the chunk offsets");
-    }
-    return CFBPE_OK;
-}
-uint64_t* lane_chunk_totals(cfbpe_ctx* ctx, Lane* ln) { return ln->d_chunk_offs + lane_offsets_alloc(ctx->max_prompts, kMaxPipeChunks); }
+uint64_t* lane_chunk_totals(cfbpe_ctx* ctx, Lane* ln) { return ln->d_chunk_offs.get() + lane_offsets_alloc(ctx->max_prompts, kMaxPipeChunks); }
 // a host call's chunks of the (sub-)batch with workspace w and offsets at q0: the offsets to the lane's buffer, the spans staged
 // in w's per-byte scratch, which is dead once the ids are out (begins in ids_by_pos, ends in dense.by_piece: a (sub-)batch has
 // no more chunks than tokens and no more tokens than bytes); base: the previous sub-batch's chunk_end, or nullptr
 ChunkView lane_chunk_view(Lane* ln, const Workspace& w, uint64_t q0, const uint64_t* base, const ChunkArgs& c) {
-    return ChunkView{c.n, c.step, ln->d_chunk_offs + q0, base, w.ids_by_pos, w.dense.by_piece, 1u, UINT64_MAX};
+    return ChunkView{c.n, c.step, ln->d_chunk_offs.get() + q0, base, w.ids_by_pos, w.dense.by_piece, 1u, UINT64_MAX};
 }
 // chunks [first, first + count) of the call, staged by lane_chunk_view in w, to their (begin, end) pairs in spans
 int download_spans(cfbpe_ctx* ctx, const Workspace& w, uint32_t* spans, uint64_t first, uint64_t count, cudaStream_t s) {
@@ -429,17 +461,17 @@ int fail_chunk_nospace(cfbpe_ctx* ctx, uint64_t need, uint64_t* offsets, uint32_
 
 // an asynchronous device-path call may still own the lane's workspace: wait for it (the caller has selected the lane's device)
 int wait_for_device_call(cfbpe_ctx* ctx, Lane* ln) {
-    if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws)); ln->ws_pending = false; }
+    if (ln->ws_pending) { CK(cudaEventSynchronize(ln->ev_ws.get())); ln->ws_pending = false; }
     return CFBPE_OK;
 }
 
 // the inputs of a one-pass host call into the lane's buffers, on s; *b: the batch as the kernels see it
 int upload_batch(cfbpe_ctx* ctx, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids, uint64_t total,
                  cudaStream_t s, BatchView* b) {
-    if (total) CK(cudaMemcpyAsync(ln->d_bytes, bytes, total, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ln->d_offsets, offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-    if (vocab_ids && n) CK(cudaMemcpyAsync(ln->d_vocab_ids, vocab_ids, n, cudaMemcpyHostToDevice, s));
-    *b = BatchView{ln->d_bytes, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n, total};
+    if (total) CK(cudaMemcpyAsync(ln->d_bytes.get(), bytes, total, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ln->d_offsets.get(), offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    if (vocab_ids && n) CK(cudaMemcpyAsync(ln->d_vocab_ids.get(), vocab_ids, n, cudaMemcpyHostToDevice, s));
+    *b = BatchView{ln->d_bytes.get(), ln->d_offsets.get(), vocab_ids ? ln->d_vocab_ids.get() : nullptr, n, total};
     return CFBPE_OK;
 }
 
@@ -470,17 +502,17 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
     for (int k = 0; k < nc; ++k) {
         const uint32_t p0 = cut[k], p1 = cut[k + 1];
         const uint64_t o0 = offsets[p0];
-        uint64_t* dst = ln->h_offs_stage + sub_batch_offsets_at(p0, k);
+        uint64_t* dst = ln->h_offs_stage.get() + sub_batch_offsets_at(p0, k);
         for (uint32_t i = p0; i <= p1; ++i) dst[i - p0] = offsets[i] - o0;
     }
     // ---- enqueue everything that does not depend on the host knowing a result
     const bool trace = G == 1 && getenv("CFBPE_PIPE_TRACE") != nullptr;
     const bool no_copy = trace && getenv("CFBPE_PIPE_NO_COPY") != nullptr;   // measurement aid: the kernels of a pipelined call without its copies (the device buffers still hold the previous call's data)
-    if (trace && !ln->trace) {
-        ln->trace = new cudaEvent_t[kMaxPipeChunks + 1][kTracePoints];
-        for (int k = 0; k <= kMaxPipeChunks; ++k) for (int j = 0; j < kTracePoints; ++j) cudaEventCreate(&ln->trace[k][j]);
+    if (trace && ln->trace.empty()) {
+        ln->trace.resize(kMaxPipeChunks + 1);
+        for (auto& events : ln->trace) for (Event& e : events) make_event(e, cudaEventDefault);
     }
-    if (trace) CK(cudaEventRecord(ln->trace[nc][0], ln->h2d_stream));
+    if (trace) CK(cudaEventRecord(ln->trace[nc][0].get(), ln->h2d_stream.get()));
     const auto host_t0 = std::chrono::steady_clock::now();
     auto host_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count(); };
     double host_enq[kMaxPipeChunks] = {}, host_dl[kMaxPipeChunks] = {};
@@ -489,58 +521,58 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         Lane* const ln = lns[k % G];
         Lane* const prev = k ? lns[(k - 1) % G] : nullptr;
         if (G > 1) CK(cudaSetDevice(dv->device));
-        cudaStream_t cs = ln->stream, hs = ln->h2d_stream;
+        cudaStream_t cs = ln->stream.get(), hs = ln->h2d_stream.get();
         const uint32_t p0 = cut[k], p1 = cut[k + 1], nk = p1 - p0;
         const uint64_t o0 = offsets[p0], len = offsets[p1] - o0, q0 = sub_batch_offsets_at(p0, k);
-        uint8_t* const d_sub = ln->d_bytes + sub_batch_bytes_at(o0, k);
+        uint8_t* const d_sub = ln->d_bytes.get() + sub_batch_bytes_at(o0, k);
         if (len && !no_copy) CK(cudaMemcpyAsync(d_sub, bytes + o0, len, cudaMemcpyHostToDevice, hs));
-        CK(cudaMemcpyAsync(ln->d_offsets + q0, lns[0]->h_offs_stage + q0, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, hs));
-        if (vocab_ids && nk) CK(cudaMemcpyAsync(ln->d_vocab_ids + p0, vocab_ids + p0, nk, cudaMemcpyHostToDevice, hs));
+        CK(cudaMemcpyAsync(ln->d_offsets.get() + q0, lns[0]->h_offs_stage.get() + q0, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, hs));
+        if (vocab_ids && nk) CK(cudaMemcpyAsync(ln->d_vocab_ids.get() + p0, vocab_ids + p0, nk, cudaMemcpyHostToDevice, hs));
         if (trunc) { const int rc = upload_budgets(ctx, ln, *trunc, p0, nk, hs); if (rc) return rc; }
-        CK(cudaEventRecord(ln->ev_h2d[k], hs));
-        if (trace) CK(cudaEventRecord(ln->trace[k][0], hs));
+        CK(cudaEventRecord(ln->ev_h2d[k].get(), hs));
+        if (trace) CK(cudaEventRecord(ln->trace[k][0].get(), hs));
         const int fk = k < kFrontStreams ? k : kFrontStreams - 1;
-        cudaStream_t ck = fk ? ln->front[fk] : cs;
+        cudaStream_t ck = fk ? ln->front[fk].get() : cs;
         const int lv = ln->prio_mode == 2 ? (k * ln->prio_levels) / nc : 0;
-        if (ln->prio_mode) ck = ln->pool[lv][(3 * k + 2) % kPoolSlots];   // the short-piece kernels of sub-batch k: priority falls with k (earlier sub-batches finish, and download, first)
+        if (ln->prio_mode) ck = ln->pool[lv][(3 * k + 2) % kPoolSlots].get();   // the short-piece kernels of sub-batch k: priority falls with k (earlier sub-batches finish, and download, first)
         Workspace w = slice_workspace(ln->ws, o0, len, static_cast<uint32_t>(k));
-        w.status = ln->d_status_arr + k;
-        BatchView b{d_sub, ln->d_offsets + q0, vocab_ids ? ln->d_vocab_ids + p0 : nullptr, nk, len};
+        w.status = ln->d_status_arr.get() + k;
+        BatchView b{d_sub, ln->d_offsets.get() + q0, vocab_ids ? ln->d_vocab_ids.get() + p0 : nullptr, nk, len};
         // split, long pieces and the back stage run on a top-priority stream of their own: the long-piece kernels are a latency
         // chain that uses little of the machine, so they start as early as possible and the short-piece kernels fill the rest
-        cudaStream_t ss = ln->prio_mode ? ln->pool[lv][(3 * k) % kPoolSlots] : ln->side[k % kSideStreams];
-        CK(cudaStreamWaitEvent(ss, ln->ev_h2d[k], 0));
+        cudaStream_t ss = ln->prio_mode ? ln->pool[lv][(3 * k) % kPoolSlots].get() : ln->side[k % kSideStreams].get();
+        CK(cudaStreamWaitEvent(ss, ln->ev_h2d[k].get(), 0));
         enqueue_split(b, dv->vs, dv->uc, w, ss, static_cast<ProfEvents*>(nullptr), static_cast<uint32_t>(dv->sm_count));
-        CK(cudaEventRecord(ln->ev_scan[k], ss));
-        if (trace) CK(cudaEventRecord(ln->trace[k][1], ss));
-        CK(cudaStreamWaitEvent(ck, ln->ev_scan[k], 0));
-        cudaStream_t ss2 = ln->prio_mode ? ln->pool[lv][(3 * k + 1) % kPoolSlots] : ln->side2[k % kSideStreams];
-        CK(cudaStreamWaitEvent(ss2, ln->ev_scan[k], 0));
+        CK(cudaEventRecord(ln->ev_scan[k].get(), ss));
+        if (trace) CK(cudaEventRecord(ln->trace[k][1].get(), ss));
+        CK(cudaStreamWaitEvent(ck, ln->ev_scan[k].get(), 0));
+        cudaStream_t ss2 = ln->prio_mode ? ln->pool[lv][(3 * k + 1) % kPoolSlots].get() : ln->side2[k % kSideStreams].get();
+        CK(cudaStreamWaitEvent(ss2, ln->ev_scan[k].get(), 0));
         enqueue_list(b, dv->vs, w, static_cast<uint32_t>(dv->sm_count * 4), ss2, static_cast<ProfEvents*>(nullptr));   // the big pieces, beside everything else
-        CK(cudaEventRecord(ln->ev_list[k], ss2));
-        if (trace) CK(cudaEventRecord(ln->trace[k][6], ss2));
+        CK(cudaEventRecord(ln->ev_list[k].get(), ss2));
+        if (trace) CK(cudaEventRecord(ln->trace[k][6].get(), ss2));
         enqueue_long(b, dv->vs, w, static_cast<uint32_t>(dv->sm_count * 4), ss, static_cast<ProfEvents*>(nullptr));   // tail overlaps what follows on cs
-        if (trace) CK(cudaEventRecord(ln->trace[k][3], ss));
+        if (trace) CK(cudaEventRecord(ln->trace[k][3].get(), ss));
         enqueue_short(b, dv->vs, w, static_cast<uint32_t>(dv->sm_count * 4), ck, static_cast<ProfEvents*>(nullptr));
-        CK(cudaEventRecord(ln->ev_front[k], ck));
-        if (trace) CK(cudaEventRecord(ln->trace[k][2], ck));
-        CK(cudaStreamWaitEvent(ss, ln->ev_front[k], 0));
-        CK(cudaStreamWaitEvent(ss, ln->ev_list[k], 0));
+        CK(cudaEventRecord(ln->ev_front[k].get(), ck));
+        if (trace) CK(cudaEventRecord(ln->trace[k][2].get(), ck));
+        CK(cudaStreamWaitEvent(ss, ln->ev_front[k].get(), 0));
+        CK(cudaStreamWaitEvent(ss, ln->ev_list[k].get(), 0));
         enqueue_count(b, w, ss, static_cast<ProfEvents*>(nullptr));
-        if (trace) CK(cudaEventRecord(ln->trace[k][7], ss));
-        if (k) CK(cudaStreamWaitEvent(ss, prev->ev_chain[k - 1], 0));    // token ranks chain through DeviceStatus::tok_end: only the scan waits
-        enqueue_scan(b, w, ss, static_cast<ProfEvents*>(nullptr), k ? &prev->d_status_arr[k - 1].tok_end : nullptr);   // (G > 1: a peer pointer)
-        if (!chunk) CK(cudaEventRecord(ln->ev_chain[k], ss));
+        if (trace) CK(cudaEventRecord(ln->trace[k][7].get(), ss));
+        if (k) CK(cudaStreamWaitEvent(ss, prev->ev_chain[k - 1].get(), 0));    // token ranks chain through DeviceStatus::tok_end: only the scan waits
+        enqueue_scan(b, w, ss, static_cast<ProfEvents*>(nullptr), k ? &prev->d_status_arr.get()[k - 1].tok_end : nullptr);   // (G > 1: a peer pointer)
+        if (!chunk) CK(cudaEventRecord(ln->ev_chain[k].get(), ss));
         const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, p0) : TruncateView{};
-        const ChunkView cv = chunk ? lane_chunk_view(ln, w, q0, k ? &prev->d_status_arr[k - 1].chunk_end : nullptr, *chunk) : ChunkView{};
-        enqueue_emit(b, w, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets + q0, ln->d_out_counts + p0,
-                     ss, static_cast<ProfEvents*>(nullptr), (out_starts || chunk) ? ln->d_out_starts : nullptr, &dv->vs, trunc ? &tv : nullptr,
+        const ChunkView cv = chunk ? lane_chunk_view(ln, w, q0, k ? &prev->d_status_arr.get()[k - 1].chunk_end : nullptr, *chunk) : ChunkView{};
+        enqueue_emit(b, w, want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get() + q0, ln->d_out_counts.get() + p0,
+                     ss, static_cast<ProfEvents*>(nullptr), (out_starts || chunk) ? ln->d_out_starts.get() : nullptr, &dv->vs, trunc ? &tv : nullptr,
                      chunk ? &cv : nullptr);
-        if (chunk) CK(cudaEventRecord(ln->ev_chain[k], ss));       // (the chunk scan read the previous chunk_end: the chain ends here)
+        if (chunk) CK(cudaEventRecord(ln->ev_chain[k].get(), ss));       // (the chunk scan read the previous chunk_end: the chain ends here)
         CK(cudaGetLastError());
-        status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr + k, ln->h_status_arr + k);
-        CK(cudaEventRecord(ln->ev_done[k], ss));
-        if (trace) { CK(cudaEventRecord(ln->trace[k][4], ss)); host_enq[k] = host_ms(); }
+        status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr.get() + k, ln->h_status_arr.get() + k);
+        CK(cudaEventRecord(ln->ev_done[k].get(), ss));
+        if (trace) { CK(cudaEventRecord(ln->trace[k][4].get(), ss)); host_enq[k] = host_ms(); }
     }
     // ---- trail the kernels with the downloads
     int err = CFBPE_OK;
@@ -548,9 +580,9 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
     for (int k = 0; k < nc; ++k) {
         Lane* const ln = lns[k % G];
         if (G > 1) CK(cudaSetDevice(dvs[k % G]->device));
-        cudaStream_t ds = ln->d2h_stream;
-        CK(cudaEventSynchronize(ln->ev_done[k]));
-        const DeviceStatus st = ln->h_status_arr[k];
+        cudaStream_t ds = ln->d2h_stream.get();
+        CK(cudaEventSynchronize(ln->ev_done[k].get()));
+        const DeviceStatus st = ln->h_status_arr.get()[k];
         const uint32_t p0 = cut[k], p1 = cut[k + 1], nk = p1 - p0;
         if (!err) err = fail_status(ctx, st);
         const uint64_t base = st.tok_end - st.n_tokens;
@@ -561,35 +593,35 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (no_copy) continue;
         if (chunk) {
             const uint64_t q0 = sub_batch_offsets_at(p0, k);
-            CK(cudaMemcpyAsync(chunk->offsets + p0, ln->d_chunk_offs + q0, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
+            CK(cudaMemcpyAsync(chunk->offsets + p0, ln->d_chunk_offs.get() + q0, (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
             if (st.chunk_end <= chunk->cap) {
                 const Workspace w = slice_workspace(ln->ws, offsets[p0], offsets[p1] - offsets[p0], static_cast<uint32_t>(k));
                 if (const int rc = download_spans(ctx, w, chunk->spans, st.chunk_end - st.n_chunks, st.n_chunks, ds)) return rc;
             }
         }
         if (want_ids && out_ids && st.tok_end <= out_cap && st.n_tokens)
-            CK(cudaMemcpyAsync(out_ids + base, ln->d_out_ids + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
+            CK(cudaMemcpyAsync(out_ids + base, ln->d_out_ids.get() + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (out_starts && st.tok_end <= out_cap && st.n_tokens)      // (prompt-relative: the same ranks and base as the ids)
-            CK(cudaMemcpyAsync(out_starts + base, ln->d_out_starts + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
-        if (out_offsets) CK(cudaMemcpyAsync(out_offsets + p0, ln->d_out_offsets + sub_batch_offsets_at(p0, k), (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
-        if (out_counts && nk) CK(cudaMemcpyAsync(out_counts + p0, ln->d_out_counts + p0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
-        if (trace) { CK(cudaEventRecord(ln->trace[k][5], ds)); host_dl[k] = host_ms(); }
+            CK(cudaMemcpyAsync(out_starts + base, ln->d_out_starts.get() + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
+        if (out_offsets) CK(cudaMemcpyAsync(out_offsets + p0, ln->d_out_offsets.get() + sub_batch_offsets_at(p0, k), (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
+        if (out_counts && nk) CK(cudaMemcpyAsync(out_counts + p0, ln->d_out_counts.get() + p0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
+        if (trace) { CK(cudaEventRecord(ln->trace[k][5].get(), ds)); host_dl[k] = host_ms(); }
     }
     for (int g = 0; g < G; ++g) {
         Lane* const lg = lns[g];
         if (G > 1) CK(cudaSetDevice(dvs[g]->device));
-        CK(cudaStreamSynchronize(lg->d2h_stream));
-        CK(cudaStreamSynchronize(lg->stream));
-        for (int k = 1; k < kFrontStreams; ++k) CK(cudaStreamSynchronize(lg->front[k]));
-        for (int k = 0; k < kSideStreams; ++k) CK(cudaStreamSynchronize(lg->side[k]));
-        for (int k = 0; k < kSideStreams; ++k) CK(cudaStreamSynchronize(lg->side2[k]));
-        if (lg->prio_mode) for (int l = 0; l < kPrioLevels; ++l) for (int j = 0; j < kPoolSlots; ++j) if (lg->pool[l][j]) CK(cudaStreamSynchronize(lg->pool[l][j]));
+        CK(cudaStreamSynchronize(lg->d2h_stream.get()));
+        CK(cudaStreamSynchronize(lg->stream.get()));
+        for (int k = 1; k < kFrontStreams; ++k) CK(cudaStreamSynchronize(lg->front[k].get()));
+        for (int k = 0; k < kSideStreams; ++k) CK(cudaStreamSynchronize(lg->side[k].get()));
+        for (int k = 0; k < kSideStreams; ++k) CK(cudaStreamSynchronize(lg->side2[k].get()));
+        if (lg->prio_mode) for (int l = 0; l < kPrioLevels; ++l) for (int j = 0; j < kPoolSlots; ++j) if (lg->pool[l][j]) CK(cudaStreamSynchronize(lg->pool[l][j].get()));
     }
     if (trace && !err) {
         fprintf(stderr, "pipe trace (ms since the first upload was enqueued): sub-batch bytes | h2d split long_end list_end short count back d2h\n");
         for (int k = 0; k < nc; ++k) {
             float t[kTracePoints] = {};
-            for (int j = 0; j < kTracePoints; ++j) if (!(no_copy && j == 5)) cudaEventElapsedTime(&t[j], ln->trace[nc][0], ln->trace[k][j]);
+            for (int j = 0; j < kTracePoints; ++j) if (!(no_copy && j == 5)) cudaEventElapsedTime(&t[j], ln->trace[nc][0].get(), ln->trace[k][j].get());
             fprintf(stderr, "  %2d %9llu | %6.2f %6.2f %6.2f %6.2f %6.2f %6.2f %6.2f %6.2f | host: enqueued %.2f download issued %.2f\n", k,
                     static_cast<unsigned long long>(offsets[cut[k + 1]] - offsets[cut[k]]), t[0], t[1], t[3], t[6], t[2], t[7], t[4], t[5], host_enq[k], host_dl[k]);
         }
@@ -613,37 +645,35 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
              const ChunkArgs* chunk = nullptr) {
     CK(cudaSetDevice(dv->device));
     int rc = wait_for_device_call(ctx, ln);
-    if (!rc && (out_starts || chunk)) rc = ensure_starts_lane(ctx, ln);
-    if (!rc && trunc) rc = ensure_truncate_lane(ctx, ln);
-    if (!rc && chunk) rc = ensure_chunk_lane(ctx, ln);
+    if (!rc) rc = ensure_call_buffers(ctx, ln, out_starts || chunk, trunc != nullptr, chunk != nullptr);
     if (rc) return rc;
     const bool profiling = ctx->profiling.load();
     if (!profiling && total >= ctx->pipe_min && n >= 2)
         return run_host_pipelined(ctx, &dv, &ln, 1, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
                                   defer, cut_out, nc_out, trunc, chunk);
-    cudaStream_t s = ln->stream;
+    cudaStream_t s = ln->stream.get();
     ProfEvents* prof = profiling ? &ln->prof : nullptr;
-    if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); }
+    if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0].get(), s); cudaEventRecord(prof->h2d[0].get(), s); }
     BatchView b;
     rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b);
     if (!rc && trunc) rc = upload_budgets(ctx, ln, *trunc, 0, n, s);
     if (rc) return rc;
-    if (prof) cudaEventRecord(prof->h2d[1], s);
+    if (prof) cudaEventRecord(prof->h2d[1].get(), s);
 
     const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, 0) : TruncateView{};
     const ChunkView cv = chunk ? lane_chunk_view(ln, ln->ws, 0, nullptr, *chunk) : ChunkView{};
-    enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets,
-                   ln->d_out_counts, static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                   ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, (out_starts || chunk) ? ln->d_out_starts : nullptr, trunc ? &tv : nullptr,
+    enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get(),
+                   ln->d_out_counts.get(), static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
+                   ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, (out_starts || chunk) ? ln->d_out_starts.get() : nullptr, trunc ? &tv : nullptr,
                    chunk ? &cv : nullptr);
     CK(cudaGetLastError());
-    if (prof) cudaEventRecord(prof->d2h[0], s);
-    CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    if (prof) cudaEventRecord(prof->d2h[0].get(), s);
+    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     if (trunc && (rc = download_cuts(ctx, ln, *trunc, 0, n, s))) return rc;
     if (!defer) {
-        if (out_offsets) CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
-        if (out_counts && n) CK(cudaMemcpyAsync(out_counts, ln->d_out_counts, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-        if (chunk) CK(cudaMemcpyAsync(chunk->offsets, ln->d_chunk_offs, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+        if (out_offsets) CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets.get(), (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+        if (out_counts && n) CK(cudaMemcpyAsync(out_counts, ln->d_out_counts.get(), static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        if (chunk) CK(cudaMemcpyAsync(chunk->offsets, ln->d_chunk_offs.get(), (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     }
     CK(cudaStreamSynchronize(s));
     const DeviceStatus st = *ln->h_status;
@@ -660,10 +690,10 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     }
     if (want_ids) {
         if (st.n_tokens > out_cap) return fail_nospace(ctx, st.n_tokens, out_offsets, n);
-        if (out_ids && st.n_tokens) CK(cudaMemcpyAsync(out_ids, ln->d_out_ids, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-        if (out_starts && st.n_tokens) CK(cudaMemcpyAsync(out_starts, ln->d_out_starts, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        if (out_ids && st.n_tokens) CK(cudaMemcpyAsync(out_ids, ln->d_out_ids.get(), st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        if (out_starts && st.n_tokens) CK(cudaMemcpyAsync(out_starts, ln->d_out_starts.get(), st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     }
-    if (prof) { cudaEventRecord(prof->d2h[1], s); cudaEventRecord(prof->total[1], s); }
+    if (prof) { cudaEventRecord(prof->d2h[1].get(), s); cudaEventRecord(prof->total[1].get(), s); }
     CK(cudaStreamSynchronize(s));
     if (prof) fill_profile(ln, total);
     return CFBPE_OK;
@@ -684,37 +714,31 @@ int fail_disallowed(cfbpe_ctx* ctx, uint32_t prompt, uint32_t vid, uint32_t k, u
                                     "), which this call disallows");
 }
 
+// the lane's special buffers, all or none: they are built aside and installed once every allocation succeeded (on a failure, what
+// was allocated is released on return).  The caller has selected the lane's device.
 int ensure_special_lane(cfbpe_ctx* ctx, Lane* ln) {
-    LaneSpecial& sp = ln->sp;
-    if (sp.ready) return CFBPE_OK;
+    if (ln->sp.h_status) return CFBPE_OK;
     const uint64_t mp = ctx->max_prompts;
-    bool ok = dmalloc(&sp.kept_n, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&sp.kept_base, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&sp.st_off, mp + 2) == cudaSuccess;
-    ok = ok && dmalloc(&sp.st_vocab, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&sp.st_id, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&sp.st_base, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&sp.fin_offsets, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&sp.fin_counts, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&sp.modes, static_cast<uint64_t>(CFBPE_MAX_VOCABS) * kMaxSpecials) == cudaSuccess;
-    ok = ok && dmalloc(&sp.status, 1) == cudaSuccess;
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&sp.h_status), sizeof(SpecialStatus)) == cudaSuccess;
+    LaneSpecial sp;
+    bool ok = dmalloc(sp.kept_n, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(sp.kept_base, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(sp.st_off, mp + 2) == cudaSuccess;
+    ok = ok && dmalloc(sp.st_vocab, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(sp.st_id, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(sp.st_base, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(sp.fin_offsets, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(sp.fin_counts, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(sp.modes, static_cast<uint64_t>(CFBPE_MAX_VOCABS) * kMaxSpecials) == cudaSuccess;
+    ok = ok && dmalloc(sp.status, 1) == cudaSuccess;
+    ok = ok && hmalloc(sp.h_status, 1) == cudaSuccess;
     if (!ok) { cudaGetLastError(); return fail(ctx, CFBPE_ENOMEM, "no device memory for the special-token buffers"); }
-    sp.ready = true;
+    ln->sp = std::move(sp);
     return CFBPE_OK;
-}
-
-void free_special_lane(Lane* ln) {
-    LaneSpecial& sp = ln->sp;
-    cudaFree(sp.kept_n); cudaFree(sp.kept_base); cudaFree(sp.st_off); cudaFree(sp.st_vocab); cudaFree(sp.st_id); cudaFree(sp.st_base);
-    cudaFree(sp.fin_offsets); cudaFree(sp.fin_counts); cudaFree(sp.modes); cudaFree(sp.status);
-    if (sp.h_status) cudaFreeHost(sp.h_status);
-    sp = LaneSpecial{};
 }
 
 SpecialWork special_work(Lane* ln) {
     const LaneSpecial& sp = ln->sp;
-    return SpecialWork{sp.kept_n, sp.kept_base, sp.st_off, sp.st_vocab, sp.st_id, sp.st_base, sp.status};
+    return SpecialWork{sp.kept_n.get(), sp.kept_base.get(), sp.st_off.get(), sp.st_vocab.get(), sp.st_id.get(), sp.st_base.get(), sp.status.get()};
 }
 
 // The special set of one call on device dv (fill_special_set), with the lane's special buffers allocated and the call's mode bytes
@@ -729,7 +753,7 @@ int special_set(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const uint8_t* const* m
         return fail(ctx, CFBPE_EINVAL, "modes[" + std::to_string(bad[0]) + "][" + std::to_string(bad[1]) + "] is not a CFBPE_SPECIAL_* value");
     for (uint32_t v = 0; v < CFBPE_MAX_VOCABS; ++v) {
         if (!out->modes[v]) continue;
-        uint8_t* dm = ln->sp.modes + static_cast<uint64_t>(v) * kMaxSpecials;
+        uint8_t* dm = ln->sp.modes.get() + static_cast<uint64_t>(v) * kMaxSpecials;
         CK(cudaMemcpyAsync(dm, out->modes[v], words[v][0], cudaMemcpyHostToDevice, s));
         out->modes[v] = dm;
     }
@@ -749,7 +773,7 @@ int enqueue_special_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchVie
     if (scan) {       // the one synchronisation of the call: the host needs the number of stretches for the launch geometry
         enqueue_special_scan(b, sp, ln->ws, sw, s);
         CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(ln->sp.h_status.get(), ln->sp.status.get(), sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         const SpecialScanResult r = special_scan_result(*ln->sp.h_status, b.n_prompts, ctx->max_prompts);
         if (r.disallowed) return fail_disallowed(ctx, r.prompt, r.vocab, r.index, out_bad);
@@ -761,11 +785,11 @@ int enqueue_special_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchVie
     const uint32_t grid = static_cast<uint32_t>(dv->sm_count * 4);
     if (!*did_splice) {
         enqueue_encode(b, dv->vs, dv->uc, ln->ws, plain.ids, plain.cap, plain.offsets, plain.counts, grid,
-                       s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+                       s, ln->aux_stream.get(), ln->aux2_stream.get(), ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), static_cast<ProfEvents*>(nullptr));
     } else {
-        enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets,
-                               ln->d_out_counts, spliced.ids, spliced.cap, spliced.offsets, spliced.counts,
-                               grid, s, ln->aux_stream, ln->aux2_stream, ln->ev_fork, ln->ev_join, ln->ev_join2, static_cast<ProfEvents*>(nullptr));
+        enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids.get(), ctx->max_bytes, ln->d_out_offsets.get(),
+                               ln->d_out_counts.get(), spliced.ids, spliced.cap, spliced.offsets, spliced.counts,
+                               grid, s, ln->aux_stream.get(), ln->aux2_stream.get(), ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), static_cast<ProfEvents*>(nullptr));
     }
     CK(cudaGetLastError());
     return CFBPE_OK;
@@ -845,9 +869,9 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     for (uint32_t d = 0; d < G && nrc == 0; ++d) {
         Lane* ln = locks[d]->ln;
         cudaSetDevice(ctx->devs[d]->device);
-        ln->h_totals[CFBPE_MAX_DEVICES] = sh[d].tokens;                                   // (slot past the gathered ones: this shard's own total)
-        cudaMemcpyAsync(ln->d_totals + CFBPE_MAX_DEVICES, ln->h_totals + CFBPE_MAX_DEVICES, sizeof(uint64_t), cudaMemcpyHostToDevice, ln->stream);
-        nrc = nc.AllGather(ln->d_totals + CFBPE_MAX_DEVICES, ln->d_totals, 1, kNcclUint64, ctx->devs[d]->comm, ln->stream);
+        ln->h_totals.get()[CFBPE_MAX_DEVICES] = sh[d].tokens;                                   // (slot past the gathered ones: this shard's own total)
+        cudaMemcpyAsync(ln->d_totals.get() + CFBPE_MAX_DEVICES, ln->h_totals.get() + CFBPE_MAX_DEVICES, sizeof(uint64_t), cudaMemcpyHostToDevice, ln->stream.get());
+        nrc = nc.AllGather(ln->d_totals.get() + CFBPE_MAX_DEVICES, ln->d_totals.get(), 1, kNcclUint64, ctx->devs[d]->comm, ln->stream.get());
     }
     { const int r2 = nc.GroupEnd(); if (nrc == 0) nrc = r2; }
     if (nrc != 0) return fail(ctx, CFBPE_EIO, std::string("ncclAllGather of the shard totals: ") + nc.GetErrorString(nrc));
@@ -868,20 +892,20 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             const uint32_t p0 = lo[d];
             auto ck = [&](cudaError_t e, const char* what) { if (e != cudaSuccess && rcs[d] == CFBPE_OK) { rcs[d] = CFBPE_EIO; errs[d] = std::string(what) + ": " + cudaGetErrorString(e); } };
             ck(cudaSetDevice(ctx->devs[d]->device), "cudaSetDevice");
-            cudaStream_t st = ln->stream;
-            ck(cudaMemcpyAsync(ln->h_totals, ln->d_totals, sizeof(uint64_t) * G, cudaMemcpyDeviceToHost, st), "totals download");
+            cudaStream_t st = ln->stream.get();
+            ck(cudaMemcpyAsync(ln->h_totals.get(), ln->d_totals.get(), sizeof(uint64_t) * G, cudaMemcpyDeviceToHost, st), "totals download");
             if (chunk) ck(cudaMemcpyAsync(lane_chunk_totals(ctx, ln), chunk_tot.data(), sizeof(uint64_t) * G, cudaMemcpyHostToDevice, st), "chunk totals upload");
             for (int k = 0; k < s.nc; ++k) {
                 const uint32_t q0 = s.cut[k], nk = s.cut[k + 1] - s.cut[k];
                 const bool last = (k + 1 == s.nc) && (d + 1 == G);
                 const uint64_t cnt = static_cast<uint64_t>(nk) + (last ? 1 : 0);      // the boundary entry belongs to the next sub-batch / shard
                 if (!cnt) continue;
-                uint64_t* src = ln->d_out_offsets + sub_batch_offsets_at(q0, k);
-                rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(src, cnt, ln->d_totals, d);
+                uint64_t* src = ln->d_out_offsets.get() + sub_batch_offsets_at(q0, k);
+                rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(src, cnt, ln->d_totals.get(), d);
                 if (out_offsets) ck(cudaMemcpyAsync(out_offsets + p0 + q0, src, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st), "offsets download");
-                if (out_counts && nk) ck(cudaMemcpyAsync(out_counts + p0 + q0, ln->d_out_counts + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "counts download");
+                if (out_counts && nk) ck(cudaMemcpyAsync(out_counts + p0 + q0, ln->d_out_counts.get() + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "counts download");
                 if (chunk) {      // chunk offsets: rebased as the token offsets, by the chunk totals of the shards before; spans: prompt-relative
-                    uint64_t* csrc = ln->d_chunk_offs + sub_batch_offsets_at(q0, k);
+                    uint64_t* csrc = ln->d_chunk_offs.get() + sub_batch_offsets_at(q0, k);
                     rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(csrc, cnt, lane_chunk_totals(ctx, ln), d);
                     ck(cudaMemcpyAsync(chunk->offsets + p0 + q0, csrc, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st), "chunk offsets download");
                     const uint64_t c0 = k ? s.chunk_end[k - 1] : 0, c1 = s.chunk_end[k];
@@ -897,9 +921,9 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             }
             ck(cudaStreamSynchronize(st), "stream sync");
             uint64_t base = 0;
-            for (uint32_t e = 0; e < d; ++e) base += ln->h_totals[e];
-            if (want_ids && out_ids && fits && s.tokens) ck(cudaMemcpyAsync(out_ids + base, ln->d_out_ids, s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "ids download");
-            if (out_starts && fits && s.tokens) ck(cudaMemcpyAsync(out_starts + base, ln->d_out_starts, s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "starts download");
+            for (uint32_t e = 0; e < d; ++e) base += ln->h_totals.get()[e];
+            if (want_ids && out_ids && fits && s.tokens) ck(cudaMemcpyAsync(out_ids + base, ln->d_out_ids.get(), s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "ids download");
+            if (out_starts && fits && s.tokens) ck(cudaMemcpyAsync(out_starts + base, ln->d_out_starts.get(), s.tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "starts download");
             ck(cudaStreamSynchronize(st), "stream sync");
         });
         for (auto& t : th) t.join();
@@ -937,9 +961,7 @@ int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* o
                 lns[g] = locks[g]->ln;
                 CK(cudaSetDevice(dvs[g]->device));
                 rc = wait_for_device_call(ctx, lns[g]);
-                if (!rc && (out_starts || chunk)) rc = ensure_starts_lane(ctx, lns[g]);
-                if (!rc && trunc) rc = ensure_truncate_lane(ctx, lns[g]);
-                if (!rc && chunk) rc = ensure_chunk_lane(ctx, lns[g]);
+                if (!rc) rc = ensure_call_buffers(ctx, lns[g], out_starts || chunk, trunc != nullptr, chunk != nullptr);
                 if (rc) return rc;
             }
             return run_host_pipelined(ctx, dvs, lns, G, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
@@ -965,29 +987,29 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
     CK(cudaSetDevice(dv->device));
     int rc = wait_for_device_call(ctx, ln);
     if (rc) return rc;
-    cudaStream_t s = ln->stream;
+    cudaStream_t s = ln->stream.get();
     SpecialSet sp;
     bool scan = false, spliced = false;
     BatchView b;
     if ((rc = special_set(ctx, dv, ln, modes, &sp, &scan, s)) || (rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b))) return rc;
-    const EncodeOut plain{want_ids ? ln->d_out_ids : nullptr, ctx->max_bytes, ln->d_out_offsets, ln->d_out_counts};
-    const EncodeOut fin{want_ids ? ln->ws.lscratch.rank : nullptr, ctx->max_bytes, ln->sp.fin_offsets, ln->sp.fin_counts};
+    const EncodeOut plain{want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get(), ln->d_out_counts.get()};
+    const EncodeOut fin{want_ids ? ln->ws.lscratch.rank : nullptr, ctx->max_bytes, ln->sp.fin_offsets.get(), ln->sp.fin_counts.get()};
     if ((rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, plain, fin, out_bad, &spliced))) return rc;
-    if (spliced) CK(cudaMemcpyAsync(ln->sp.h_status, ln->sp.status, sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    if (spliced) CK(cudaMemcpyAsync(ln->sp.h_status.get(), ln->sp.status.get(), sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     const DeviceStatus st = *ln->h_status;
     if ((rc = fail_status(ctx, st))) return rc;
     const uint64_t n_tokens = spliced ? ln->sp.h_status->fin.n_tokens : st.n_tokens;
     // where the call's ids, offsets and counts are on the device
-    const uint32_t* ids_src = spliced ? ln->ws.lscratch.rank : ln->d_out_ids;
-    const uint64_t* offs_src = spliced ? ln->sp.fin_offsets : ln->d_out_offsets;
-    const uint32_t* counts_src = spliced ? ln->sp.fin_counts : ln->d_out_counts;
+    const uint32_t* ids_src = spliced ? ln->ws.lscratch.rank : ln->d_out_ids.get();
+    const uint64_t* offs_src = spliced ? ln->sp.fin_offsets.get() : ln->d_out_offsets.get();
+    const uint32_t* counts_src = spliced ? ln->sp.fin_counts.get() : ln->d_out_counts.get();
     if (defer) {       // a shard of a multi-device call: its results go where run_multi_device downloads them from
         if (spliced) {
-            if (want_ids && n_tokens) CK(cudaMemcpyAsync(ln->d_out_ids, ids_src, n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-            CK(cudaMemcpyAsync(ln->d_out_offsets, offs_src, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
-            if (n) CK(cudaMemcpyAsync(ln->d_out_counts, counts_src, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+            if (want_ids && n_tokens) CK(cudaMemcpyAsync(ln->d_out_ids.get(), ids_src, n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+            CK(cudaMemcpyAsync(ln->d_out_offsets.get(), offs_src, (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+            if (n) CK(cudaMemcpyAsync(ln->d_out_counts.get(), counts_src, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
             CK(cudaStreamSynchronize(s));
         }
         *defer = n_tokens;
@@ -1028,108 +1050,65 @@ int run_host_special(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
 // ---------------------------------------------------------------------------------------
 // construction / destruction
 // ---------------------------------------------------------------------------------------
-void destroy_lane(Lane* ln) {
-    if (!ln) return;
-    cudaSetDevice(ln->device);
-    free_special_lane(ln);
-    cudaFree(ln->d_bytes); cudaFree(ln->d_offsets); cudaFree(ln->d_vocab_ids);
-    cudaFree(ln->d_out_ids); cudaFree(ln->d_out_offsets); cudaFree(ln->d_out_counts); cudaFree(ln->d_out_starts); cudaFree(ln->d_trunc);
-    cudaFree(ln->d_chunk_offs);
-    for_each_ws_buffer(ln->ws, [](auto*& p, WsKind) { cudaFree(p); });
-    cudaFree(ln->ws.status);
-    cudaFree(ln->d_dec_sums); cudaFree(ln->d_dec_base); cudaFree(ln->d_totals);
-    if (ln->h_status) cudaFreeHost(ln->h_status);
-    if (ln->h_status_arr) cudaFreeHost(ln->h_status_arr);
-    if (ln->h_offs_stage) cudaFreeHost(ln->h_offs_stage);
-    if (ln->h_totals) cudaFreeHost(ln->h_totals);
-    cudaFree(ln->d_status_arr);
-    for (int k = 0; k < kMaxPipeChunks; ++k) {
-        if (ln->ev_h2d[k]) cudaEventDestroy(ln->ev_h2d[k]); if (ln->ev_done[k]) cudaEventDestroy(ln->ev_done[k]);
-        if (ln->ev_front[k]) cudaEventDestroy(ln->ev_front[k]); if (ln->ev_chain[k]) cudaEventDestroy(ln->ev_chain[k]);
-        if (ln->ev_scan[k]) cudaEventDestroy(ln->ev_scan[k]); if (ln->ev_list[k]) cudaEventDestroy(ln->ev_list[k]);
-    }
-    for (int k = 1; k < kFrontStreams; ++k) if (ln->front[k]) cudaStreamDestroy(ln->front[k]);
-    for (int l = 0; l < kPrioLevels; ++l) for (int j = 0; j < kPoolSlots; ++j) if (ln->pool[l][j]) cudaStreamDestroy(ln->pool[l][j]);
-    for (int k = 0; k < kSideStreams; ++k) { if (ln->side[k]) cudaStreamDestroy(ln->side[k]); if (ln->side2[k]) cudaStreamDestroy(ln->side2[k]); }
-    if (ln->aux_stream) cudaStreamDestroy(ln->aux_stream);
-    if (ln->aux2_stream) cudaStreamDestroy(ln->aux2_stream);
-    if (ln->ev_fork) cudaEventDestroy(ln->ev_fork);
-    if (ln->ev_join) cudaEventDestroy(ln->ev_join);
-    if (ln->ev_join2) cudaEventDestroy(ln->ev_join2);
-    if (ln->ev_ws) cudaEventDestroy(ln->ev_ws);
-    if (ln->h2d_stream) cudaStreamDestroy(ln->h2d_stream);
-    if (ln->d2h_stream) cudaStreamDestroy(ln->d2h_stream);
-    for (int k = 0; k < CFBPE_NUM_KERNELS; ++k) for (int j = 0; j < 2; ++j) if (ln->prof.ev[k][j]) cudaEventDestroy(ln->prof.ev[k][j]);
-    for (int j = 0; j < 2; ++j) {
-        if (ln->prof.h2d[j]) cudaEventDestroy(ln->prof.h2d[j]);
-        if (ln->prof.d2h[j]) cudaEventDestroy(ln->prof.d2h[j]);
-        if (ln->prof.total[j]) cudaEventDestroy(ln->prof.total[j]);
-    }
-    if (ln->stream) cudaStreamDestroy(ln->stream);
-}
-
 // everything one call touches on the device, sized by max_batch_bytes (~33 bytes per byte of it)
 bool create_lane(Lane* ln, int device, uint64_t mb, uint64_t mp) {
     ln->device = device;
     ln->max_bytes = mb;
     int prio_lo = 0, prio_hi = 0;
     cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    bool ok = cudaStreamCreateWithPriority(&ln->stream, cudaStreamNonBlocking, prio_hi) == cudaSuccess;   // front stream of sub-batch 0
-    ok = ok && dmalloc(&ln->d_bytes, lane_bytes_alloc(mb, kMaxPipeChunks)) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_offsets, lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_vocab_ids, mp + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_out_ids, mb + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_out_offsets, lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_out_counts, mp + 1) == cudaSuccess;
+    bool ok = make_stream(ln->stream, prio_hi) == cudaSuccess;   // front stream of sub-batch 0
+    ok = ok && dmalloc(ln->d_bytes, lane_bytes_alloc(mb, kMaxPipeChunks)) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_offsets, lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_vocab_ids, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_out_ids, mb + 1) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_out_offsets, lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_out_counts, mp + 1) == cudaSuccess;
     const WsSizes ws = workspace_alloc(mb, kMaxPipeChunks);
     for_each_ws_buffer(ln->ws, [&](auto*& p, WsKind kind) { ok = ok && dmalloc(&p, ws.n[kind]) == cudaSuccess; });
     set_workspace_caps(ln->ws, ws);      // a one-shot call may use all of it
-    ok = ok && dmalloc(&ln->d_dec_sums, mb / kDecodeTile + 2) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_dec_base, mb / kDecodeTile + 2) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_totals, CFBPE_MAX_DEVICES + 1) == cudaSuccess;
-    ok = ok && dmalloc(&ln->ws.status, 1) == cudaSuccess;
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_status), sizeof(DeviceStatus)) == cudaSuccess;
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_totals), sizeof(uint64_t) * (CFBPE_MAX_DEVICES + 1)) == cudaSuccess;
-    ok = ok && cudaStreamCreateWithFlags(&ln->h2d_stream, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaStreamCreateWithFlags(&ln->d2h_stream, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && dmalloc(&ln->d_status_arr, kMaxPipeChunks) == cudaSuccess;
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_status_arr), sizeof(DeviceStatus) * kMaxPipeChunks) == cudaSuccess;
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&ln->h_offs_stage), sizeof(uint64_t) * lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_dec_sums, mb / kDecodeTile + 2) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_dec_base, mb / kDecodeTile + 2) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_totals, CFBPE_MAX_DEVICES + 1) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_status, 1) == cudaSuccess;
+    ln->ws.status = ln->d_status.get();
+    ok = ok && hmalloc(ln->h_status, 1) == cudaSuccess;
+    ok = ok && hmalloc(ln->h_totals, CFBPE_MAX_DEVICES + 1) == cudaSuccess;
+    ok = ok && make_stream(ln->h2d_stream, 0) == cudaSuccess;      // (0: the default priority)
+    ok = ok && make_stream(ln->d2h_stream, 0) == cudaSuccess;
+    ok = ok && dmalloc(ln->d_status_arr, kMaxPipeChunks) == cudaSuccess;
+    ok = ok && hmalloc(ln->h_status_arr, kMaxPipeChunks) == cudaSuccess;
+    ok = ok && hmalloc(ln->h_offs_stage, lane_offsets_alloc(mp, kMaxPipeChunks)) == cudaSuccess;
     {   // a pipelined host call gives earlier sub-batches the higher priority, so that they finish first and their downloads
         // run while the later ones compute (with equal priorities the sub-batches finished together and the downloads queued up
         // at the end: tools/pipe_trace.py)
         const int levels = prio_lo - prio_hi + 1;
-        for (int k = 1; ok && k < kFrontStreams; ++k)
-            ok = cudaStreamCreateWithPriority(&ln->front[k], cudaStreamNonBlocking, prio_hi + (k < levels ? k : levels - 1)) == cudaSuccess;
-        for (int k = 0; ok && k < kSideStreams; ++k) ok = cudaStreamCreateWithPriority(&ln->side[k], cudaStreamNonBlocking, prio_hi) == cudaSuccess;
-        for (int k = 0; ok && k < kSideStreams; ++k) ok = cudaStreamCreateWithPriority(&ln->side2[k], cudaStreamNonBlocking, prio_hi) == cudaSuccess;
+        for (int k = 1; ok && k < kFrontStreams; ++k) ok = make_stream(ln->front[k], prio_hi + (k < levels ? k : levels - 1)) == cudaSuccess;
+        for (int k = 0; ok && k < kSideStreams; ++k) ok = make_stream(ln->side[k], prio_hi) == cudaSuccess;
+        for (int k = 0; ok && k < kSideStreams; ++k) ok = make_stream(ln->side2[k], prio_hi) == cudaSuccess;
         if (const char* e = std::getenv("CFBPE_PIPE_PRIO")) {      // experiment: 1 = every kernel at one priority, 2 = priority by the sub-batch's age
             ln->prio_mode = std::atoi(e);
             ln->prio_levels = ln->prio_mode == 2 ? (levels < kPrioLevels ? levels : kPrioLevels) : 1;
             for (int l = 0; ok && ln->prio_mode && l < ln->prio_levels; ++l)
-                for (int j = 0; ok && j < kPoolSlots; ++j) ok = cudaStreamCreateWithPriority(&ln->pool[l][j], cudaStreamNonBlocking, prio_hi + l) == cudaSuccess;
+                for (int j = 0; ok && j < kPoolSlots; ++j) ok = make_stream(ln->pool[l][j], prio_hi + l) == cudaSuccess;
         }
     }
     // the long-piece kernels are latency-bound and small: their CTAs go first, the short-piece kernels fill the rest
     // (A/B of lower priorities and of CTA caps: no gain)
-    ok = ok && cudaStreamCreateWithPriority(&ln->aux_stream, cudaStreamNonBlocking, prio_hi) == cudaSuccess;
-    ok = ok && cudaStreamCreateWithPriority(&ln->aux2_stream, cudaStreamNonBlocking, prio_hi) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&ln->ev_fork, cudaEventDisableTiming) == cudaSuccess && cudaEventCreateWithFlags(&ln->ev_join, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&ln->ev_ws, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&ln->ev_join2, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && make_stream(ln->aux_stream, prio_hi) == cudaSuccess;
+    ok = ok && make_stream(ln->aux2_stream, prio_hi) == cudaSuccess;
+    ok = ok && make_event(ln->ev_fork, cudaEventDisableTiming) == cudaSuccess && make_event(ln->ev_join, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && make_event(ln->ev_ws, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && make_event(ln->ev_join2, cudaEventDisableTiming) == cudaSuccess;
     for (int k = 0; ok && k < kMaxPipeChunks; ++k)
-        ok = cudaEventCreateWithFlags(&ln->ev_h2d[k], cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ln->ev_front[k], cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ln->ev_done[k], cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ln->ev_chain[k], cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ln->ev_scan[k], cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ln->ev_list[k], cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaMemset(ln->d_bytes, 0, lane_bytes_alloc(mb, kMaxPipeChunks)) == cudaSuccess;
+        ok = make_event(ln->ev_h2d[k], cudaEventDisableTiming) == cudaSuccess && make_event(ln->ev_front[k], cudaEventDisableTiming) == cudaSuccess &&
+             make_event(ln->ev_done[k], cudaEventDisableTiming) == cudaSuccess && make_event(ln->ev_chain[k], cudaEventDisableTiming) == cudaSuccess &&
+             make_event(ln->ev_scan[k], cudaEventDisableTiming) == cudaSuccess && make_event(ln->ev_list[k], cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && cudaMemset(ln->d_bytes.get(), 0, lane_bytes_alloc(mb, kMaxPipeChunks)) == cudaSuccess;
     for (int k = 0; ok && k < CFBPE_NUM_KERNELS; ++k)
-        ok = cudaEventCreate(&ln->prof.ev[k][0]) == cudaSuccess && cudaEventCreate(&ln->prof.ev[k][1]) == cudaSuccess;
+        ok = make_event(ln->prof.ev[k][0], cudaEventDefault) == cudaSuccess && make_event(ln->prof.ev[k][1], cudaEventDefault) == cudaSuccess;
     for (int k = 0; ok && k < 2; ++k)
-        ok = cudaEventCreate(&ln->prof.h2d[k]) == cudaSuccess && cudaEventCreate(&ln->prof.d2h[k]) == cudaSuccess &&
-             cudaEventCreate(&ln->prof.total[k]) == cudaSuccess;
+        ok = make_event(ln->prof.h2d[k], cudaEventDefault) == cudaSuccess && make_event(ln->prof.d2h[k], cudaEventDefault) == cudaSuccess &&
+             make_event(ln->prof.total[k], cudaEventDefault) == cudaSuccess;
     return ok;
 }
 
@@ -1141,33 +1120,33 @@ bool create_device(DeviceCtx* dv, int device, int index, uint32_t n_lanes, uint6
     dv->sm_count = prop.multiProcessorCount;
     bool ok = cudaFuncSetAttribute(bpe_list_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kListSmemBytes)) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(pretok_split16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kNumPatterns * kProdTableBytes)) == cudaSuccess;
-    ok = ok && dmalloc(&dv->d_uc1, sizeof cfbpe_uc_stage1) == cudaSuccess;
-    ok = ok && dmalloc(&dv->d_uc2, sizeof cfbpe_uc_stage2) == cudaSuccess;
-    ok = ok && cudaMemcpy(dv->d_uc1, cfbpe_uc_stage1, sizeof cfbpe_uc_stage1, cudaMemcpyHostToDevice) == cudaSuccess;
-    ok = ok && cudaMemcpy(dv->d_uc2, cfbpe_uc_stage2, sizeof cfbpe_uc_stage2, cudaMemcpyHostToDevice) == cudaSuccess;
+    ok = ok && dmalloc(dv->d_uc1, sizeof cfbpe_uc_stage1) == cudaSuccess;
+    ok = ok && dmalloc(dv->d_uc2, sizeof cfbpe_uc_stage2) == cudaSuccess;
+    ok = ok && cudaMemcpy(dv->d_uc1.get(), cfbpe_uc_stage1, sizeof cfbpe_uc_stage1, cudaMemcpyHostToDevice) == cudaSuccess;
+    ok = ok && cudaMemcpy(dv->d_uc2.get(), cfbpe_uc_stage2, sizeof cfbpe_uc_stage2, cudaMemcpyHostToDevice) == cudaSuccess;
     {
         std::vector<uint16_t> fsm(kNumPatterns * kPretokTableSize);
         uint8_t ascii[128];
         build_pretok_tables(fsm.data());
         build_ascii_classes(ascii);
-        ok = ok && dmalloc(&dv->d_ascii, 128) == cudaSuccess;
-        ok = ok && dmalloc(&dv->d_fsm, fsm.size()) == cudaSuccess;
-        ok = ok && cudaMemcpy(dv->d_ascii, ascii, 128, cudaMemcpyHostToDevice) == cudaSuccess;
-        ok = ok && cudaMemcpy(dv->d_fsm, fsm.data(), fsm.size() * sizeof(uint16_t), cudaMemcpyHostToDevice) == cudaSuccess;
+        ok = ok && dmalloc(dv->d_ascii, 128) == cudaSuccess;
+        ok = ok && dmalloc(dv->d_fsm, fsm.size()) == cudaSuccess;
+        ok = ok && cudaMemcpy(dv->d_ascii.get(), ascii, 128, cudaMemcpyHostToDevice) == cudaSuccess;
+        ok = ok && cudaMemcpy(dv->d_fsm.get(), fsm.data(), fsm.size() * sizeof(uint16_t), cudaMemcpyHostToDevice) == cudaSuccess;
         std::vector<SplitTablesHost> st(1);
         build_split_tables(st.data());
-        ok = ok && dmalloc(&dv->d_split_tables, sizeof(SplitTablesHost)) == cudaSuccess;
-        ok = ok && cudaMemcpy(dv->d_split_tables, st.data(), sizeof(SplitTablesHost), cudaMemcpyHostToDevice) == cudaSuccess;
+        ok = ok && dmalloc(dv->d_split_tables, sizeof(SplitTablesHost)) == cudaSuccess;
+        ok = ok && cudaMemcpy(dv->d_split_tables.get(), st.data(), sizeof(SplitTablesHost), cudaMemcpyHostToDevice) == cudaSuccess;
     }
     if (!ok) return false;
-    dv->uc = UcTables{dv->d_uc1, dv->d_uc2, dv->d_ascii, dv->d_fsm,
-                      dv->d_split_tables + offsetof(SplitTablesHost, cls256),
-                      reinterpret_cast<const uint16_t*>(dv->d_split_tables + offsetof(SplitTablesHost, fsm16)),
-                      reinterpret_cast<const uint16_t*>(dv->d_split_tables + offsetof(SplitTablesHost, ctx16)),
-                      reinterpret_cast<const uint64_t*>(dv->d_split_tables + offsetof(SplitTablesHost, prod)),
-                      reinterpret_cast<const ProdInfo*>(dv->d_split_tables + offsetof(SplitTablesHost, prod_info)),
-                      dv->d_split_tables + offsetof(SplitTablesHost, prod_skip),
-                      dv->d_split_tables + offsetof(SplitTablesHost, prod_start)};
+    dv->uc = UcTables{dv->d_uc1.get(), dv->d_uc2.get(), dv->d_ascii.get(), dv->d_fsm.get(),
+                      dv->d_split_tables.get() + offsetof(SplitTablesHost, cls256),
+                      reinterpret_cast<const uint16_t*>(dv->d_split_tables.get() + offsetof(SplitTablesHost, fsm16)),
+                      reinterpret_cast<const uint16_t*>(dv->d_split_tables.get() + offsetof(SplitTablesHost, ctx16)),
+                      reinterpret_cast<const uint64_t*>(dv->d_split_tables.get() + offsetof(SplitTablesHost, prod)),
+                      reinterpret_cast<const ProdInfo*>(dv->d_split_tables.get() + offsetof(SplitTablesHost, prod_info)),
+                      dv->d_split_tables.get() + offsetof(SplitTablesHost, prod_skip),
+                      dv->d_split_tables.get() + offsetof(SplitTablesHost, prod_start)};
     for (uint32_t i = 0; i < n_lanes; ++i) {
         dv->lanes.emplace_back(new Lane());
         if (!create_lane(dv->lanes.back().get(), device, mb, mp)) return false;
@@ -1219,19 +1198,19 @@ int device_call(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     // a lane is one workspace: a call on another stream waits (on the device) for the lane's previous device-path call;
     // consecutive calls take different lanes when the context has several (n_workspaces) and then overlap
-    if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws, 0));
+    if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws.get(), 0));
     ProfEvents* prof = profiled && ctx->profiling.load() ? &ln->prof : nullptr;
-    if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0], s); cudaEventRecord(prof->h2d[0], s); cudaEventRecord(prof->h2d[1], s); }
+    if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0].get(), s); cudaEventRecord(prof->h2d[0].get(), s); cudaEventRecord(prof->h2d[1].get(), s); }
     const int rc = enqueue(dv, ln, BatchView{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes}, s, prof);
     if (rc) return rc;
-    CK(cudaEventRecord(ln->ev_ws, s));
+    CK(cudaEventRecord(ln->ev_ws.get(), s));
     ln->ws_pending = true;
     ln->dev_out_cap = out_cap;
     ln->dev_want_ids = want_ids;
     tl_device_lane = ln;
-    if (prof) { cudaEventRecord(prof->d2h[0], s); cudaEventRecord(prof->d2h[1], s); cudaEventRecord(prof->total[1], s); }
+    if (prof) { cudaEventRecord(prof->d2h[0].get(), s); cudaEventRecord(prof->d2h[1].get(), s); cudaEventRecord(prof->total[1].get(), s); }
     if (!n_tokens && !prof) return CFBPE_OK;
-    CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     if (prof) fill_profile(ln, total_bytes);
     if (n_tokens) *n_tokens = ln->h_status->n_tokens;
@@ -1245,8 +1224,8 @@ int run_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint6
     return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_offsets, d_out_ids != nullptr, out_cap, n_tokens, stream, true,
                        [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents* prof) {
         enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts,
-                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                       ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, d_out_starts);   // profiling: one stream, so that the per-kernel times do not overlap
+                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
+                       ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, d_out_starts);   // profiling: one stream, so that the per-kernel times do not overlap
         CK(cudaGetLastError());
         return CFBPE_OK;
     });
@@ -1276,9 +1255,9 @@ int run_device_truncate(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_byt
     return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_cut, false, 0, nullptr, stream, true,
                        [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents* prof) {
         const TruncateView tv{d_budgets, mode == CFBPE_TRUNCATE_TAIL ? 1u : 0u, d_out_cut, d_out_kept};
-        enqueue_encode(b, dv->vs, dv->uc, ln->ws, ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets, d_out_counts,
-                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                       ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, nullptr, &tv);
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, ln->d_out_ids.get(), ctx->max_bytes, ln->d_out_offsets.get(), d_out_counts,
+                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
+                       ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, nullptr, &tv);
         CK(cudaGetLastError());
         return CFBPE_OK;
     });
@@ -1291,11 +1270,11 @@ int run_device_chunk(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes,
                      uint64_t* d_out_chunk_offsets, uint32_t* d_out_counts, uint64_t* n_chunks, void* stream) {
     return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_chunk_offsets, true, chunk_cap, n_chunks, stream, true,
                        [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents* prof) {
-        if (const int rc = ensure_starts_lane(ctx, ln)) return rc;
+        if (const int rc = ensure_call_buffers(ctx, ln, true, false, false)) return rc;     // the starts
         const ChunkView cv{chunk_tokens, chunk_tokens - overlap_tokens, d_out_chunk_offsets, nullptr, d_out_spans, d_out_spans + 1, 2u, chunk_cap};
-        enqueue_encode(b, dv->vs, dv->uc, ln->ws, ln->d_out_ids, ctx->max_bytes, ln->d_out_offsets, d_out_counts,
-                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream, prof ? s : ln->aux2_stream,
-                       ln->ev_fork, ln->ev_join, ln->ev_join2, prof, nullptr, ln->d_out_starts, nullptr, &cv);
+        enqueue_encode(b, dv->vs, dv->uc, ln->ws, ln->d_out_ids.get(), ctx->max_bytes, ln->d_out_offsets.get(), d_out_counts,
+                       static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
+                       ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, ln->d_out_starts.get(), nullptr, &cv);
         CK(cudaGetLastError());
         static_assert(offsetof(DeviceStatus, chunk_end) == offsetof(DeviceStatus, n_chunks) + sizeof(uint64_t) &&
                       offsetof(DeviceStatus, tok_end) == offsetof(DeviceStatus, n_tokens) + sizeof(uint64_t), "count, then end");
@@ -1387,16 +1366,11 @@ int cfbpe_create(const cfbpe_config* cfg, cfbpe_ctx** out) {
 void cfbpe_destroy(cfbpe_ctx* ctx) {
     DeviceGuard restore_device;
     if (!ctx) return;
-    for (auto& dvp : ctx->devs) {
-        DeviceCtx* dv = dvp.get();
+    for (auto& dv : ctx->devs) {
         cudaSetDevice(dv->device);
         cudaDeviceSynchronize();             // device-path calls may still be running on the caller's streams
         if (dv->comm && ctx->nccl.CommDestroy) ctx->nccl.CommDestroy(dv->comm);
-        for (auto& ln : dv->lanes) destroy_lane(ln.get());
-        cudaSetDevice(dv->device);
-        cudaFree(dv->d_uc1); cudaFree(dv->d_uc2); cudaFree(dv->d_ascii); cudaFree(dv->d_fsm); cudaFree(dv->d_split_tables);
-        for (auto& v : dv->vocabs) { if (v.d_blob) cudaFree(v.d_blob); }
-        for (auto* t : dv->d_specials) cudaFree(t);
+        dv.reset();                          // its lanes, then its tables
     }
     delete ctx;
 }
@@ -1528,31 +1502,31 @@ int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, con
     CK(cudaSetDevice(dv->device));
     const int rc = wait_for_device_call(ctx, ln);
     if (rc) return rc;
-    cudaStream_t s = ln->stream;
-    if (n_ids) CK(cudaMemcpyAsync(ln->d_out_ids, ids, n_ids * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ln->d_offsets, id_offsets, (static_cast<uint64_t>(n_seqs) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-    if (vocab_ids && n_seqs) CK(cudaMemcpyAsync(ln->d_vocab_ids, vocab_ids, n_seqs, cudaMemcpyHostToDevice, s));
+    cudaStream_t s = ln->stream.get();
+    if (n_ids) CK(cudaMemcpyAsync(ln->d_out_ids.get(), ids, n_ids * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ln->d_offsets.get(), id_offsets, (static_cast<uint64_t>(n_seqs) + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    if (vocab_ids && n_seqs) CK(cudaMemcpyAsync(ln->d_vocab_ids.get(), vocab_ids, n_seqs, cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(ln->ws.status, 0, sizeof(DeviceStatus), s));
-    DecodeView d{ln->d_out_ids, ln->d_offsets, vocab_ids ? ln->d_vocab_ids : nullptr, n_seqs, n_ids};
+    DecodeView d{ln->d_out_ids.get(), ln->d_offsets.get(), vocab_ids ? ln->d_vocab_ids.get() : nullptr, n_seqs, n_ids};
     const uint32_t n_tiles = static_cast<uint32_t>((n_ids + kDecodeTile - 1) / kDecodeTile);
-    if (n_tiles) decode_len_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_sums, ln->ws.status, dv->specials);
-    tile_scan_kernel<<<1, n_tiles ? 1024 : 32, 0, s>>>(ln->d_dec_sums, n_tiles, ln->d_dec_base, ln->ws.status, nullptr);
-    if (n_tiles) decode_copy_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_base, ln->d_bytes, ctx->max_bytes, dv->specials);
-    decode_offsets_kernel<<<static_cast<unsigned>((static_cast<uint64_t>(n_seqs) + 1 + 255) / 256), 256, 0, s>>>(d, ln->ws.ids_by_pos, ln->d_dec_base, ln->d_out_offsets, ln->ws.status);
+    if (n_tiles) decode_len_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_sums.get(), ln->ws.status, dv->specials);
+    tile_scan_kernel<<<1, n_tiles ? 1024 : 32, 0, s>>>(ln->d_dec_sums.get(), n_tiles, ln->d_dec_base.get(), ln->ws.status, nullptr);
+    if (n_tiles) decode_copy_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_base.get(), ln->d_bytes.get(), ctx->max_bytes, dv->specials);
+    decode_offsets_kernel<<<static_cast<unsigned>((static_cast<uint64_t>(n_seqs) + 1 + 255) / 256), 256, 0, s>>>(d, ln->ws.ids_by_pos, ln->d_dec_base.get(), ln->d_out_offsets.get(), ln->ws.status);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     const DeviceStatus st = *ln->h_status;
     if (st.bad_utf8) return fail(ctx, CFBPE_EINVAL, "a token id is outside its vocabulary");
     const uint64_t total = st.tok_end;
     if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "the decoded batch exceeds max_batch_bytes of this context");
-    CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets, (static_cast<uint64_t>(n_seqs) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets.get(), (static_cast<uint64_t>(n_seqs) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     if (total > out_cap || (total && !out_bytes)) {
         CK(cudaStreamSynchronize(s));
         out_offsets[n_seqs] = total;
         return fail(ctx, CFBPE_ENOSPC, "out_cap too small: need " + std::to_string(total) + " bytes");
     }
-    if (total) CK(cudaMemcpyAsync(out_bytes, ln->d_bytes, total, cudaMemcpyDeviceToHost, s));
+    if (total) CK(cudaMemcpyAsync(out_bytes, ln->d_bytes.get(), total, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     return CFBPE_OK;
 }
@@ -1613,14 +1587,13 @@ int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, cons
     std::unique_lock<std::shared_mutex> lock(ctx->vocab_mu);
     if (!ctx->vocabs[vocab_id].loaded) return fail(ctx, CFBPE_ENOENT, "vocab " + std::to_string(vocab_id) + " is not loaded");
     const size_t G = ctx->devs.size();
-    std::vector<uint32_t*> nt(G, nullptr);
+    std::vector<DevPtr<uint32_t>> nt(G);      // the new tables, one a device: released on return unless installed
     if (!words.empty()) {
         for (size_t d = 0; d < G; ++d) {      // a plain copy to every device: the table is a few KB
             cudaSetDevice(ctx->devs[d]->device);
-            cudaError_t ce = dmalloc(&nt[d], words.size());
-            if (ce == cudaSuccess) ce = cudaMemcpy(nt[d], words.data(), words.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
+            cudaError_t ce = dmalloc(nt[d], words.size());
+            if (ce == cudaSuccess) ce = cudaMemcpy(nt[d].get(), words.data(), words.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
             if (ce != cudaSuccess) {
-                for (size_t k = 0; k <= d; ++k) { cudaSetDevice(ctx->devs[k]->device); cudaFree(nt[k]); }
                 cudaGetLastError();
                 return fail(ctx, CFBPE_ENOMEM, std::string("special-token table upload: ") + cudaGetErrorString(ce));
             }
@@ -1630,8 +1603,8 @@ int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, cons
     ctx->specials[vocab_id] = std::move(words);
     for (size_t d = 0; d < G; ++d) {
         DeviceCtx* dv = ctx->devs[d].get();
-        dv->d_specials[vocab_id] = nt[d];
-        dv->specials.v[vocab_id] = make_special_view(nt[d], ctx->specials[vocab_id]);
+        dv->d_specials[vocab_id] = std::move(nt[d]);
+        dv->specials.v[vocab_id] = make_special_view(dv->d_specials[vocab_id].get(), ctx->specials[vocab_id]);
     }
     return CFBPE_OK;
 }
@@ -1662,7 +1635,7 @@ int cfbpe_device_status(cfbpe_ctx* ctx, void* stream) {
     std::lock_guard<std::mutex> lock(ln->mu);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     CK(cudaSetDevice(ln->device));
-    CK(cudaMemcpyAsync(ln->h_status, ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     return device_call_status(ctx, ln);
 }
@@ -1678,7 +1651,7 @@ void* cfbpe_host_alloc(cfbpe_ctx* ctx, size_t size) {
 void cfbpe_host_free(cfbpe_ctx* ctx, void* ptr) {
     DeviceGuard restore_device;
     if (!ctx || !ptr) return;
-    cudaFreeHost(ptr);
+    HostFree{}(ptr);
 }
 
 int cfbpe_profile_enable(cfbpe_ctx* ctx, int on) {
