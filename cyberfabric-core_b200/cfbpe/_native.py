@@ -13,6 +13,7 @@ OK, ENOENT, EIO, ENOMEM, ENODEV, EINVAL, ENOSPC, EILSEQ, EBADMSG = 0, -2, -5, -1
 SPECIAL_ORDINARY, SPECIAL_ALLOW, SPECIAL_DISALLOW = 0, 1, 2      # what an occurrence of a special token means in one call
 MAX_SPECIALS, MAX_SPECIAL_LEN = 4096, 64
 TRUNCATE_HEAD, TRUNCATE_TAIL = 0, 1      # keep the first / the last tokens of every prompt (cfbpe_truncate_batch)
+UNIT_CODEPOINT, UNIT_UTF16 = 0, 1        # what a unit start counts (cfbpe_encode_batch_char_starts)
 FORMAT_TIKTOKEN, FORMAT_TEKKEN_JSON = 0, 1
 PATTERN_CL100K, PATTERN_O200K, PATTERN_LLAMA3, PATTERN_TEKKEN = 0, 1, 2, 3
 PATTERN_IDS = {"cl100k": 0, "o200k": 1, "llama3": 2, "tekken": 3}
@@ -28,6 +29,7 @@ EXPORTS = [
     "cfbpe_profile_enable", "cfbpe_profile_read", "cfbpe_decode_batch",
     "cfbpe_vocab_set_specials", "cfbpe_encode_batch_special", "cfbpe_encode_batch_special_device",
     "cfbpe_encode_batch_starts", "cfbpe_encode_batch_starts_device",
+    "cfbpe_encode_batch_char_starts", "cfbpe_encode_batch_char_starts_device",
     "cfbpe_truncate_batch", "cfbpe_truncate_batch_device",
     "cfbpe_chunk_batch", "cfbpe_chunk_batch_device",
 ]
@@ -109,6 +111,11 @@ def load():
     L.cfbpe_encode_batch_starts_device.restype = C.c_int
     L.cfbpe_encode_batch_starts_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, C.c_uint64, vp, vp,
                                                    C.POINTER(C.c_uint64), vp]
+    L.cfbpe_encode_batch_char_starts.restype = C.c_int
+    L.cfbpe_encode_batch_char_starts.argtypes = [vp, C.c_uint32, u8p, vp, u8p, C.c_uint32, vp, vp, C.c_uint64, vp, vp, vp]
+    L.cfbpe_encode_batch_char_starts_device.restype = C.c_int
+    L.cfbpe_encode_batch_char_starts_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, C.c_uint32, vp, vp, C.c_uint64, vp, vp,
+                                                        vp, C.POINTER(C.c_uint64), vp]
     L.cfbpe_truncate_batch.restype = C.c_int
     L.cfbpe_truncate_batch.argtypes = [vp, C.c_uint32, u8p, vp, u8p, vp, C.c_uint32, vp, vp, vp]
     L.cfbpe_truncate_batch_device.restype = C.c_int
@@ -288,6 +295,35 @@ class Context:
         nt = int(out_offsets[n])
         return out_ids[:nt], out_starts[:nt], out_offsets, out_counts[:n]
 
+    def encode_batch_char_starts(self, data: np.ndarray, offsets: np.ndarray, unit=UNIT_CODEPOINT, vocab_ids=None, out_ids=None,
+                                 out_starts=None, out_offsets=None, out_counts=None, out_lens=None):
+        """encode_batch plus each token's start within its prompt in `unit` (UNIT_CODEPOINT: str indices, UNIT_UTF16: UTF-16 code
+        units): (ids, starts uint32, offsets, counts, lens uint32 -- every prompt's length in the unit).  A token's start is that of
+        the character holding its first byte, so byte tokens of one character share it: their spans are empty."""
+        n = self._check_inputs(data, offsets, vocab_ids)
+        total = int(offsets[n])
+        if out_ids is None:
+            out_ids = np.empty(max(total, 1), dtype=np.uint32)
+        if out_starts is None:
+            out_starts = np.empty(out_ids.size, dtype=np.uint32)
+        if out_starts.dtype != np.uint32 or out_starts.size < out_ids.size or not out_starts.flags.c_contiguous:
+            raise NativeError(EINVAL, "out_starts must be a C-contiguous uint32 array with room for as many entries as out_ids")
+        if out_offsets is None:
+            out_offsets = np.empty(n + 1, dtype=np.uint64)
+        if out_counts is None:
+            out_counts = np.empty(max(n, 1), dtype=np.uint32)
+        if out_lens is None:
+            out_lens = np.empty(max(n, 1), dtype=np.uint32)
+        elif not isinstance(out_lens, np.ndarray) or out_lens.dtype != np.uint32 or out_lens.size < n or not out_lens.flags.c_contiguous:
+            raise NativeError(EINVAL, "out_lens must be a C-contiguous uint32 array with one entry per prompt")
+        vid = None if vocab_ids is None else vocab_ids.ctypes.data
+        rc = load().cfbpe_encode_batch_char_starts(self._h, n, data.ctypes.data if data.size else None, offsets.ctypes.data, vid, int(unit),
+                                                   out_ids.ctypes.data, out_starts.ctypes.data, out_ids.size, out_offsets.ctypes.data,
+                                                   out_counts.ctypes.data, out_lens.ctypes.data)
+        self._check(rc)
+        nt = int(out_offsets[n])
+        return out_ids[:nt], out_starts[:nt], out_offsets, out_counts[:n], out_lens[:n]
+
     @staticmethod
     def budget_array(budgets, n):
         """an int (every prompt) or one budget per prompt -> a C-contiguous uint32 array of max(n, 1) entries"""
@@ -397,6 +433,17 @@ class Context:
         rc = load().cfbpe_encode_batch_starts_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids,
                                                      d_out_starts, out_cap, d_out_offsets, d_out_counts,
                                                      C.byref(nt) if sync else None, stream)
+        self._check(rc)
+        return nt.value if sync else None
+
+    def encode_batch_char_starts_device(self, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, unit, d_out_ids, d_out_starts, out_cap,
+                                        d_out_offsets, d_out_counts, d_out_lens, stream=0, sync=True):
+        """cfbpe_encode_batch_char_starts_device on raw device pointers (d_out_starts: room for out_cap uint32; d_out_lens: n_prompts
+        uint32 or None); the id count when sync, else fully asynchronous"""
+        nt = C.c_uint64(0)
+        rc = load().cfbpe_encode_batch_char_starts_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, int(unit), d_out_ids,
+                                                          d_out_starts, out_cap, d_out_offsets, d_out_counts, d_out_lens,
+                                                          C.byref(nt) if sync else None, stream)
         self._check(rc)
         return nt.value if sync else None
 

@@ -99,6 +99,7 @@ class EncodeBatchRequest:
     vocab_index: Optional[np.ndarray] = None   # uint8, n: with it, vocabs_per_prompt lists the DISTINCT vocabularies and
                                                # vocab_index[i] picks prompt i's (large batches: no per-prompt objects)
     with_starts: bool = False    # also return every token's byte offset within its prompt (EncodeBatchResponse.starts)
+    starts_unit: str = "byte"    # with with_starts: "byte", or "codepoint" / "utf16" -- the starts in that unit and EncodeBatchResponse.lens
 
 
 @dataclass
@@ -106,7 +107,8 @@ class EncodeBatchResponse:
     ids: np.ndarray              # uint32 dense id stream
     offsets: np.ndarray          # uint64, n+1
     counts: np.ndarray           # uint32, n
-    starts: Optional[np.ndarray] = None   # uint32, one per id: byte offset of the token within its prompt (with_starts)
+    starts: Optional[np.ndarray] = None   # uint32, one per id: offset of the token within its prompt in starts_unit (with_starts)
+    lens: Optional[np.ndarray] = None     # uint32, one per prompt: its length in starts_unit (a "codepoint" / "utf16" request)
 
 
 @dataclass
@@ -203,6 +205,38 @@ def chunk_spans(data: np.ndarray, offsets: np.ndarray, id_offsets: np.ndarray, s
             spans.append((floor(a), floor(min(a + chunk_tokens, c))))
         coffs[i + 1] = coffs[i] + k
     return (np.array(spans, dtype=np.uint32).reshape(-1, 2), coffs)
+
+
+STARTS_UNITS = {"byte": None, "codepoint": N.UNIT_CODEPOINT, "utf16": N.UNIT_UTF16}   # EncodeBatchRequest.starts_unit -> CFBPE_UNIT_*
+
+
+def _starts_unit(unit: str) -> str:
+    if unit not in STARTS_UNITS:
+        raise InvalidInput("the offset unit must be 'byte', 'codepoint' or 'utf16', not %r" % (unit,))
+    return unit
+
+
+def unit_starts(data: np.ndarray, offsets: np.ndarray, id_offsets: np.ndarray, starts: np.ndarray, unit: str) -> Tuple[np.ndarray, np.ndarray]:
+    """The unit-start contract (include/cfbpe.h, cfbpe_encode_batch_char_starts) from every token's byte start: (starts uint32, one
+    per id; lens uint32, one per prompt) in `unit` ("byte", "codepoint" or "utf16").  A token's start is the number of units before
+    the character that holds its first byte; a prompt's length is its units.  The prompts must be valid UTF-8."""
+    n = len(offsets) - 1
+    offs = np.asarray(offsets, dtype=np.int64)
+    st = np.asarray(starts, dtype=np.int64)[:int(id_offsets[n])]
+    if unit == "byte":
+        return st.astype(np.uint32), np.diff(offs).astype(np.uint32)
+    b = np.asarray(data[:int(offs[n])], dtype=np.uint8)
+    lead = (b & 0xC0) != 0x80
+    w = lead.astype(np.uint32)
+    if unit == "utf16":
+        w += (b >= 0xF0).astype(np.uint32)                     # a code point above the BMP is a surrogate pair
+    cum = np.zeros(len(b) + 1, dtype=np.int64)
+    np.cumsum(w, out=cum[1:])                                  # cum[x] = units of the characters that start before byte x
+    char_start = np.maximum.accumulate(np.where(lead, np.arange(len(b), dtype=np.int64), 0)) if len(b) else np.zeros(0, np.int64)
+    prompt = np.repeat(np.arange(n, dtype=np.int64), np.diff(np.asarray(id_offsets, dtype=np.int64)))
+    pos = offs[prompt] + st                                    # each token's first byte in the batch
+    out = cum[char_start[pos]] - cum[offs[prompt]] if len(pos) else np.zeros(0, np.int64)
+    return out.astype(np.uint32), (cum[offs[1:]] - cum[offs[:-1]]).astype(np.uint32)
 
 
 @dataclass
@@ -349,6 +383,18 @@ class TokenizerPluginClient:
             raise ServiceUnavailable("the tokenizer plugin does not return token starts")
         cut, kept = truncate_cuts(req.bytes, req.offsets, r.offsets, r.starts, bud, tail)
         return TruncateBatchResponse(cut, kept, np.asarray(r.counts[:n], dtype=np.uint32))
+
+    def encode_batch_unit_starts(self, ctx: SecurityContext, req: EncodeBatchRequest) -> EncodeBatchResponse:
+        """encode_batch with every token's start in req.starts_unit and every prompt's length in it (EncodeBatchResponse.lens) --
+        include/cfbpe.h, cfbpe_encode_batch_char_starts.  This default works on any plugin that returns byte starts: encode_batch
+        with byte starts, then unit_starts on the host."""
+        unit = _starts_unit(req.starts_unit)
+        r = self.encode_batch(ctx, EncodeBatchRequest(req.vocab, req.bytes, req.offsets, req.vocabs_per_prompt, req.vocab_index,
+                                                      with_starts=True))
+        if r.starts is None:
+            raise ServiceUnavailable("the tokenizer plugin does not return token starts")
+        starts, lens = unit_starts(req.bytes, req.offsets, r.offsets, r.starts, unit)
+        return EncodeBatchResponse(r.ids, r.offsets, r.counts, starts, lens)
 
     def chunk_batch(self, ctx: SecurityContext, req: EncodeBatchRequest, chunk_tokens: int, overlap_tokens: int = 0) -> ChunkBatchResponse:
         """Cut every prompt of `req` into chunks of at most chunk_tokens tokens that overlap by overlap_tokens, at character
@@ -518,7 +564,14 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
     def encode_batch(self, ctx: SecurityContext, req: EncodeBatchRequest, out: Optional[EncodeBatchResponse] = None) -> EncodeBatchResponse:
         self._check_arrays(req)
         vid = self._vocab_ids(req)
+        unit = STARTS_UNITS[_starts_unit(req.starts_unit)]
         try:
+            if req.with_starts and unit is not None:
+                ids, starts, offs, counts, lens = self.ctx.encode_batch_char_starts(
+                    req.bytes, req.offsets, unit, vid,
+                    None if out is None else out.ids, None if out is None else out.starts,
+                    None if out is None else out.offsets, None if out is None else out.counts, None if out is None else out.lens)
+                return EncodeBatchResponse(ids, offs, counts, starts, lens)
             if req.with_starts:
                 ids, starts, offs, counts = self.ctx.encode_batch_starts(
                     req.bytes, req.offsets, vid,
@@ -532,6 +585,13 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
         except N.NativeError as e:
             raise _map_native(e) from e
         return EncodeBatchResponse(ids, offs, counts)
+
+    def encode_batch_unit_starts(self, ctx: SecurityContext, req: EncodeBatchRequest) -> EncodeBatchResponse:
+        """the device path (cfbpe_encode_batch_char_starts): the unit starts are computed where the ids and byte starts are"""
+        if req.starts_unit == "byte":
+            return super().encode_batch_unit_starts(ctx, req)
+        return self.encode_batch(ctx, EncodeBatchRequest(req.vocab, req.bytes, req.offsets, req.vocabs_per_prompt, req.vocab_index,
+                                                         with_starts=True, starts_unit=req.starts_unit))
 
     def count_tokens(self, ctx: SecurityContext, req: CountTokensRequest, out_counts: Optional[np.ndarray] = None) -> np.ndarray:
         self._check_arrays(req)
@@ -642,14 +702,23 @@ class LlmGatewayTokenizerService:
         r = self._plugin().encode_batch(ctx, EncodeBatchRequest(VocabRef(model), data, offs))
         return [r.ids[int(r.offsets[i]):int(r.offsets[i + 1])] for i in range(len(texts))]
 
-    def encode_with_offsets(self, ctx: SecurityContext, model: str, texts: Sequence[str]) -> List[Tuple[np.ndarray, np.ndarray]]:
-        """per text: (ids, spans), spans an (n, 2) uint64 array of each token's [start, end) byte range in text.encode("utf-8")
-        (tiktoken's decode_with_offsets gives the starts in characters; Hugging Face tokenizers' `offsets` are such spans).
-        Cutting a text to a context window or into chunks of at most N tokens is a cut at a span boundary."""
+    def encode_with_offsets(self, ctx: SecurityContext, model: str, texts: Sequence[str], unit: str = "byte") -> List[Tuple[np.ndarray, np.ndarray]]:
+        """per text: (ids, spans), spans an (n, 2) uint64 array of each token's [start, end) range in `unit`:
+          "byte"       indices into text.encode("utf-8");
+          "codepoint"  indices into the str (tiktoken's decode_with_offsets gives these starts; Hugging Face tokenizers' `offsets`
+                       are such spans);
+          "utf16"      indices into the UTF-16 code units of the text, as JavaScript, Java and C# index their strings.
+        In a character unit, a token's start is that of the character that holds its first byte: byte tokens of one character
+        share a start, so some spans are empty, and the spans still slice the text back into exactly itself.  Cutting a text to a
+        context window or into chunks of at most N tokens is a cut at a span boundary."""
+        _starts_unit(unit)
         data, offs = pack_texts(texts)
-        r = self._plugin().encode_batch(ctx, EncodeBatchRequest(VocabRef(model), data, offs, with_starts=True))
+        req = EncodeBatchRequest(VocabRef(model), data, offs, with_starts=True, starts_unit=unit)
+        plug = self._plugin()
+        r = plug.encode_batch(ctx, req) if unit == "byte" else plug.encode_batch_unit_starts(ctx, req)
         if r.starts is None:
             raise ServiceUnavailable("the tokenizer plugin does not return token starts")
+        lens = np.diff(offs) if unit == "byte" else r.lens
         out = []
         for i in range(len(texts)):
             a, b = int(r.offsets[i]), int(r.offsets[i + 1])
@@ -658,7 +727,7 @@ class LlmGatewayTokenizerService:
             spans[:, 0] = st
             spans[:-1, 1] = st[1:]
             if b > a:
-                spans[-1, 1] = int(offs[i + 1]) - int(offs[i])
+                spans[-1, 1] = int(lens[i])
             out.append((r.ids[a:b], spans))
         return out
 

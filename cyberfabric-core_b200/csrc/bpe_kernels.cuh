@@ -1939,6 +1939,146 @@ chunk_emit_kernel(BatchView b, const uint64_t* __restrict__ out_offsets, const u
     }
 }
 
+// Unit starts (pipeline.cuh, enqueue_emit; after starts_emit): each token's start in code points or UTF-16 units, written over its
+// byte start.  Every byte has a weight w: 0 for a continuation byte (0x80 .. 0xBF), 2 for a lead byte >= 0xF0 in UTF-16 (a code
+// point above the BMP is a surrogate pair), else 1; a token's weight u is the sum over its bytes in the vocabulary blob.  The sum
+// W of u over the prompt's tokens before token k counts every character whose first byte lies before the token's byte start x, so
+// start = W, less w(lead) when x is inside a character (that character was counted, and the token starts in it: its lead byte is
+// at most 3 bytes back in the prompt).  For code points this is tiktoken's decode_with_offsets.  The prompt's length in units is W
+// over all its tokens.
+//   W is relative to the prompt, and the prompt's first token is in general not in the tile of the token at hand.  A per-prompt
+//   base would cost a buffer a prompt and another pass to fill it; instead the scan RESTARTS at every prompt's first token (the
+//   token whose byte start is 0), as a segmented scan: an element is (flag, u), and (a + b) = b when b holds a prompt start,
+//   else (a.flag | b.flag, a.u + b.u).  Each value is already prompt-relative, and the tile arrays of the byte starts (free again
+//   once starts_emit has run) are all the memory it needs.
+//   unit_len:       every tile's aggregate (flag in bit 31: a tile has at most 2048 x 255 bytes of tokens)
+//   unit_tile_scan: one CTA, as tile_scan: the exclusive segmented scan of the aggregates, in 64 bits (a prompt may exceed 2 GiB)
+//   unit_emit:      the segmented scan inside the tile after the tile's base, the lead-byte correction, and the prompt's length
+//                   from the thread that holds its last token (the caller zeroes the lengths: an empty prompt has no token)
+struct UnitView {
+    uint32_t utf16;             // 1: UTF-16 code units, 0: code points
+    uint32_t* lens;             // nullable: out, every prompt's length in units [n_prompts of the (sub-)batch]
+};
+constexpr uint32_t kSegFlag = 0x80000000u;
+constexpr uint64_t kSegFlag64 = 1ull << 63;
+__device__ __forceinline__ uint32_t seg_add(uint32_t a, uint32_t b) { return (b & kSegFlag) ? b : a + b; }
+__device__ __forceinline__ uint64_t seg_add64(uint64_t a, uint64_t b) { return (b & kSegFlag64) ? b : a + b; }
+__device__ __forceinline__ uint32_t unit_weight(uint32_t byte, uint32_t utf16) {
+    return (byte & 0xC0u) == 0x80u ? 0u : (utf16 && byte >= 0xF0u) ? 2u : 1u;
+}
+__device__ __forceinline__ uint32_t token_units(const TablesView& T, uint32_t id, uint32_t utf16) {
+    if (id >= T.n_ranks) return 0u;                 // (ids of a failed pass may be anything)
+    const uint32_t a = T.tokoff[id], e = T.tokoff[id + 1];
+    uint32_t u = 0;
+    for (uint32_t i = a; i < e; ++i) u += unit_weight(T.blob[i], utf16);
+    return u;
+}
+// the exclusive segmented scan of x over a CTA of 256 threads in thread order; *total: the CTA's aggregate.  Every thread calls it.
+__device__ __forceinline__ uint32_t block_seg_scan_256(uint32_t x, uint32_t* s_warp, uint32_t* total) {
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(kFull, x, d); if (lane >= d) x = seg_add(o, x); }
+    const uint32_t prev = __shfl_up_sync(kFull, x, 1);
+    if (lane == 31) s_warp[wid] = x;
+    __syncthreads();
+    uint32_t before = 0, all = 0;
+    for (uint32_t k = 0; k < 8; ++k) { const uint32_t v = s_warp[k]; if (k < wid) before = seg_add(before, v); all = seg_add(all, v); }
+    *total = all;
+    return seg_add(before, lane ? prev : 0u);
+}
+// token r's element: its units, flagged when it is its prompt's first token (byte start 0)
+__device__ __forceinline__ uint32_t unit_elem(uint32_t x, uint32_t u) { return (x ? 0u : kSegFlag) | u; }
+
+__global__ void __launch_bounds__(256)
+unit_len_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ ids, const uint64_t* __restrict__ out_offsets, uint64_t out_cap,
+                const DeviceStatus* status, const uint32_t* __restrict__ starts, uint32_t utf16, uint32_t* __restrict__ tile_aggs) {
+    __shared__ uint32_t s_warp[8];
+    const uint64_t n = status->n_tokens, r0 = status->tok_end - n;
+    const uint64_t lim = r0 + n < out_cap ? r0 + n : out_cap;
+    const uint64_t r = r0 + static_cast<uint64_t>(blockIdx.x) * kStartsTile + 8u * threadIdx.x;
+    uint32_t agg = 0;
+    if (r < lim) {
+        uint32_t p = find_prompt(out_offsets, b.n_prompts, r);
+        for (uint32_t k = 0; k < 8 && r + k < lim; ++k) {
+            p = starts_prompt(out_offsets, p, r + k);
+            agg = seg_add(agg, unit_elem(starts[r + k], token_units(prompt_tables(b, vs, p), ids[r + k], utf16)));
+        }
+    }
+    uint32_t total;
+    block_seg_scan_256(agg, s_warp, &total);
+    if (threadIdx.x == 0) tile_aggs[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(1024)
+unit_tile_scan_kernel(const uint32_t* __restrict__ tile_aggs, uint32_t n_tiles, uint64_t* __restrict__ tile_base) {
+    __shared__ uint64_t s_warp[32];
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarps = (blockDim.x + 31) >> 5;
+    const uint32_t per = ((n_tiles + nwarps - 1) / nwarps + 31u) & ~31u;          // tiles per warp, a multiple of 32
+    const uint32_t lo = wid * per < n_tiles ? wid * per : n_tiles;
+    const uint32_t hi = lo + per < n_tiles ? lo + per : n_tiles;
+    auto scan32 = [&](uint32_t i0, uint64_t* prev) -> uint64_t {     // inclusive scan of tiles i0 .. i0 + 31 (identity past hi)
+        const uint32_t i = i0 + lane;
+        const uint32_t v = i < hi ? tile_aggs[i] : 0u;
+        uint64_t x = static_cast<uint64_t>(v & ~kSegFlag) | (static_cast<uint64_t>(v & kSegFlag) << 32);
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) { const uint64_t o = __shfl_up_sync(kFull, x, d); if (lane >= d) x = seg_add64(o, x); }
+        const uint64_t p = __shfl_up_sync(kFull, x, 1);
+        *prev = lane ? p : 0;
+        return x;
+    };
+    uint64_t agg = 0, prev;
+    for (uint32_t i0 = lo; i0 < hi; i0 += 32) agg = seg_add64(agg, __shfl_sync(kFull, scan32(i0, &prev), 31));
+    if (lane == 0) s_warp[wid] = agg;
+    __syncthreads();
+    uint64_t carry = 0;
+    for (uint32_t w = 0; w < wid; ++w) carry = seg_add64(carry, s_warp[w]);
+    for (uint32_t i0 = lo; i0 < hi; i0 += 32) {
+        const uint64_t x = scan32(i0, &prev);
+        if (i0 + lane < hi) tile_base[i0 + lane] = seg_add64(carry, prev) & ~kSegFlag64;
+        carry = seg_add64(carry, __shfl_sync(kFull, x, 31));
+    }
+}
+
+__global__ void __launch_bounds__(256)
+unit_emit_kernel(BatchView b, VocabSet vs, const uint32_t* __restrict__ ids, const uint64_t* __restrict__ out_offsets, uint64_t out_cap,
+                 const DeviceStatus* status, const uint64_t* __restrict__ tile_base, UnitView uv, uint32_t* __restrict__ starts) {
+    __shared__ uint32_t s_warp[8];
+    const uint64_t n = status->n_tokens, r0 = status->tok_end - n;
+    const uint64_t lim = r0 + n < out_cap ? r0 + n : out_cap;
+    const uint64_t r = r0 + static_cast<uint64_t>(blockIdx.x) * kStartsTile + 8u * threadIdx.x;
+    const uint32_t p0 = r < lim ? find_prompt(out_offsets, b.n_prompts, r) : 0u;
+    uint32_t x[8], u[8], agg = 0;
+#pragma unroll
+    for (uint32_t k = 0, p = p0; k < 8; ++k) {
+        x[k] = 1u; u[k] = 0u;
+        if (r + k < lim) {
+            p = starts_prompt(out_offsets, p, r + k);
+            x[k] = starts[r + k];
+            u[k] = token_units(prompt_tables(b, vs, p), ids[r + k], uv.utf16);
+            agg = seg_add(agg, unit_elem(x[k], u[k]));
+        }
+    }
+    uint32_t total;
+    const uint32_t excl = block_seg_scan_256(agg, s_warp, &total);
+    if (r >= lim) return;
+    uint64_t run = (excl & kSegFlag) ? (excl & ~kSegFlag) : tile_base[blockIdx.x] + excl;   // units of the prompt before token r
+#pragma unroll
+    for (uint32_t k = 0, p = p0; k < 8; ++k) {
+        if (r + k >= lim) break;
+        p = starts_prompt(out_offsets, p, r + k);
+        if (x[k] == 0) run = 0;
+        const uint8_t* s = b.bytes + b.offsets[p];
+        uint32_t start = static_cast<uint32_t>(run), j = x[k];
+        if ((s[j] & 0xC0u) == 0x80u) {            // inside a character: it was counted, and the token starts in it
+            while (j > 0 && (s[j] & 0xC0u) == 0x80u) --j;
+            start -= unit_weight(s[j], uv.utf16);
+        }
+        starts[r + k] = start;
+        run += u[k];
+        if (uv.lens && r + k + 1 == out_offsets[p + 1]) uv.lens[p] = static_cast<uint32_t>(run);
+    }
+}
+
 // ---------------------------------------------------------------------------------------
 // Decode (SURVEY.md section 8(f) item 2): ids -> bytes.  tiktoken's decode_bytes: the concatenation of the tokens' bytes.
 //   decode_len:    length of every token (0xFFFFFFFF + status->bad_utf8-style flag for an id outside the vocabulary),

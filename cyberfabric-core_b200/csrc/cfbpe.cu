@@ -146,6 +146,8 @@ struct Lane {
     DevPtr<uint32_t> d_out_starts;       // host calls with token starts: [max_bytes + 1], allocated on the lane's first such call
     DevPtr<uint32_t> d_trunc;            // host truncate calls: budgets, cuts, kept counts [3 x (max_prompts + 1)], allocated on the
                                          // lane's first such call
+    DevPtr<uint32_t> d_unit_lens;        // host unit-start calls with lengths: every prompt's length in units [max_prompts], allocated
+                                         // on the lane's first such call
     DevPtr<uint64_t> d_chunk_offs;       // host chunk calls: chunk offsets in the layout of d_out_offsets, then the shard chunk totals
                                          // of a multi-device call [CFBPE_MAX_DEVICES]; allocated on the lane's first such call
     Workspace ws{};                      // the kernels' view: its sized buffers are released by ~Lane, its status is d_status
@@ -403,13 +405,26 @@ int ensure_lane_buffer(cfbpe_ctx* ctx, DevPtr<T>& p, uint64_t count, const char*
     cudaGetLastError();
     return fail(ctx, CFBPE_ENOMEM, std::string("no device memory for ") + what);
 }
-// the lane buffers of a call with token starts (cfbpe_encode_batch_starts, chunk calls), of a truncate call, of a host chunk call
-int ensure_call_buffers(cfbpe_ctx* ctx, Lane* ln, bool starts, bool trunc, bool chunk) {
+// the lane buffers of a call with token starts (cfbpe_encode_batch_starts, chunk calls), of a truncate call, of a host chunk call,
+// of a host unit-start call with lengths
+int ensure_call_buffers(cfbpe_ctx* ctx, Lane* ln, bool starts, bool trunc, bool chunk, bool lens = false) {
     const uint64_t mp = ctx->max_prompts;
     int rc = starts ? ensure_lane_buffer(ctx, ln->d_out_starts, ln->max_bytes + 1, "the token starts") : CFBPE_OK;
     if (!rc && trunc) rc = ensure_lane_buffer(ctx, ln->d_trunc, 3 * (mp + 1), "the truncate buffers");
     if (!rc && chunk) rc = ensure_lane_buffer(ctx, ln->d_chunk_offs, lane_offsets_alloc(mp, kMaxPipeChunks) + CFBPE_MAX_DEVICES, "the chunk offsets");
+    if (!rc && lens) rc = ensure_lane_buffer(ctx, ln->d_unit_lens, mp + 1, "the unit lengths");
     return rc;
+}
+
+// A host unit-start call (cfbpe_encode_batch_char_starts): the starts go where byte starts go (the lane's starts buffer, then
+// out_starts), in code points or UTF-16 units; lens (nullable) gets every prompt's length in them.  Under `defer` (a shard of a
+// multi-device call) lens is only a flag: the lengths stay in the lane's buffer at the shard's prompt indices.
+struct UnitArgs { uint32_t utf16; uint32_t* lens; };
+// prompts p0 .. of the call in the lane's length buffer (a sub-batch's prompts keep their index in the call)
+UnitView lane_unit_view(Lane* ln, const UnitArgs& u, uint32_t p0) { return UnitView{u.utf16, u.lens ? ln->d_unit_lens.get() + p0 : nullptr}; }
+int download_lens(cfbpe_ctx* ctx, Lane* ln, uint32_t* lens, uint32_t p0, uint32_t n, cudaStream_t s) {
+    if (lens && n) CK(cudaMemcpyAsync(lens + p0, ln->d_unit_lens.get() + p0, static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    return CFBPE_OK;
 }
 
 // A host truncate call (cfbpe_truncate_batch): budgets in, cuts and kept counts out, one per prompt of the call.  The ids it needs go to
@@ -489,7 +504,7 @@ int upload_batch(cfbpe_ctx* ctx, Lane* ln, uint32_t n, const uint8_t* bytes, con
 int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, int G, uint32_t n, const uint8_t* bytes, const uint64_t* offsets,
                        const uint8_t* vocab_ids, uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
                        bool want_ids, uint64_t total, uint64_t* defer, uint32_t* cut_out, int* nc_out, const TruncateArgs* trunc,
-                       const ChunkArgs* chunk) {
+                       const ChunkArgs* chunk, const UnitArgs* unit = nullptr) {
     // ---- cut
     uint32_t cut[kMaxPipeChunks + 1];
     const int nc = plan_sub_batches(offsets, n, total, ctx->pipe_chunk, kMaxPipeChunks, cut);
@@ -565,9 +580,10 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         if (!chunk) CK(cudaEventRecord(ln->ev_chain[k].get(), ss));
         const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, p0) : TruncateView{};
         const ChunkView cv = chunk ? lane_chunk_view(ln, w, q0, k ? &prev->d_status_arr.get()[k - 1].chunk_end : nullptr, *chunk) : ChunkView{};
+        const UnitView uv = unit ? lane_unit_view(ln, *unit, p0) : UnitView{};
         enqueue_emit(b, w, want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get() + q0, ln->d_out_counts.get() + p0,
                      ss, static_cast<ProfEvents*>(nullptr), (out_starts || chunk) ? ln->d_out_starts.get() : nullptr, &dv->vs, trunc ? &tv : nullptr,
-                     chunk ? &cv : nullptr);
+                     chunk ? &cv : nullptr, unit ? &uv : nullptr);
         if (chunk) CK(cudaEventRecord(ln->ev_chain[k].get(), ss));       // (the chunk scan read the previous chunk_end: the chain ends here)
         CK(cudaGetLastError());
         status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr.get() + k, ln->h_status_arr.get() + k);
@@ -605,6 +621,7 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
             CK(cudaMemcpyAsync(out_starts + base, ln->d_out_starts.get() + base, st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
         if (out_offsets) CK(cudaMemcpyAsync(out_offsets + p0, ln->d_out_offsets.get() + sub_batch_offsets_at(p0, k), (static_cast<uint64_t>(nk) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, ds));
         if (out_counts && nk) CK(cudaMemcpyAsync(out_counts + p0, ln->d_out_counts.get() + p0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, ds));
+        if (unit) { const int rc = download_lens(ctx, ln, unit->lens, p0, nk, ds); if (rc) return rc; }
         if (trace) { CK(cudaEventRecord(ln->trace[k][5].get(), ds)); host_dl[k] = host_ms(); }
     }
     for (int g = 0; g < G; ++g) {
@@ -639,18 +656,19 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
 // trunc != nullptr: a truncate call (the ids stay in the lane; the cuts and kept counts are downloaded, under `defer` too).
 // chunk != nullptr: a chunk call (the ids and starts stay in the lane; the chunk offsets and spans are downloaded, except under
 // `defer`, where chunk->sub_end[0] gets the chunk total).
+// unit != nullptr: a unit-start call (out_starts gets the unit starts; the lengths are downloaded, except under `defer`).
 int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
              uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
              uint64_t* defer = nullptr, uint32_t* cut_out = nullptr, int* nc_out = nullptr, const TruncateArgs* trunc = nullptr,
-             const ChunkArgs* chunk = nullptr) {
+             const ChunkArgs* chunk = nullptr, const UnitArgs* unit = nullptr) {
     CK(cudaSetDevice(dv->device));
     int rc = wait_for_device_call(ctx, ln);
-    if (!rc) rc = ensure_call_buffers(ctx, ln, out_starts || chunk, trunc != nullptr, chunk != nullptr);
+    if (!rc) rc = ensure_call_buffers(ctx, ln, out_starts || chunk, trunc != nullptr, chunk != nullptr, unit && unit->lens);
     if (rc) return rc;
     const bool profiling = ctx->profiling.load();
     if (!profiling && total >= ctx->pipe_min && n >= 2)
         return run_host_pipelined(ctx, &dv, &ln, 1, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                                  defer, cut_out, nc_out, trunc, chunk);
+                                  defer, cut_out, nc_out, trunc, chunk, unit);
     cudaStream_t s = ln->stream.get();
     ProfEvents* prof = profiling ? &ln->prof : nullptr;
     if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0].get(), s); cudaEventRecord(prof->h2d[0].get(), s); }
@@ -662,10 +680,11 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
 
     const TruncateView tv = trunc ? lane_truncate_view(ctx, ln, trunc->tail, 0) : TruncateView{};
     const ChunkView cv = chunk ? lane_chunk_view(ln, ln->ws, 0, nullptr, *chunk) : ChunkView{};
+    const UnitView uv = unit ? lane_unit_view(ln, *unit, 0) : UnitView{};
     enqueue_encode(b, dv->vs, dv->uc, ln->ws, want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get(),
                    ln->d_out_counts.get(), static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
                    ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, (out_starts || chunk) ? ln->d_out_starts.get() : nullptr, trunc ? &tv : nullptr,
-                   chunk ? &cv : nullptr);
+                   chunk ? &cv : nullptr, unit ? &uv : nullptr);
     CK(cudaGetLastError());
     if (prof) cudaEventRecord(prof->d2h[0].get(), s);
     CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
@@ -674,6 +693,7 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
         if (out_offsets) CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets.get(), (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
         if (out_counts && n) CK(cudaMemcpyAsync(out_counts, ln->d_out_counts.get(), static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         if (chunk) CK(cudaMemcpyAsync(chunk->offsets, ln->d_chunk_offs.get(), (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+        if (unit && (rc = download_lens(ctx, ln, unit->lens, 0, n, s))) return rc;
     }
     CK(cudaStreamSynchronize(s));
     const DeviceStatus st = *ln->h_status;
@@ -816,7 +836,8 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
 struct SpecialArgs { const uint8_t* const* modes; uint32_t* bad; };
 int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
                      uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
-                     const SpecialArgs* special = nullptr, const TruncateArgs* trunc = nullptr, const ChunkArgs* chunk = nullptr) {
+                     const SpecialArgs* special = nullptr, const TruncateArgs* trunc = nullptr, const ChunkArgs* chunk = nullptr,
+                     const UnitArgs* unit = nullptr) {
     const uint32_t G = static_cast<uint32_t>(ctx->devs.size());
     std::vector<uint32_t> lo(G + 1, 0);
     for (uint32_t d = 1; d < G; ++d) {      // first prompt whose start is >= d * total / G
@@ -851,7 +872,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
                 const ChunkArgs shard_chunk = chunk ? ChunkArgs{chunk->n, chunk->step, nullptr, UINT64_MAX, nullptr, s.chunk_end} : ChunkArgs{};
                 s.rc = run_lane(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
                                 nullptr, out_starts, 0, nullptr, nullptr, want_ids, s.local_offs[nd], &s.tokens, s.cut, &s.nc,
-                                trunc ? &shard_trunc : nullptr, chunk ? &shard_chunk : nullptr);
+                                trunc ? &shard_trunc : nullptr, chunk ? &shard_chunk : nullptr, unit);
             }
             if (s.rc) s.err = tl_err;
         });
@@ -904,6 +925,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
                 rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(src, cnt, ln->d_totals.get(), d);
                 if (out_offsets) ck(cudaMemcpyAsync(out_offsets + p0 + q0, src, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st), "offsets download");
                 if (out_counts && nk) ck(cudaMemcpyAsync(out_counts + p0 + q0, ln->d_out_counts.get() + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "counts download");
+                if (unit && unit->lens && nk) ck(cudaMemcpyAsync(unit->lens + p0 + q0, ln->d_unit_lens.get() + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "lengths download");
                 if (chunk) {      // chunk offsets: rebased as the token offsets, by the chunk totals of the shards before; spans: prompt-relative
                     uint64_t* csrc = ln->d_chunk_offs.get() + sub_batch_offsets_at(q0, k);
                     rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(csrc, cnt, lane_chunk_totals(ctx, ln), d);
@@ -934,12 +956,12 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     return CFBPE_OK;
 }
 
-// shared body of encode_batch / encode_batch_starts / count_batch / truncate_batch / chunk_batch (host buffers); out_starts: NULL
-// but for encode_batch_starts; trunc: NULL but for truncate_batch, chunk: NULL but for chunk_batch (both emit the ids into the lane,
-// out_ids NULL, out_cap unlimited)
+// shared body of encode_batch / encode_batch_starts / encode_batch_char_starts / count_batch / truncate_batch / chunk_batch (host
+// buffers); out_starts: NULL but for encode_batch_starts and encode_batch_char_starts; trunc: NULL but for truncate_batch, chunk: NULL
+// but for chunk_batch (both emit the ids into the lane, out_ids NULL, out_cap unlimited); unit: NULL but for encode_batch_char_starts
 int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
              uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
-             const TruncateArgs* trunc = nullptr, const ChunkArgs* chunk = nullptr) {
+             const TruncateArgs* trunc = nullptr, const ChunkArgs* chunk = nullptr, const UnitArgs* unit = nullptr) {
     tl_err.clear();
     std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
     uint64_t total = 0;
@@ -961,20 +983,20 @@ int run_host(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* o
                 lns[g] = locks[g]->ln;
                 CK(cudaSetDevice(dvs[g]->device));
                 rc = wait_for_device_call(ctx, lns[g]);
-                if (!rc) rc = ensure_call_buffers(ctx, lns[g], out_starts || chunk, trunc != nullptr, chunk != nullptr);
+                if (!rc) rc = ensure_call_buffers(ctx, lns[g], out_starts || chunk, trunc != nullptr, chunk != nullptr, unit && unit->lens);
                 if (rc) return rc;
             }
             return run_host_pipelined(ctx, dvs, lns, G, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                                      nullptr, nullptr, nullptr, trunc, chunk);
+                                      nullptr, nullptr, nullptr, trunc, chunk, unit);
         }
         return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total, nullptr, trunc,
-                                chunk);
+                                chunk, unit);
     }
     if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds max_batch_bytes of this context");
     DeviceCtx* dv = ctx->devs[0].get();
     LaneLock lk(dv);
     return run_lane(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, want_ids, total,
-                    nullptr, nullptr, nullptr, trunc, chunk);
+                    nullptr, nullptr, nullptr, trunc, chunk, unit);
 }
 
 
@@ -1217,15 +1239,17 @@ int device_call(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint
     return device_call_status(ctx, ln);
 }
 
-// shared body of encode_batch_device / encode_batch_starts_device: d_out_starts (nullable) gets the starts, beside d_out_ids
+// shared body of encode_batch_device / encode_batch_starts_device / encode_batch_char_starts_device: d_out_starts (nullable) gets the
+// starts, beside d_out_ids; unit (nullable): in code points or UTF-16 units, and the prompts' lengths in them
 int run_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
                const uint8_t* d_vocab_ids, uint32_t* d_out_ids, uint32_t* d_out_starts, uint64_t out_cap, uint64_t* d_out_offsets,
-               uint32_t* d_out_counts, uint64_t* n_tokens, void* stream) {
+               uint32_t* d_out_counts, uint64_t* n_tokens, void* stream, const UnitView* unit = nullptr) {
     return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_offsets, d_out_ids != nullptr, out_cap, n_tokens, stream, true,
                        [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents* prof) {
         enqueue_encode(b, dv->vs, dv->uc, ln->ws, d_out_ids, out_cap, d_out_offsets, d_out_counts,
                        static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
-                       ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, d_out_starts);   // profiling: one stream, so that the per-kernel times do not overlap
+                       ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, d_out_starts, nullptr, nullptr,
+                       unit);   // profiling: one stream, so that the per-kernel times do not overlap
         CK(cudaGetLastError());
         return CFBPE_OK;
     });
@@ -1451,6 +1475,17 @@ int cfbpe_encode_batch_starts(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t*
     return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, true);
 }
 
+int cfbpe_encode_batch_char_starts(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                                   uint32_t unit, uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets,
+                                   uint32_t* out_counts, uint32_t* out_lens) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (const char* e = unit_args_error(unit, out_ids, out_starts)) return fail(ctx, CFBPE_EINVAL, e);
+    const UnitArgs u{unit == CFBPE_UNIT_UTF16 ? 1u : 0u, out_lens};
+    return run_host(ctx, n_prompts, bytes, offsets, vocab_ids, out_ids, out_starts, out_cap, out_offsets, out_counts, true, nullptr, nullptr, &u);
+}
+
 int cfbpe_count_batch(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets,
                       const uint8_t* vocab_ids, uint32_t* out_counts) {
     DeviceGuard restore_device;
@@ -1551,6 +1586,19 @@ int cfbpe_encode_batch_starts_device(cfbpe_ctx* ctx, uint32_t n_prompts, const u
     if (!d_out_ids || !d_out_starts) return fail(ctx, CFBPE_EINVAL, "d_out_ids and d_out_starts are required");
     return run_device(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, d_out_starts, out_cap, d_out_offsets, d_out_counts,
                       n_tokens, stream);
+}
+
+int cfbpe_encode_batch_char_starts_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes,
+                                          const uint64_t* d_offsets, const uint8_t* d_vocab_ids, uint32_t unit, uint32_t* d_out_ids,
+                                          uint32_t* d_out_starts, uint64_t out_cap, uint64_t* d_out_offsets, uint32_t* d_out_counts,
+                                          uint32_t* d_out_lens, uint64_t* n_tokens, void* stream) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (const char* e = unit_args_error(unit, d_out_ids, d_out_starts)) return fail(ctx, CFBPE_EINVAL, e);
+    const UnitView uv{unit == CFBPE_UNIT_UTF16 ? 1u : 0u, d_out_lens};
+    return run_device(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, d_out_starts, out_cap, d_out_offsets, d_out_counts,
+                      n_tokens, stream, &uv);
 }
 
 int cfbpe_truncate_batch_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,

@@ -144,6 +144,13 @@ inline const char* chunk_args_error(uint32_t chunk_tokens, uint32_t overlap_toke
     return nullptr;
 }
 
+// the checks of a unit-starts call's own arguments (cfbpe_encode_batch_char_starts and its device form): the error, or nullptr
+inline const char* unit_args_error(uint32_t unit, const uint32_t* ids, const uint32_t* starts) {
+    if (unit != CFBPE_UNIT_CODEPOINT && unit != CFBPE_UNIT_UTF16) return "unit is not a CFBPE_UNIT_* value";
+    if (!ids || !starts) return "out_ids and out_starts are required";
+    return nullptr;
+}
+
 // K2b CTAs per SM (long_grid = 4 x SM count).  8 x 128 threads x 64 registers is the whole register file of an SM: the
 // short-piece kernels on the other stream then wait for K2b instead of running beside it.
 #ifndef CFBPE_LONG_CTAS
@@ -266,11 +273,13 @@ inline void enqueue_scan(const BatchView& b, const Workspace& w, Stream stream, 
 // (truncate_kernel, and truncate_long_kernel for the prompts with more ids to sum than one warp takes).
 // chunk (nullable; only with out_starts): every prompt's chunks of chunk->n tokens, from the starts (chunk_scan, then chunk_emit
 // over a grid of at most kChunkEmitCtas CTAs; a (sub-)batch has no more chunks than bytes).
+// unit (nullable; only with out_starts): the starts in code points or UTF-16 units instead of bytes, and every prompt's length in
+// them (unit_len, unit_tile_scan, unit_emit: a scan of the tokens' units that restarts at every prompt, over the byte starts).
 constexpr uint32_t kChunkEmitCtas = 1024;
 template <typename Stream, typename Prof>
 inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
                          uint32_t* out_counts, Stream stream, Prof* prof, uint32_t* out_starts = nullptr, const VocabSet* vs = nullptr,
-                         const TruncateView* trunc = nullptr, const ChunkView* chunk = nullptr) {
+                         const TruncateView* trunc = nullptr, const ChunkView* chunk = nullptr, const UnitView* unit = nullptr) {
     CFBPE_MARK(prof, K_EMIT, stream, true);
     if (b.total_bytes && out_ids) {
         CFBPE_LAUNCH(emit_compact_kernel, n_scan_tiles(b.total_bytes), 256, stream, w.tok_bits, w.piece_bits, n_flag_words(b.total_bytes), w.tile_base,
@@ -285,6 +294,17 @@ inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_i
         CFBPE_LAUNCH(tile_scan_kernel, 1u, 1024, stream, w.dense.tile_pieces, n_tiles, w.dense.piece_base, static_cast<DeviceStatus*>(nullptr),
                      static_cast<const uint64_t*>(nullptr));
         CFBPE_LAUNCH(starts_emit_kernel, n_tiles, 256, stream, b, out_offsets, out_cap, w.status, w.dense.piece_base, out_starts);
+    }
+    if (out_ids && out_starts && unit) {
+        if (unit->lens && b.n_prompts) CFBPE_ZERO(unit->lens, static_cast<uint64_t>(b.n_prompts) * sizeof(uint32_t), stream);   // (an empty prompt has no token)
+        if (b.total_bytes) {
+            const uint32_t n_tiles = static_cast<uint32_t>((b.total_bytes + kStartsTile - 1) / kStartsTile);
+            CFBPE_LAUNCH(unit_len_kernel, n_tiles, 256, stream, b, *vs, static_cast<const uint32_t*>(out_ids), out_offsets, out_cap, w.status,
+                         static_cast<const uint32_t*>(out_starts), unit->utf16, w.dense.tile_pieces);
+            CFBPE_LAUNCH(unit_tile_scan_kernel, 1u, 1024, stream, static_cast<const uint32_t*>(w.dense.tile_pieces), n_tiles, w.dense.piece_base);
+            CFBPE_LAUNCH(unit_emit_kernel, n_tiles, 256, stream, b, *vs, static_cast<const uint32_t*>(out_ids), out_offsets, out_cap, w.status,
+                         static_cast<const uint64_t*>(w.dense.piece_base), *unit, out_starts);
+        }
     }
     if (out_ids && trunc && b.n_prompts) {
         CFBPE_LAUNCH(truncate_kernel, static_cast<unsigned>((static_cast<uint64_t>(b.n_prompts) + 7) / 8), 256, stream,    // a warp per prompt
@@ -306,22 +326,24 @@ inline void enqueue_emit(const BatchView& b, const Workspace& w, uint32_t* out_i
 template <typename Stream, typename Prof>
 inline void enqueue_back(const BatchView& b, const Workspace& w, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets,
                          uint32_t* out_counts, Stream stream, Prof* prof, const uint64_t* token_base, uint32_t* out_starts = nullptr,
-                         const VocabSet* vs = nullptr, const TruncateView* trunc = nullptr, const ChunkView* chunk = nullptr) {
+                         const VocabSet* vs = nullptr, const TruncateView* trunc = nullptr, const ChunkView* chunk = nullptr,
+                         const UnitView* unit = nullptr) {
     enqueue_count(b, w, stream, prof);
     enqueue_scan(b, w, stream, prof, token_base);
-    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs, trunc, chunk);
+    enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs, trunc, chunk, unit);
 }
 
 // The whole path.  `aux` / `aux2` are streams of their own for the two long-piece kernels (pass the main stream to run everything
 // in order); CFBPE_FORK / CFBPE_JOIN order them.  out_ids may be nullptr (count only); out_starts (nullable, with out_ids): the
 // tokens' byte offsets within their prompts; trunc (nullable, with out_ids): the prompts' cuts to their token budgets; chunk
-// (nullable, with out_starts): the prompts' chunks.  Everything is asynchronous.
+// (nullable, with out_starts): the prompts' chunks; unit (nullable, with out_starts): the starts in code points or UTF-16 units.
+// Everything is asynchronous.
 template <typename Stream, typename Prof, typename Ev>
 inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTables& uc, const Workspace& w,
                            uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
                            uint32_t long_grid, Stream stream, Stream aux, Stream aux2, Ev ev_fork, Ev ev_join, Ev ev_join2, Prof* prof,
                            const uint64_t* token_base = nullptr, uint32_t* out_starts = nullptr, const TruncateView* trunc = nullptr,
-                           const ChunkView* chunk = nullptr) {
+                           const ChunkView* chunk = nullptr, const UnitView* unit = nullptr) {
     enqueue_split(b, vs, uc, w, stream, prof, long_grid / 4);
     CFBPE_FORK(stream, aux2, ev_fork);
     enqueue_list(b, vs, w, long_grid, aux2, prof);
@@ -330,7 +352,7 @@ inline void enqueue_encode(const BatchView& b, const VocabSet& vs, const UcTable
     enqueue_short(b, vs, w, long_grid, stream, prof);
     CFBPE_JOIN(stream, aux, ev_join);
     CFBPE_JOIN(stream, aux2, ev_join2);
-    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base, out_starts, &vs, trunc, chunk);
+    enqueue_back(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, token_base, out_starts, &vs, trunc, chunk, unit);
 }
 
 }  // namespace cfbpe

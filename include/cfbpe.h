@@ -168,6 +168,26 @@ CFBPE_API int cfbpe_encode_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8
 CFBPE_API int cfbpe_encode_batch_starts(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
                                         const uint8_t *vocab_ids, uint32_t *out_ids, uint32_t *out_starts, uint64_t out_cap,
                                         uint64_t *out_offsets, uint32_t *out_counts);
+/* what a unit start counts (cfbpe_encode_batch_char_starts); byte starts are cfbpe_encode_batch_starts */
+#define CFBPE_UNIT_CODEPOINT 0u   /* Unicode code points: Python str indices, tiktoken's decode_with_offsets */
+#define CFBPE_UNIT_UTF16 1u       /* UTF-16 code units (a code point >= U+10000 counts 2): JavaScript, Java and C# string indices */
+/* cfbpe_encode_batch_starts with each token's start counted in `unit` instead of bytes.  For prompt p with bytes b and token k's
+ * byte start x_k (cfbpe_encode_batch_starts), F(x) = the largest character start <= x (the snap of CFBPE_TRUNCATE_HEAD and of the
+ * chunk spans) and U(s) = the units of the byte string s:
+ *   out_starts[k] = U(b[0 .. F(x_k))): the unit index of the character that holds the token's first byte.  For
+ *                   CFBPE_UNIT_CODEPOINT this is tiktoken 0.12.0 decode_with_offsets(ids)[1].
+ *   out_lens[p]   = U(b) (n_prompts entries, may be NULL): closes the last token's span without walking the text.
+ * Within a prompt the starts never decrease and the first is 0.  A character split into several byte tokens gives them all the
+ * same start, so a span built from consecutive starts ([out_starts[k], out_starts[k + 1]), the last one closed by out_lens[p])
+ * can be EMPTY; the spans of a prompt still tile [0, out_lens[p]).  Ids, offsets and counts are those of cfbpe_encode_batch on the
+ * same inputs.  Errors: as cfbpe_encode_batch_starts (CFBPE_ENOSPC: out_offsets[n_prompts] = ids needed); an unknown unit, a NULL
+ * out_ids or a NULL out_starts is CFBPE_EINVAL.  Costs: the lane's token-start buffer (as cfbpe_encode_batch_starts), 4 bytes
+ * per prompt of max_prompts for the lengths on each lane that runs a host call with out_lens (allocated on its first one,
+ * CFBPE_ENOMEM if that fails), and three small kernels after the byte starts: every token's units from the vocabulary's token
+ * bytes, scanned within each prompt. */
+CFBPE_API int cfbpe_encode_batch_char_starts(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
+                                             const uint8_t *vocab_ids, uint32_t unit, uint32_t *out_ids, uint32_t *out_starts,
+                                             uint64_t out_cap, uint64_t *out_offsets, uint32_t *out_counts, uint32_t *out_lens);
 /* Token counts only (no id stream leaves the device). */
 CFBPE_API int cfbpe_count_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
                       const uint8_t *vocab_ids, uint32_t *out_counts);
@@ -282,6 +302,14 @@ CFBPE_API int cfbpe_encode_batch_starts_device(cfbpe_ctx *ctx, uint32_t n_prompt
                                                const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t *d_out_ids,
                                                uint32_t *d_out_starts, uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
                                                uint64_t *n_tokens, void *stream);
+/* cfbpe_encode_batch_char_starts on device-resident buffers, as cfbpe_encode_batch_starts_device: the unit starts go straight to
+ * d_out_starts (room for out_cap entries), the lengths to d_out_lens (n_prompts entries, device memory, may be NULL).  d_out_ids
+ * and d_out_starts are required and unit must be a CFBPE_UNIT_* value (else CFBPE_EINVAL).  n_tokens (host, may be NULL) is
+ * written after an internal stream sync; with n_tokens == NULL the call is fully asynchronous. */
+CFBPE_API int cfbpe_encode_batch_char_starts_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
+                                                    const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t unit,
+                                                    uint32_t *d_out_ids, uint32_t *d_out_starts, uint64_t out_cap, uint64_t *d_out_offsets,
+                                                    uint32_t *d_out_counts, uint32_t *d_out_lens, uint64_t *n_tokens, void *stream);
 /* cfbpe_truncate_batch on device-resident buffers, enqueued on `stream` as cfbpe_encode_batch_device (d_bytes readable for 32
  * bytes past total_bytes).  d_budgets, d_out_cut, d_out_kept and d_out_counts (may be NULL) are device memory.  Fully
  * asynchronous: nothing has to come back to the host, and the ids, which never exceed max_batch_bytes, stay in the lane's

@@ -29,6 +29,10 @@ pub const CFBPE_MAX_SPECIALS: usize = 4096;
 pub const CFBPE_TRUNCATE_HEAD: u32 = 0;
 pub const CFBPE_TRUNCATE_TAIL: u32 = 1;
 
+/// `cfbpe_encode_batch_char_starts`: what a unit start counts
+pub const CFBPE_UNIT_CODEPOINT: u32 = 0;
+pub const CFBPE_UNIT_UTF16: u32 = 1;
+
 pub const CFBPE_FORMAT_TIKTOKEN: u32 = 0;
 pub const CFBPE_FORMAT_TEKKEN_JSON: u32 = 1;
 pub const CFBPE_MAX_VOCABS: u32 = 8;
@@ -84,6 +88,13 @@ extern "C" {
     pub fn cfbpe_encode_batch_starts_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64, d_offsets: *const u64,
                                             d_vocab_ids: *const u8, d_out_ids: *mut u32, d_out_starts: *mut u32, out_cap: u64,
                                             d_out_offsets: *mut u64, d_out_counts: *mut u32, n_tokens: *mut u64, stream: *mut c_void) -> c_int;
+    pub fn cfbpe_encode_batch_char_starts(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64, vocab_ids: *const u8,
+                                          unit: u32, out_ids: *mut u32, out_starts: *mut u32, out_cap: u64, out_offsets: *mut u64,
+                                          out_counts: *mut u32, out_lens: *mut u32) -> c_int;
+    pub fn cfbpe_encode_batch_char_starts_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64, d_offsets: *const u64,
+                                                 d_vocab_ids: *const u8, unit: u32, d_out_ids: *mut u32, d_out_starts: *mut u32, out_cap: u64,
+                                                 d_out_offsets: *mut u64, d_out_counts: *mut u32, d_out_lens: *mut u32, n_tokens: *mut u64,
+                                                 stream: *mut c_void) -> c_int;
     pub fn cfbpe_count_batch(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64,
                              vocab_ids: *const u8, out_counts: *mut u32) -> c_int;
     pub fn cfbpe_truncate_batch(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64, vocab_ids: *const u8,
@@ -266,6 +277,30 @@ impl Ctx {
         starts.truncate(out.ids.len());
         out.counts.truncate(n as usize);
         Ok((out, starts))
+    }
+
+    /// [`Ctx::encode_batch`] plus every token's start within its prompt in `unit` (`CFBPE_UNIT_CODEPOINT` or `CFBPE_UNIT_UTF16`):
+    /// `(out, starts, lens)`, `starts[k]` for `ids[k]` and `lens[i]` the length of prompt i in the unit.  A token's start is that of
+    /// the character holding its first byte, so byte tokens of one character share it.
+    pub fn encode_batch_char_starts(&self, bytes: &[u8], offsets: &[u64], vocab_ids: Option<&[u8]>, unit: u32)
+        -> Result<(Encoded, Vec<u32>, Vec<u32>), NativeError> {
+        let n = Self::check_inputs(bytes.len(), offsets, vocab_ids)?;
+        let total = offsets[n as usize] as usize;
+        let mut out = Encoded { ids: vec![0; total.max(1)], offsets: vec![0; n as usize + 1], counts: vec![0; (n as usize).max(1)] };
+        let mut starts = vec![0u32; total.max(1)];
+        let mut lens = vec![0u32; (n as usize).max(1)];
+        // SAFETY: all buffers are valid for the sizes passed; `starts` has room for as many entries as `ids`, `lens` one per prompt.
+        let rc = unsafe {
+            cfbpe_encode_batch_char_starts(self.0.as_ptr(), n, bytes.as_ptr(), offsets.as_ptr(), vocab_ids.map_or(std::ptr::null(), <[u8]>::as_ptr),
+                                           unit, out.ids.as_mut_ptr(), starts.as_mut_ptr(), out.ids.len() as u64, out.offsets.as_mut_ptr(),
+                                           out.counts.as_mut_ptr(), lens.as_mut_ptr())
+        };
+        self.check(rc)?;
+        out.ids.truncate(out.offsets[n as usize] as usize);
+        starts.truncate(out.ids.len());
+        out.counts.truncate(n as usize);
+        lens.truncate(n as usize);
+        Ok((out, starts, lens))
     }
 
     /// Register `(token, id)` pairs as the special tokens of a vocabulary slot (the pair order is the special index the

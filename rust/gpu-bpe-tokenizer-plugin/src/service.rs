@@ -6,8 +6,8 @@ use std::sync::Arc;
 use async_trait::async_trait;
 use cfbpe_sys::{Ctx, NativeError};
 use llm_gateway_sdk::{
-    ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens, TokenizerError,
-    TokenizerPluginClient, TruncateBatchResponse, TruncateKeep, VocabRef,
+    ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, OffsetUnit, SpecialTokens,
+    TokenizerError, TokenizerPluginClient, TruncateBatchResponse, TruncateKeep, VocabRef,
 };
 use modkit_security::SecurityContext;
 use sha2::{Digest, Sha256};
@@ -109,17 +109,27 @@ impl TokenizerPluginClient for Service {
         let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
         let native = self.native.clone();
         // never block a tokio worker on a CUDA synchronisation (precedent: modules/file-parser/src/infra/parsers/html_parser.rs:47)
-        let (out, starts) = tokio::task::spawn_blocking(move || {
-            if req.with_starts {
-                native.encode_batch_starts(&req.bytes, &req.offsets, vid.as_deref()).map(|(e, s)| (e, Some(s)))
-            } else {
-                native.encode_batch(&req.bytes, &req.offsets, vid.as_deref()).map(|e| (e, None))
+        let (out, starts, lens) = tokio::task::spawn_blocking(move || {
+            let unit = match req.starts_unit {
+                OffsetUnit::Byte => None,
+                OffsetUnit::Codepoint => Some(cfbpe_sys::CFBPE_UNIT_CODEPOINT),
+                OffsetUnit::Utf16 => Some(cfbpe_sys::CFBPE_UNIT_UTF16),
+            };
+            match (req.with_starts, unit) {
+                (true, Some(u)) => native.encode_batch_char_starts(&req.bytes, &req.offsets, vid.as_deref(), u).map(|(e, s, l)| (e, Some(s), Some(l))),
+                (true, None) => native.encode_batch_starts(&req.bytes, &req.offsets, vid.as_deref()).map(|(e, s)| (e, Some(s), None)),
+                (false, _) => native.encode_batch(&req.bytes, &req.offsets, vid.as_deref()).map(|e| (e, None, None)),
             }
         })
             .await
             .map_err(|e| TokenizerError::Internal(e.to_string()))?
             .map_err(map_native)?;
-        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts })
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts, lens })
+    }
+
+    /// The device path (`cfbpe_encode_batch_char_starts`): the unit starts are computed where the ids and byte starts are.
+    async fn encode_batch_unit_starts(&self, ctx: &SecurityContext, req: EncodeBatchRequest) -> Result<EncodeBatchResponse, TokenizerError> {
+        self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, ..req }).await
     }
 
     async fn count_tokens(&self, _ctx: &SecurityContext, req: CountTokensRequest) -> Result<Vec<u32>, TokenizerError> {
@@ -211,7 +221,7 @@ impl TokenizerPluginClient for Service {
         .await
         .map_err(|e| TokenizerError::Internal(e.to_string()))?
         .map_err(map_native)?;
-        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts: None })
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts: None, lens: None })
     }
 }
 

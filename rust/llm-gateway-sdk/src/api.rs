@@ -5,16 +5,18 @@ use modkit_security::SecurityContext;
 use serde_json::Value;
 
 use crate::error::TokenizerError;
-use crate::models::{ChatTemplate, SpecialTokens, TruncateKeep, Usage};
+use crate::models::{ChatTemplate, OffsetUnit, SpecialTokens, TruncateKeep, Usage};
 
 #[async_trait]
 pub trait TokenizerClient: Send + Sync {
     /// `encode_ordinary` of every text under the vocabulary of `model` (canonical id or vocabulary name).
     async fn encode(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<Vec<u32>>, TokenizerError>;
 
-    /// Per text: the ids and each token's `[start, end)` byte span in the text's UTF-8 (cut to a context window or into chunks
-    /// at a span boundary).
-    async fn encode_with_offsets(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError>;
+    /// Per text: the ids and each token's `[start, end)` span in `unit`: bytes of the text's UTF-8, code points, or UTF-16 code
+    /// units (cut to a context window or into chunks at a span boundary).  In a character unit, byte tokens of one character share
+    /// its start, so some spans are empty; the spans still tile the text.
+    async fn encode_with_offsets(&self, ctx: &SecurityContext, model: &str, texts: &[String], unit: OffsetUnit)
+        -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError>;
 
     /// Fit texts into a context window: per text, (the kept text, its tokens, the tokens of the whole text).  `max_tokens`: one
     /// budget per text; `keep`: the first or the last tokens.  The cut is at a character boundary, so the kept text is valid UTF-8.

@@ -19,7 +19,7 @@ pub use api::TokenizerClient;
 pub use error::TokenizerError;
 pub use gts::TokenizerPluginSpecV1;
 pub use models::{
-    chunk_spans, truncate_cut, ChatTemplate, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens,
+    chunk_spans, truncate_cut, unit_starts, ChatTemplate, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, OffsetUnit, SpecialTokens,
     TruncateBatchResponse, TruncateKeep, Usage, VocabRef,
 };
 pub use plugin_api::TokenizerPluginClient;

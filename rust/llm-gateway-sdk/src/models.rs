@@ -27,6 +27,9 @@ pub struct EncodeBatchRequest {
     pub vocab_index: Option<Vec<u8>>,
     /// also return every token's byte offset within its prompt (`EncodeBatchResponse::starts`); `false` for a plain encode
     pub with_starts: bool,
+    /// with `with_starts`: the unit of the starts (`OffsetUnit::Byte` for byte offsets; a character unit also fills
+    /// `EncodeBatchResponse::lens`)
+    pub starts_unit: OffsetUnit,
 }
 
 #[derive(Debug, Clone, Default, Serialize, Deserialize)]
@@ -40,6 +43,46 @@ pub struct EncodeBatchResponse {
     /// `bytes[offsets_in[i] + starts[k] .. offsets_in[i] + end)`, `end` the next start or the prompt's length)
     #[serde(default, skip_serializing_if = "Option::is_none")]
     pub starts: Option<Vec<u32>>,
+    /// with a character `starts_unit`: every prompt's length in that unit (closes the last token's span)
+    #[serde(default, skip_serializing_if = "Option::is_none")]
+    pub lens: Option<Vec<u32>>,
+}
+
+/// What a token start counts (`include/cfbpe.h`, `cfbpe_encode_batch_char_starts`).
+#[derive(Debug, Clone, Copy, PartialEq, Eq, Default, Serialize, Deserialize, schemars::JsonSchema)]
+#[serde(rename_all = "lowercase")]
+pub enum OffsetUnit {
+    /// bytes of the UTF-8 text
+    #[default]
+    Byte,
+    /// Unicode code points: Python `str` indices, tiktoken's `decode_with_offsets`
+    Codepoint,
+    /// UTF-16 code units (a code point >= U+10000 counts 2): JavaScript, Java and C# string indices
+    Utf16,
+}
+
+/// The unit-start contract on the host, from every token's byte start (`EncodeBatchResponse::starts`): `(starts, len)` of prompt
+/// `prompt` (its UTF-8 bytes, valid), whose tokens start at byte `byte_starts`, in `unit`.  A token's start is the number of units
+/// before the character that holds its first byte; `len` is the prompt's length in units.
+pub fn unit_starts(prompt: &[u8], byte_starts: &[u32], unit: OffsetUnit) -> (Vec<u32>, u32) {
+    if unit == OffsetUnit::Byte {
+        return (byte_starts.to_vec(), prompt.len() as u32);
+    }
+    let weight = |b: u8| -> u32 {
+        if b & 0xC0 == 0x80 { 0 } else if unit == OffsetUnit::Utf16 && b >= 0xF0 { 2 } else { 1 }
+    };
+    // units[x] = units of the characters that start before byte x
+    let mut units = Vec::with_capacity(prompt.len() + 1);
+    units.push(0u32);
+    for &b in prompt {
+        units.push(units.last().copied().unwrap_or(0) + weight(b));
+    }
+    let starts = byte_starts.iter().map(|&x| {
+        let mut x = x as usize;
+        while x > 0 && x < prompt.len() && prompt[x] & 0xC0 == 0x80 { x -= 1; }
+        units[x]
+    }).collect();
+    (starts, units[prompt.len()])
 }
 
 /// Which tokens a truncation keeps.

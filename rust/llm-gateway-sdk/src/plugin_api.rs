@@ -4,8 +4,8 @@ use async_trait::async_trait;
 use modkit_security::SecurityContext;
 
 use crate::error::TokenizerError;
-use crate::models::{chunk_spans, truncate_cut, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, SpecialTokens,
-                    TruncateBatchResponse, TruncateKeep, VocabRef};
+use crate::models::{chunk_spans, truncate_cut, unit_starts, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse,
+                    OffsetUnit, SpecialTokens, TruncateBatchResponse, TruncateKeep, VocabRef};
 
 /// Each plugin registers this trait with a scoped `ClientHub` entry using its GTS instance id as the scope.  Clients are
 /// `Arc<dyn … + Send + Sync>` shared by all tokio tasks (`libs/modkit/src/client_hub.rs:142-165`): calls are concurrent and
@@ -36,7 +36,7 @@ pub trait TokenizerPluginClient: Send + Sync {
         }
         let bytes = req.bytes.clone();
         let offsets = req.offsets.clone();
-        let enc = self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, ..req }).await?;
+        let enc = self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, starts_unit: OffsetUnit::Byte, ..req }).await?;
         let starts = enc.starts.ok_or_else(|| TokenizerError::ServiceUnavailable("the tokenizer plugin does not return token starts".to_owned()))?;
         let mut out = TruncateBatchResponse { cut: Vec::with_capacity(n), kept: Vec::with_capacity(n), counts: enc.counts };
         for i in 0..n {
@@ -60,7 +60,7 @@ pub trait TokenizerPluginClient: Send + Sync {
         let n = req.offsets.len().saturating_sub(1);
         let bytes = req.bytes.clone();
         let offsets = req.offsets.clone();
-        let enc = self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, ..req }).await?;
+        let enc = self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, starts_unit: OffsetUnit::Byte, ..req }).await?;
         let starts = enc.starts.ok_or_else(|| TokenizerError::ServiceUnavailable("the tokenizer plugin does not return token starts".to_owned()))?;
         let mut out = ChunkBatchResponse { spans: Vec::new(), chunk_offsets: Vec::with_capacity(n + 1), counts: enc.counts };
         out.chunk_offsets.push(0);
@@ -70,6 +70,32 @@ pub trait TokenizerPluginClient: Send + Sync {
             out.chunk_offsets.push(out.spans.len() as u64);
         }
         Ok(out)
+    }
+
+    /// `encode_batch` with every token's start in `req.starts_unit` and, for a character unit, every prompt's length in it
+    /// (`EncodeBatchResponse::lens`) -- `include/cfbpe.h`, `cfbpe_encode_batch_char_starts`.  The default works on any plugin that
+    /// returns byte starts: one `encode_batch` with byte starts, then `unit_starts` on the host.  `gpu-bpe-tokenizer-plugin`
+    /// overrides it with the device call, which walks no text on the host.
+    async fn encode_batch_unit_starts(&self, ctx: &SecurityContext, req: EncodeBatchRequest) -> Result<EncodeBatchResponse, TokenizerError> {
+        let unit = req.starts_unit;
+        let n = req.offsets.len().saturating_sub(1);
+        let bytes = req.bytes.clone();
+        let offsets = req.offsets.clone();
+        let mut enc = self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, starts_unit: OffsetUnit::Byte, ..req }).await?;
+        if unit == OffsetUnit::Byte {
+            return Ok(enc);
+        }
+        let byte_starts = enc.starts.take().ok_or_else(|| TokenizerError::ServiceUnavailable("the tokenizer plugin does not return token starts".to_owned()))?;
+        let (mut starts, mut lens) = (Vec::with_capacity(byte_starts.len()), Vec::with_capacity(n));
+        for i in 0..n {
+            let prompt = &bytes[offsets[i] as usize..offsets[i + 1] as usize];
+            let (s, len) = unit_starts(prompt, &byte_starts[enc.offsets[i] as usize..enc.offsets[i + 1] as usize], unit);
+            starts.extend(s);
+            lens.push(len);
+        }
+        enc.starts = Some(starts);
+        enc.lens = Some(lens);
+        Ok(enc)
     }
 
     /// tiktoken's `encode(text, allowed_special = …, disallowed_special = …)` for every prompt of the batch; `InvalidInput` when
@@ -115,14 +141,14 @@ pub trait TokenizerPluginClient: Send + Sync {
             plan.push(steps);
         }
         let enc = if stretches.is_empty() {
-            EncodeBatchResponse { ids: Vec::new(), offsets: vec![0], counts: Vec::new(), starts: None }
+            EncodeBatchResponse { ids: Vec::new(), offsets: vec![0], counts: Vec::new(), starts: None, lens: None }
         } else {
             let mut bytes = Vec::new();
             let mut offsets = vec![0u64];
             for s in &stretches { bytes.extend_from_slice(s.as_bytes()); offsets.push(bytes.len() as u64); }
-            self.encode_batch(ctx, EncodeBatchRequest { vocab: req.vocab.clone(), bytes: bytes.into(), offsets, vocabs_per_prompt: per.take(), vocab_index: None, with_starts: false }).await?
+            self.encode_batch(ctx, EncodeBatchRequest { vocab: req.vocab.clone(), bytes: bytes.into(), offsets, vocabs_per_prompt: per.take(), vocab_index: None, with_starts: false, starts_unit: OffsetUnit::Byte }).await?
         };
-        let mut out = EncodeBatchResponse { ids: Vec::new(), offsets: vec![0u64], counts: Vec::with_capacity(n), starts: None };
+        let mut out = EncodeBatchResponse { ids: Vec::new(), offsets: vec![0u64], counts: Vec::with_capacity(n), starts: None, lens: None };
         for steps in plan {
             let start = out.ids.len();
             for s in steps {

@@ -14,9 +14,13 @@ pub struct TokenizeRequest {
     /// return the ids as well as the counts
     #[serde(default)]
     pub return_ids: bool,
-    /// return each token's `[start, end)` byte span in its text's UTF-8 as well
+    /// return each token's `[start, end)` span in its text as well
     #[serde(default)]
     pub return_offsets: bool,
+    /// the unit of `offsets`: `byte` (UTF-8, the default), `codepoint` (Python string indices) or `utf16` (JavaScript, Java and C#
+    /// string indices).  In a character unit, byte tokens of one character share its start, so some spans are empty.
+    #[serde(default)]
+    pub offset_unit: llm_gateway_sdk::OffsetUnit,
 }
 
 #[derive(Debug, Serialize, JsonSchema)]
@@ -27,7 +31,7 @@ pub struct TokenizeResponse {
     /// token ids of every text, when asked for
     #[serde(skip_serializing_if = "Option::is_none")]
     pub ids: Option<Vec<Vec<u32>>>,
-    /// byte span of every token of every text, when asked for
+    /// span of every token of every text in `offset_unit`, when asked for
     #[serde(skip_serializing_if = "Option::is_none")]
     pub offsets: Option<Vec<Vec<[u64; 2]>>>,
 }

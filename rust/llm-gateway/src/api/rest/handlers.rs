@@ -30,7 +30,7 @@ pub async fn tokenize(
     // only sizes are logged, never the text (docs/DESIGN.md:120-124)
     tracing::debug!(model = %req.model, texts = req.texts.len(), bytes = req.texts.iter().map(String::len).sum::<usize>(), "tokenize");
     let (ids, offsets) = if req.return_offsets {
-        let r = service.encode_with_offsets(&ctx, &req.model, &req.texts).await.map_err(problem)?;
+        let r = service.encode_with_offsets(&ctx, &req.model, &req.texts, req.offset_unit).await.map_err(problem)?;
         let (ids, spans): (Vec<_>, Vec<_>) = r.into_iter().unzip();
         (ids, Some(spans))
     } else {

@@ -7,7 +7,7 @@ use std::sync::Arc;
 use async_trait::async_trait;
 use bytes::Bytes;
 use llm_gateway_sdk::{
-    ChatTemplate, CountTokensRequest, EncodeBatchRequest, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1,
+    ChatTemplate, CountTokensRequest, EncodeBatchRequest, OffsetUnit, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1,
     TruncateKeep, Usage, VocabRef,
 };
 use modkit::client_hub::{ClientHub, ClientScope};
@@ -63,7 +63,8 @@ impl TokenizerService {
     pub async fn chunk_with_spans(&self, ctx: &SecurityContext, model: &str, texts: &[String], max_tokens: u32, overlap: u32)
         -> Result<Vec<(Vec<String>, Vec<[u32; 2]>, u32)>, TokenizerError> {
         let (bytes, offsets) = pack_texts(texts);
-        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false };
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
+                                       starts_unit: OffsetUnit::Byte };
         let r = self.plugin().await?.chunk_batch(ctx, req, max_tokens, overlap).await?;
         texts.iter().enumerate().map(|(i, t)| {
             let spans = r.spans[r.chunk_offsets[i] as usize..r.chunk_offsets[i + 1] as usize].to_vec();
@@ -90,19 +91,28 @@ impl TokenizerService {
 impl TokenizerClient for TokenizerService {
     async fn encode(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<Vec<u32>>, TokenizerError> {
         let (bytes, offsets) = pack_texts(texts);
-        let r = self.plugin().await?.encode_batch(ctx, EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false }).await?;
+        let r = self.plugin().await?.encode_batch(ctx, EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
+                                       starts_unit: OffsetUnit::Byte }).await?;
         Ok((0..texts.len()).map(|i| r.ids[r.offsets[i] as usize..r.offsets[i + 1] as usize].to_vec()).collect())
     }
 
-    async fn encode_with_offsets(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError> {
+    async fn encode_with_offsets(&self, ctx: &SecurityContext, model: &str, texts: &[String], unit: OffsetUnit)
+        -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError> {
         let (bytes, offsets) = pack_texts(texts);
         let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets: offsets.clone(), vocabs_per_prompt: None, vocab_index: None,
-                                       with_starts: true };
-        let r = self.plugin().await?.encode_batch(ctx, req).await?;
+                                       with_starts: true, starts_unit: unit };
+        // a character unit: the plugin does the work (the trait's default converts byte starts on the host, the GPU plugin counts on the device)
+        let plugin = self.plugin().await?;
+        let r = if unit == OffsetUnit::Byte { plugin.encode_batch(ctx, req).await? } else { plugin.encode_batch_unit_starts(ctx, req).await? };
         let starts = r.starts.ok_or_else(|| TokenizerError::ServiceUnavailable("the tokenizer plugin does not return token starts".to_owned()))?;
+        let lens: Vec<u64> = match (unit, &r.lens) {
+            (OffsetUnit::Byte, _) => (0..texts.len()).map(|i| offsets[i + 1] - offsets[i]).collect(),
+            (_, Some(l)) => l.iter().map(|&x| u64::from(x)).collect(),
+            (_, None) => return Err(TokenizerError::ServiceUnavailable("the tokenizer plugin does not return prompt lengths".to_owned())),
+        };
         Ok((0..texts.len()).map(|i| {
             let (a, b) = (r.offsets[i] as usize, r.offsets[i + 1] as usize);
-            let len = offsets[i + 1] - offsets[i];
+            let len = lens[i];
             let spans = (a..b).map(|k| [u64::from(starts[k]), if k + 1 < b { u64::from(starts[k + 1]) } else { len }]).collect();
             (r.ids[a..b].to_vec(), spans)
         }).collect())
@@ -115,7 +125,8 @@ impl TokenizerClient for TokenizerService {
             return Err(TokenizerError::InvalidInput("one token budget per text".to_owned()));
         }
         let (bytes, offsets) = pack_texts(texts);
-        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false };
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
+                                       starts_unit: OffsetUnit::Byte };
         let r = self.plugin().await?.truncate_batch(ctx, req, max_tokens, keep).await?;
         texts.iter().enumerate().map(|(i, t)| {
             let cut = r.cut[i] as usize;
@@ -138,7 +149,8 @@ impl TokenizerClient for TokenizerService {
             return Err(TokenizerError::InvalidInput(format!("allowed special token without an id: {unknown}")));
         }
         let (bytes, offsets) = pack_texts(texts);
-        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false };
+        let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
+                                       starts_unit: OffsetUnit::Byte };
         let r = self.plugin().await?.encode_batch_special(ctx, req, special).await?;
         Ok((0..texts.len()).map(|i| r.ids[r.offsets[i] as usize..r.offsets[i + 1] as usize].to_vec()).collect())
     }
