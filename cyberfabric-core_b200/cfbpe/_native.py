@@ -32,6 +32,7 @@ EXPORTS = [
     "cfbpe_encode_batch_char_starts", "cfbpe_encode_batch_char_starts_device",
     "cfbpe_truncate_batch", "cfbpe_truncate_batch_device",
     "cfbpe_chunk_batch", "cfbpe_chunk_batch_device",
+    "cfbpe_encode_batch_lossy", "cfbpe_encode_batch_lossy_device",
 ]
 
 
@@ -132,6 +133,11 @@ def load():
     L.cfbpe_encode_batch_special_device.restype = C.c_int
     L.cfbpe_encode_batch_special_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, C.c_uint64, vp, vp,
                                                     C.POINTER(C.c_uint64), vp, vp]
+    L.cfbpe_encode_batch_lossy.restype = C.c_int
+    L.cfbpe_encode_batch_lossy.argtypes = [vp, C.c_uint32, u8p, vp, u8p, vp, C.c_uint64, vp, vp, vp]
+    L.cfbpe_encode_batch_lossy_device.restype = C.c_int
+    L.cfbpe_encode_batch_lossy_device.argtypes = [vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp, vp,
+                                                  C.POINTER(C.c_uint64), vp]
     L.cfbpe_device_status.restype = C.c_int
     L.cfbpe_device_status.argtypes = [vp, vp]
     L.cfbpe_host_alloc.restype = vp
@@ -531,6 +537,40 @@ class Context:
             e = NativeError(rc, load().cfbpe_last_error(self._h).decode("utf-8", "replace"))
             e.bad = (int(bad[0]), int(bad[1])) if rc == EBADMSG else None
             raise e
+
+    # ---- bytes that are not valid UTF-8
+    def encode_batch_lossy(self, data: np.ndarray, offsets: np.ndarray, vocab_ids=None, out_ids=None, out_offsets=None, out_counts=None,
+                           out_replaced=None, counts_only=False):
+        """encode every prompt as b.decode("utf-8", "replace") would be encoded: (ids, offsets, counts, replaced).  replaced: uint32,
+        the U+FFFD the decode inserted into each prompt (0: valid UTF-8).  counts_only: ids is None."""
+        n = self._check_inputs(data, offsets, vocab_ids)
+        total = int(offsets[n])
+        if out_ids is None and not counts_only:
+            out_ids = np.empty(max(3 * total, 1), dtype=np.uint32)      # (the repaired text is at most 3 bytes a byte)
+        if out_offsets is None:
+            out_offsets = np.empty(n + 1, dtype=np.uint64)
+        if out_counts is None:
+            out_counts = np.empty(max(n, 1), dtype=np.uint32)
+        if out_replaced is None:
+            out_replaced = np.empty(max(n, 1), dtype=np.uint32)
+        elif not isinstance(out_replaced, np.ndarray) or out_replaced.dtype != np.uint32 or out_replaced.size < n or not out_replaced.flags.c_contiguous:
+            raise NativeError(EINVAL, "out_replaced must be a C-contiguous uint32 array with one entry per prompt")
+        vid = None if vocab_ids is None else vocab_ids.ctypes.data
+        rc = load().cfbpe_encode_batch_lossy(self._h, n, data.ctypes.data if data.size else None, offsets.ctypes.data, vid,
+                                             None if counts_only else out_ids.ctypes.data, 0 if counts_only else out_ids.size,
+                                             out_offsets.ctypes.data, out_counts.ctypes.data, out_replaced.ctypes.data)
+        self._check(rc)
+        return (None if counts_only else out_ids[:int(out_offsets[n])]), out_offsets, out_counts[:n], out_replaced[:n]
+
+    def encode_batch_lossy_device(self, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, out_cap, d_out_offsets,
+                                  d_out_counts, d_out_replaced, stream=0, sync=True):
+        """cfbpe_encode_batch_lossy_device on raw device pointers (d_out_replaced: n_prompts uint32 or None); the id count when sync.
+        The call synchronises `stream` once after its scan either way."""
+        nt = C.c_uint64(0)
+        rc = load().cfbpe_encode_batch_lossy_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, out_cap,
+                                                    d_out_offsets, d_out_counts, d_out_replaced, C.byref(nt) if sync else None, stream)
+        self._check(rc)
+        return nt.value if sync else None
 
     def device_status(self, stream=0):
         self._check(load().cfbpe_device_status(self._h, stream))

@@ -100,6 +100,8 @@ class EncodeBatchRequest:
                                                # vocab_index[i] picks prompt i's (large batches: no per-prompt objects)
     with_starts: bool = False    # also return every token's byte offset within its prompt (EncodeBatchResponse.starts)
     starts_unit: str = "byte"    # with with_starts: "byte", or "codepoint" / "utf16" -- the starts in that unit and EncodeBatchResponse.lens
+    errors: str = "strict"       # bytes that are not valid UTF-8: "strict" fails the call, "replace" encodes every prompt as
+                                 # bytes.decode("utf-8", "replace") (EncodeBatchResponse.replaced; not with with_starts)
 
 
 @dataclass
@@ -109,6 +111,7 @@ class EncodeBatchResponse:
     counts: np.ndarray           # uint32, n
     starts: Optional[np.ndarray] = None   # uint32, one per id: offset of the token within its prompt in starts_unit (with_starts)
     lens: Optional[np.ndarray] = None     # uint32, one per prompt: its length in starts_unit (a "codepoint" / "utf16" request)
+    replaced: Optional[np.ndarray] = None  # uint32, one per prompt: the U+FFFD its decode inserted (an errors="replace" request)
 
 
 @dataclass
@@ -246,6 +249,42 @@ class CountTokensRequest:
     offsets: np.ndarray
     vocabs_per_prompt: Optional[Sequence[VocabRef]] = None
     vocab_index: Optional[np.ndarray] = None
+    errors: str = "strict"       # as EncodeBatchRequest.errors
+
+
+UTF8_ERRORS = ("strict", "replace")
+
+
+def _errors(req) -> str:
+    """req.errors, checked: "replace" gives positions in the repaired text, not the caller's bytes, so it takes no starts"""
+    e = getattr(req, "errors", "strict")
+    if e not in UTF8_ERRORS:
+        raise InvalidInput("errors must be 'strict' or 'replace', not %r" % (e,))
+    if e == "replace" and getattr(req, "with_starts", False):
+        raise InvalidInput("errors='replace' does not return starts: they would index the repaired text, not the request's bytes")
+    return e
+
+
+def repair_utf8(data: np.ndarray, offsets: np.ndarray):
+    """every prompt as bytes.decode("utf-8", "replace").encode("utf-8") on the host: (bytes uint8, offsets uint64, replaced uint32
+    -- the U+FFFD each decode inserted, one per maximal subpart of an ill-formed sequence)"""
+    n = len(offsets) - 1
+    raw = data.tobytes()
+    parts, replaced = [], np.zeros(n, dtype=np.uint32)
+    for i in range(n):
+        p = raw[int(offsets[i]):int(offsets[i + 1])]
+        try:
+            parts.append(p.decode("utf-8").encode("utf-8"))
+            continue
+        except UnicodeDecodeError:
+            pass
+        text = p.decode("utf-8", "replace")
+        replaced[i] = text.count("\ufffd") - p.count("\ufffd".encode("utf-8"))
+        parts.append(text.encode("utf-8"))
+    out_offs = np.zeros(n + 1, dtype=np.uint64)
+    if n:
+        out_offs[1:] = np.cumsum([len(x) for x in parts], dtype=np.uint64)
+    return np.frombuffer(b"".join(parts) + b"\0", dtype=np.uint8)[:int(out_offs[-1])].copy(), out_offs, replaced
 
 
 @dataclass
@@ -320,6 +359,21 @@ class TokenizerPluginClient:
 
     def decode_batch(self, ctx: SecurityContext, req: "DecodeBatchRequest") -> "DecodeBatchResponse":
         raise NotImplementedError
+
+    def encode_batch_lossy(self, ctx: SecurityContext, req: EncodeBatchRequest) -> EncodeBatchResponse:
+        """encode_batch of a request with errors="replace": every prompt encoded as bytes.decode("utf-8", "replace") would be, and
+        EncodeBatchResponse.replaced.  This default works on any plugin: it repairs every prompt on the host (repair_utf8) and
+        encodes the repaired batch strictly."""
+        _errors(req)
+        data, offs, replaced = repair_utf8(req.bytes, req.offsets)
+        r = self.encode_batch(ctx, EncodeBatchRequest(req.vocab, data, offs, req.vocabs_per_prompt, req.vocab_index))
+        return EncodeBatchResponse(r.ids, r.offsets, r.counts, replaced=replaced)
+
+    def count_tokens_lossy(self, ctx: SecurityContext, req: CountTokensRequest) -> np.ndarray:
+        """count_tokens of a request with errors="replace"; this default repairs on the host, as encode_batch_lossy"""
+        _errors(req)
+        data, offs, _ = repair_utf8(req.bytes, req.offsets)
+        return self.count_tokens(ctx, CountTokensRequest(req.vocab, data, offs, req.vocabs_per_prompt, req.vocab_index))
 
     def encode_batch_special(self, ctx: SecurityContext, req: EncodeBatchRequest, special_tokens: dict, allowed: set,
                              disallowed: set) -> EncodeBatchResponse:
@@ -562,6 +616,8 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
 
     # -- TokenizerPluginClient
     def encode_batch(self, ctx: SecurityContext, req: EncodeBatchRequest, out: Optional[EncodeBatchResponse] = None) -> EncodeBatchResponse:
+        if _errors(req) == "replace":
+            return self.encode_batch_lossy(ctx, req, out)
         self._check_arrays(req)
         vid = self._vocab_ids(req)
         unit = STARTS_UNITS[_starts_unit(req.starts_unit)]
@@ -594,10 +650,35 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
                                                          with_starts=True, starts_unit=req.starts_unit))
 
     def count_tokens(self, ctx: SecurityContext, req: CountTokensRequest, out_counts: Optional[np.ndarray] = None) -> np.ndarray:
+        if _errors(req) == "replace":
+            return self.count_tokens_lossy(ctx, req, out_counts)
         self._check_arrays(req)
         vid = self._vocab_ids(req)
         try:
             return self.ctx.count_batch(req.bytes, req.offsets, vid, out_counts)
+        except N.NativeError as e:
+            raise _map_native(e) from e
+
+    def encode_batch_lossy(self, ctx: SecurityContext, req: EncodeBatchRequest, out: Optional[EncodeBatchResponse] = None) -> EncodeBatchResponse:
+        """the device path (cfbpe_encode_batch_lossy): the bytes are checked, and repaired when they must be, on the device"""
+        _errors(req)
+        self._check_arrays(req)
+        vid = self._vocab_ids(req)
+        try:
+            ids, offs, counts, replaced = self.ctx.encode_batch_lossy(
+                req.bytes, req.offsets, vid, None if out is None else out.ids, None if out is None else out.offsets,
+                None if out is None else out.counts, None if out is None else out.replaced)
+        except N.NativeError as e:
+            raise _map_native(e) from e
+        return EncodeBatchResponse(ids, offs, counts, replaced=replaced)
+
+    def count_tokens_lossy(self, ctx: SecurityContext, req: CountTokensRequest, out_counts: Optional[np.ndarray] = None) -> np.ndarray:
+        """the device path (cfbpe_encode_batch_lossy without ids)"""
+        _errors(req)
+        self._check_arrays(req)
+        vid = self._vocab_ids(req)
+        try:
+            return self.ctx.encode_batch_lossy(req.bytes, req.offsets, vid, out_counts=out_counts, counts_only=True)[2]
         except N.NativeError as e:
             raise _map_native(e) from e
 

@@ -32,6 +32,7 @@ static inline void prof_mark(ProfEvents* p, int idx, cudaStream_t s, bool begin)
 #include "specials.cuh"
 #include "subbatch.h"
 #include "unicode_tables.h"
+#include "utf8_repair.cuh"
 #include "vocab.h"
 
 using namespace cfbpe;
@@ -103,6 +104,15 @@ struct LaneSpecial {
     HostPtr<SpecialStatus> h_status;      // pinned
 };
 
+// the buffers of lossy calls (cfbpe_encode_batch_lossy*), allocated on the lane's first such call, all or none: a context that never
+// makes one keeps the footprint it had
+struct LaneLossy {
+    DevPtr<uint64_t> offsets;             // [max_prompts + 1] the prompts' offsets in the repaired batch
+    DevPtr<uint32_t> replaced;            // [max_prompts] U+FFFD inserted per prompt
+    DevPtr<LossyStatus> status;
+    HostPtr<LossyStatus> h_status;        // pinned
+};
+
 struct Lane {
     std::mutex mu;                        // held for the duration of a call
     int device = 0;
@@ -155,6 +165,7 @@ struct Lane {
     HostPtr<DeviceStatus> h_status;      // pinned
     ProfEvents prof{};
     LaneSpecial sp;
+    LaneLossy lossy;
 
     ~Lane() {                            // the members' deleters run after this body, on the lane's device
         cudaSetDevice(device);
@@ -830,14 +841,20 @@ __global__ void rebase_offsets_kernel(uint64_t* __restrict__ offsets, uint64_t n
 int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
                      const uint8_t* const* modes, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids,
                      uint64_t total, uint32_t* out_bad, uint64_t* defer);
+int run_lane_lossy(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                   uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
+                   uint32_t* out_replaced, uint64_t* defer);
 
 // special != nullptr: a special-token call (cfbpe_encode_batch_special): every shard runs its own special pass; special->modes
 // are the call's modes, special->bad gets the prompt and special index of a CFBPE_EBADMSG
 struct SpecialArgs { const uint8_t* const* modes; uint32_t* bad; };
+// lossy != nullptr: a lossy call (cfbpe_encode_batch_lossy): every shard runs its own scan and, when it needs one, its own repair;
+// lossy->replaced (nullable) gets every prompt's U+FFFD count
+struct LossyArgs { uint32_t* replaced; };
 int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
                      uint32_t* out_ids, uint32_t* out_starts, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
                      const SpecialArgs* special = nullptr, const TruncateArgs* trunc = nullptr, const ChunkArgs* chunk = nullptr,
-                     const UnitArgs* unit = nullptr) {
+                     const UnitArgs* unit = nullptr, const LossyArgs* lossy = nullptr) {
     const uint32_t G = static_cast<uint32_t>(ctx->devs.size());
     std::vector<uint32_t> lo(G + 1, 0);
     for (uint32_t d = 1; d < G; ++d) {      // first prompt whose start is >= d * total / G
@@ -866,6 +883,10 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
             if (special) {
                 s.rc = run_lane_special(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
                                         special->modes, nullptr, 0, nullptr, nullptr, want_ids, s.local_offs[nd], s.bad, &s.tokens);
+                s.cut[0] = 0; s.cut[1] = nd; s.nc = 1;
+            } else if (lossy) {
+                s.rc = run_lane_lossy(ctx, ctx->devs[d].get(), locks[d]->ln, nd, bytes + o0, s.local_offs.data(), vocab_ids ? vocab_ids + p0 : nullptr,
+                                      nullptr, 0, nullptr, nullptr, want_ids, s.local_offs[nd], nullptr, &s.tokens);
                 s.cut[0] = 0; s.cut[1] = nd; s.nc = 1;
             } else {
                 const TruncateArgs shard_trunc = trunc ? truncate_from(*trunc, p0) : TruncateArgs{};
@@ -925,6 +946,7 @@ int run_multi_device(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
                 rebase_offsets_kernel<<<static_cast<unsigned>((cnt + 255) / 256), 256, 0, st>>>(src, cnt, ln->d_totals.get(), d);
                 if (out_offsets) ck(cudaMemcpyAsync(out_offsets + p0 + q0, src, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st), "offsets download");
                 if (out_counts && nk) ck(cudaMemcpyAsync(out_counts + p0 + q0, ln->d_out_counts.get() + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "counts download");
+                if (lossy && lossy->replaced && nk) ck(cudaMemcpyAsync(lossy->replaced + p0 + q0, ln->lossy.replaced.get() + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "replaced download");
                 if (unit && unit->lens && nk) ck(cudaMemcpyAsync(unit->lens + p0 + q0, ln->d_unit_lens.get() + q0, static_cast<uint64_t>(nk) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "lengths download");
                 if (chunk) {      // chunk offsets: rebased as the token offsets, by the chunk totals of the shards before; spans: prompt-relative
                     uint64_t* csrc = ln->d_chunk_offs.get() + sub_batch_offsets_at(q0, k);
@@ -1067,6 +1089,109 @@ int run_host_special(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uin
     DeviceCtx* dv = ctx->devs[0].get();
     LaneLock lk(dv);
     return run_lane_special(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, modes, out_ids, out_cap, out_offsets, out_counts, want_ids, total, out_bad, nullptr);
+}
+
+// ---------------------------------------------------------------------------------------
+// bytes that are not valid UTF-8 (utf8_repair.cuh)
+// ---------------------------------------------------------------------------------------
+// the lane's lossy buffers, all or none (as ensure_special_lane).  The caller has selected the lane's device.
+int ensure_lossy_lane(cfbpe_ctx* ctx, Lane* ln) {
+    if (ln->lossy.h_status) return CFBPE_OK;
+    const uint64_t mp = ctx->max_prompts;
+    LaneLossy lz;
+    bool ok = dmalloc(lz.offsets, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(lz.replaced, mp + 1) == cudaSuccess;
+    ok = ok && dmalloc(lz.status, 1) == cudaSuccess;
+    ok = ok && hmalloc(lz.h_status, 1) == cudaSuccess;
+    if (!ok) { cudaGetLastError(); return fail(ctx, CFBPE_ENOMEM, "no device memory for the lossy-call buffers"); }
+    ln->lossy = std::move(lz);
+    return CFBPE_OK;
+}
+
+// The rest of a lossy call once its batch is on the device: the scan, the one synchronisation of the call (the host needs the
+// scan's verdict and the repaired size for the launch geometry), then the ordinary path into `out` on the bytes as they are (no
+// invalid byte) or on the repaired batch, which goes to the lane's byte buffer.  When b.bytes IS that buffer (a host call), the
+// bytes are first copied to ids_by_pos (4 bytes a byte, dead until the ordinary pass starts).  The prompts' U+FFFD counts are left
+// in the lane's replaced buffer.  A repaired batch over max_batch_bytes fails with CFBPE_EINVAL before anything is written to `out`.
+int enqueue_lossy_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, const EncodeOut& out) {
+    const LossyWork lw{ln->lossy.replaced.get(), ln->lossy.offsets.get(), ln->lossy.status.get()};
+    enqueue_utf8_scan(b, dv->vs, ln->ws, lw, s);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(ln->lossy.h_status.get(), lw.status, sizeof(LossyStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    const LossyScanResult r = lossy_scan_result(*ln->lossy.h_status, b.total_bytes);
+    BatchView eb = b;
+    if (r.dirty) {
+        if (r.total > ctx->max_bytes)
+            return fail(ctx, CFBPE_EINVAL, "the repaired batch (" + std::to_string(r.total) + " bytes) exceeds max_batch_bytes of this context");
+        BatchView raw = b;
+        if (b.bytes == ln->d_bytes.get()) {
+            uint8_t* stage = reinterpret_cast<uint8_t*>(ln->ws.ids_by_pos);
+            CK(cudaMemcpyAsync(stage, b.bytes, b.total_bytes, cudaMemcpyDeviceToDevice, s));
+            raw.bytes = stage;
+        }
+        enqueue_utf8_repair(raw, ln->ws, lw, ln->d_bytes.get(), r.total, s);
+        eb = BatchView{ln->d_bytes.get(), lw.offsets, b.vocab_ids, b.n_prompts, r.total};
+    }
+    enqueue_encode(eb, dv->vs, dv->uc, ln->ws, out.ids, out.cap, out.offsets, out.counts, static_cast<uint32_t>(dv->sm_count * 4),
+                   s, ln->aux_stream.get(), ln->aux2_stream.get(), ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), static_cast<ProfEvents*>(nullptr));
+    CK(cudaGetLastError());
+    return CFBPE_OK;
+}
+
+// A lossy host call on one lane (the whole call on a single-device context, one shard of a multi-device one), as one pass: upload,
+// scan, the ordinary path on the prompts as they are or repaired, download.  defer: see run_lane (the ids, offsets and counts are
+// left in the lane's d_out_* buffers, the U+FFFD counts in its replaced buffer).
+int run_lane_lossy(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                   uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, bool want_ids, uint64_t total,
+                   uint32_t* out_replaced, uint64_t* defer) {
+    CK(cudaSetDevice(dv->device));
+    int rc = wait_for_device_call(ctx, ln);
+    if (!rc) rc = ensure_lossy_lane(ctx, ln);
+    if (rc) return rc;
+    cudaStream_t s = ln->stream.get();
+    BatchView b;
+    if ((rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b))) return rc;
+    const EncodeOut out{want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get(), ln->d_out_counts.get()};
+    if ((rc = enqueue_lossy_call(ctx, dv, ln, b, s, out))) return rc;
+    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    if (!defer) {
+        if (out_offsets) CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets.get(), (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+        if (out_counts && n) CK(cudaMemcpyAsync(out_counts, ln->d_out_counts.get(), static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        if (out_replaced && n) CK(cudaMemcpyAsync(out_replaced, ln->lossy.replaced.get(), static_cast<uint64_t>(n) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaStreamSynchronize(s));
+    const DeviceStatus st = *ln->h_status;
+    if ((rc = fail_status(ctx, st))) return rc;
+    if (defer) { *defer = st.n_tokens; return CFBPE_OK; }
+    if (want_ids && st.n_tokens > out_cap) return fail_nospace(ctx, st.n_tokens, out_offsets, n);
+    if (want_ids && st.n_tokens) {
+        CK(cudaMemcpyAsync(out_ids, ln->d_out_ids.get(), st.n_tokens * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+    }
+    return CFBPE_OK;
+}
+
+// shared body of the lossy host call
+int run_host_lossy(cfbpe_ctx* ctx, uint32_t n, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids, uint32_t* out_ids,
+                   uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, uint32_t* out_replaced) {
+    tl_err.clear();
+    std::shared_lock<std::shared_mutex> vocabs(ctx->vocab_mu);
+    uint64_t total = 0;
+    int rc = validate_batch(ctx, n, offsets, vocab_ids, &total);
+    if (rc) return rc;
+    const bool want_ids = out_ids != nullptr;
+    if (total && !bytes) return fail(ctx, CFBPE_EINVAL, "bytes is NULL");
+    if (!out_offsets) return fail(ctx, CFBPE_EINVAL, "out_offsets is NULL");
+    if (ctx->devs.size() > 1 && n >= ctx->devs.size()) {    // one contiguous shard a device, each with its own scan and repair
+        const LossyArgs la{out_replaced};
+        return run_multi_device(ctx, n, bytes, offsets, vocab_ids, out_ids, nullptr, out_cap, out_offsets, out_counts, want_ids, total, nullptr,
+                                nullptr, nullptr, nullptr, &la);
+    }
+    if (total > ctx->max_bytes) return fail(ctx, CFBPE_EINVAL, "batch exceeds max_batch_bytes of this context");
+    DeviceCtx* dv = ctx->devs[0].get();
+    LaneLock lk(dv);
+    return run_lane_lossy(ctx, dv, lk.ln, n, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, want_ids, total, out_replaced, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1268,6 +1393,21 @@ int run_device_special(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_byte
         if (!rc) rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, out, out, out_bad, &spliced);
         // the lane's status carries the call's id count (cfbpe_device_status checks it against out_cap): n_tokens and tok_end
         if (!rc && spliced) CK(cudaMemcpyAsync(&ln->ws.status->n_tokens, &ln->sp.status->fin.n_tokens, 2 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
+        return rc;
+    });
+}
+
+// shared body of encode_batch_lossy_device: the repaired batch (when one is needed) goes to the lane's byte buffer; the U+FFFD counts
+// are copied to d_out_replaced once the repaired size is known to fit
+int run_device_lossy(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                     const uint8_t* d_vocab_ids, uint32_t* d_out_ids, uint64_t out_cap, uint64_t* d_out_offsets, uint32_t* d_out_counts,
+                     uint32_t* d_out_replaced, uint64_t* n_tokens, void* stream) {
+    return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_offsets, d_out_ids != nullptr, out_cap, n_tokens, stream, false,
+                       [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents*) {
+        int rc = ensure_lossy_lane(ctx, ln);
+        if (!rc) rc = enqueue_lossy_call(ctx, dv, ln, b, s, EncodeOut{d_out_ids, out_cap, d_out_offsets, d_out_counts});
+        if (!rc && d_out_replaced && n_prompts)
+            CK(cudaMemcpyAsync(d_out_replaced, ln->lossy.replaced.get(), static_cast<uint64_t>(n_prompts) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
         return rc;
     });
 }
@@ -1673,6 +1813,23 @@ int cfbpe_encode_batch_special_device(cfbpe_ctx* ctx, uint32_t n_prompts, const 
     tl_err.clear();
     return run_device_special(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, modes, d_out_ids, out_cap, d_out_offsets, d_out_counts,
                               n_tokens, out_bad, stream);
+}
+
+int cfbpe_encode_batch_lossy(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* bytes, const uint64_t* offsets, const uint8_t* vocab_ids,
+                             uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts, uint32_t* out_replaced) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    return run_host_lossy(ctx, n_prompts, bytes, offsets, vocab_ids, out_ids, out_cap, out_offsets, out_counts, out_replaced);
+}
+
+int cfbpe_encode_batch_lossy_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint64_t total_bytes, const uint64_t* d_offsets,
+                                    const uint8_t* d_vocab_ids, uint32_t* d_out_ids, uint64_t out_cap, uint64_t* d_out_offsets,
+                                    uint32_t* d_out_counts, uint32_t* d_out_replaced, uint64_t* n_tokens, void* stream) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    return run_device_lossy(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_ids, out_cap, d_out_offsets, d_out_counts,
+                            d_out_replaced, n_tokens, stream);
 }
 
 int cfbpe_device_status(cfbpe_ctx* ctx, void* stream) {

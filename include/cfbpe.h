@@ -328,6 +328,38 @@ CFBPE_API int cfbpe_chunk_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, const
                                        const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t chunk_tokens,
                                        uint32_t overlap_tokens, uint32_t *d_out_spans, uint64_t chunk_cap,
                                        uint64_t *d_out_chunk_offsets, uint32_t *d_out_counts, uint64_t *n_chunks, void *stream);
+/* Encode as if every prompt had first been decoded with Python's bytes.decode("utf-8", errors="replace") and encoded again as
+ * UTF-8.  For prompt p with bytes b and R(b) = b.decode("utf-8", "replace").encode("utf-8"):
+ *   ids, offsets, counts  those of cfbpe_encode_batch on R(b) for every prompt: tiktoken 0.12.0
+ *                         encode_ordinary(b.decode("utf-8", "replace")).  A prompt of valid UTF-8 gets exactly its
+ *                         cfbpe_encode_batch ids.
+ *   out_replaced[p]       the number of U+FFFD the decode inserted into prompt p (a U+FFFD that was already in the text does not
+ *                         count; 0: the prompt is valid UTF-8).  n_prompts entries, may be NULL.  A strict caller can refuse just
+ *                         the prompts with out_replaced[p] > 0.
+ * The replacement rule is CPython's, the Unicode Standard's "substitution of maximal subparts" (chapter 3), which
+ * String::from_utf8_lossy and the WHATWG decoder follow too: each maximal subpart of an ill-formed sequence becomes one U+FFFD
+ * (F0 9F 98 -> 1, ED A0 80 -> 3, C0 AF -> 2, F4 90 80 80 -> 4, F0 9F 98 61 -> U+FFFD "a").  A sequence never spans two prompts:
+ * a lead byte that ends prompt i is a subpart of its own, and the continuation bytes that open prompt i + 1 are strays.
+ * out_ids == NULL: counts and offsets only.  Other arguments and CFBPE_ENOSPC (out_offsets[n_prompts] = ids needed) as
+ * cfbpe_encode_batch.  The call never returns CFBPE_EILSEQ.  The repaired batch is up to 3 times the input: when a device's
+ * share of it exceeds max_batch_bytes the call returns CFBPE_EINVAL (the message gives the repaired size) and writes no output.
+ * A host call runs as one pass on its lane, or as one contiguous shard of whole prompts a device on a multi-device context (not
+ * pipelined, and not spread round-robin like cfbpe_encode_batch).  Costs: a scan over the bytes and one synchronisation before the
+ * ordinary path; when some byte is not valid UTF-8, the repaired copy is written first (the ordinary path then runs on it).
+ * 12 bytes of device memory per prompt of max_prompts on each lane that runs such a call, allocated on its first one
+ * (CFBPE_ENOMEM if that fails). */
+CFBPE_API int cfbpe_encode_batch_lossy(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *bytes, const uint64_t *offsets,
+                                       const uint8_t *vocab_ids, uint32_t *out_ids, uint64_t out_cap, uint64_t *out_offsets,
+                                       uint32_t *out_counts, uint32_t *out_replaced);
+/* The same on device-resident buffers, as cfbpe_encode_batch_device (d_bytes readable for 32 bytes past total_bytes, whose
+ * contents do not matter); d_out_replaced (n_prompts entries, may be NULL) is device memory.  The call synchronises `stream` once,
+ * after the scan: the host needs its verdict and the repaired size to choose the launch geometry.  The rest is enqueued
+ * asynchronously as in cfbpe_encode_batch_device (n_tokens == NULL: nothing more is waited for).  The repaired batch is written to
+ * the library's own buffers; the caller's bytes are only read. */
+CFBPE_API int cfbpe_encode_batch_lossy_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
+                                              const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t *d_out_ids,
+                                              uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
+                                              uint32_t *d_out_replaced, uint64_t *n_tokens, void *stream);
 /* Synchronise `stream` and return the status word of the last device call (0, CFBPE_EILSEQ, CFBPE_ENOSPC). */
 CFBPE_API int cfbpe_device_status(cfbpe_ctx *ctx, void *stream);
 

@@ -122,6 +122,11 @@ extern "C" {
                                              d_vocab_ids: *const u8, modes: *const *const u8, d_out_ids: *mut u32, out_cap: u64,
                                              d_out_offsets: *mut u64, d_out_counts: *mut u32, n_tokens: *mut u64, out_bad: *mut u32,
                                              stream: *mut c_void) -> c_int;
+    pub fn cfbpe_encode_batch_lossy(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64, vocab_ids: *const u8,
+                                    out_ids: *mut u32, out_cap: u64, out_offsets: *mut u64, out_counts: *mut u32, out_replaced: *mut u32) -> c_int;
+    pub fn cfbpe_encode_batch_lossy_device(ctx: *mut cfbpe_ctx, n_prompts: u32, d_bytes: *const u8, total_bytes: u64, d_offsets: *const u64,
+                                           d_vocab_ids: *const u8, d_out_ids: *mut u32, out_cap: u64, d_out_offsets: *mut u64,
+                                           d_out_counts: *mut u32, d_out_replaced: *mut u32, n_tokens: *mut u64, stream: *mut c_void) -> c_int;
     pub fn cfbpe_device_status(ctx: *mut cfbpe_ctx, stream: *mut c_void) -> c_int;
     pub fn cfbpe_host_alloc(ctx: *mut cfbpe_ctx, size: usize) -> *mut c_void;
     pub fn cfbpe_host_free(ctx: *mut cfbpe_ctx, ptr: *mut c_void);
@@ -344,6 +349,43 @@ impl Ctx {
         out.ids.truncate(out.offsets[n as usize] as usize);
         out.counts.truncate(n as usize);
         Ok(out)
+    }
+
+    /// Encode every prompt as `String::from_utf8_lossy` (Python's `decode("utf-8", "replace")`) would have it: each maximal
+    /// subpart of an ill-formed sequence becomes one U+FFFD, on the device.  Returns the encoding of the repaired text and the
+    /// U+FFFD inserted into every prompt (0: the prompt is valid UTF-8).  Never fails with `CFBPE_EILSEQ`.
+    pub fn encode_batch_lossy(&self, bytes: &[u8], offsets: &[u64], vocab_ids: Option<&[u8]>) -> Result<(Encoded, Vec<u32>), NativeError> {
+        let n = Self::check_inputs(bytes.len(), offsets, vocab_ids)?;
+        let total = offsets[n as usize] as usize;
+        let mut out = Encoded { ids: vec![0; (3 * total).max(1)], offsets: vec![0; n as usize + 1], counts: vec![0; (n as usize).max(1)] };
+        let mut replaced = vec![0u32; (n as usize).max(1)];
+        // SAFETY: as encode_batch; out.ids holds out_cap ids (the repaired text has at most 3 bytes a byte, and an id covers >= 1
+        // byte), replaced one entry per prompt.
+        let rc = unsafe {
+            cfbpe_encode_batch_lossy(self.0.as_ptr(), n, bytes.as_ptr(), offsets.as_ptr(), vocab_ids.map_or(std::ptr::null(), <[u8]>::as_ptr),
+                                     out.ids.as_mut_ptr(), out.ids.len() as u64, out.offsets.as_mut_ptr(), out.counts.as_mut_ptr(),
+                                     replaced.as_mut_ptr())
+        };
+        self.check(rc)?;
+        out.ids.truncate(out.offsets[n as usize] as usize);
+        out.counts.truncate(n as usize);
+        replaced.truncate(n as usize);
+        Ok((out, replaced))
+    }
+
+    /// `count_batch` of the text `encode_batch_lossy` encodes: only the counts leave the device.
+    pub fn count_batch_lossy(&self, bytes: &[u8], offsets: &[u64], vocab_ids: Option<&[u8]>) -> Result<Vec<u32>, NativeError> {
+        let n = Self::check_inputs(bytes.len(), offsets, vocab_ids)?;
+        let mut out_offsets = vec![0u64; n as usize + 1];
+        let mut counts = vec![0u32; (n as usize).max(1)];
+        // SAFETY: as above; out_ids NULL asks for counts and offsets only.
+        let rc = unsafe {
+            cfbpe_encode_batch_lossy(self.0.as_ptr(), n, bytes.as_ptr(), offsets.as_ptr(), vocab_ids.map_or(std::ptr::null(), <[u8]>::as_ptr),
+                                     std::ptr::null_mut(), 0, out_offsets.as_mut_ptr(), counts.as_mut_ptr(), std::ptr::null_mut())
+        };
+        self.check(rc)?;
+        counts.truncate(n as usize);
+        Ok(counts)
     }
 
     /// `usage::count_tokens`: only the per-prompt counts leave the device.

@@ -6,7 +6,7 @@ use std::sync::Arc;
 use async_trait::async_trait;
 use cfbpe_sys::{Ctx, NativeError};
 use llm_gateway_sdk::{
-    ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, OffsetUnit, SpecialTokens,
+    ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, InvalidUtf8, OffsetUnit, SpecialTokens,
     TokenizerError, TokenizerPluginClient, TruncateBatchResponse, TruncateKeep, VocabRef,
 };
 use modkit_security::SecurityContext;
@@ -104,7 +104,10 @@ impl Service {
 
 #[async_trait]
 impl TokenizerPluginClient for Service {
-    async fn encode_batch(&self, _ctx: &SecurityContext, req: EncodeBatchRequest) -> Result<EncodeBatchResponse, TokenizerError> {
+    async fn encode_batch(&self, ctx: &SecurityContext, req: EncodeBatchRequest) -> Result<EncodeBatchResponse, TokenizerError> {
+        if req.invalid_utf8 == InvalidUtf8::Replace {
+            return self.encode_batch_lossy(ctx, req).await;
+        }
         let n = req.offsets.len().saturating_sub(1);
         let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
         let native = self.native.clone();
@@ -124,7 +127,33 @@ impl TokenizerPluginClient for Service {
             .await
             .map_err(|e| TokenizerError::Internal(e.to_string()))?
             .map_err(map_native)?;
-        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts, lens })
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts, lens, replaced: None })
+    }
+
+    /// The device path (`cfbpe_encode_batch_lossy`): the bytes are checked, and repaired where they must be, on the device.
+    async fn encode_batch_lossy(&self, _ctx: &SecurityContext, req: EncodeBatchRequest) -> Result<EncodeBatchResponse, TokenizerError> {
+        if req.with_starts {
+            return Err(TokenizerError::InvalidInput("InvalidUtf8::Replace returns no starts: they would index the repaired text".to_owned()));
+        }
+        let n = req.offsets.len().saturating_sub(1);
+        let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
+        let native = self.native.clone();
+        let (out, replaced) = tokio::task::spawn_blocking(move || native.encode_batch_lossy(&req.bytes, &req.offsets, vid.as_deref()))
+            .await
+            .map_err(|e| TokenizerError::Internal(e.to_string()))?
+            .map_err(map_native)?;
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts: None, lens: None, replaced: Some(replaced) })
+    }
+
+    /// The device path (`cfbpe_encode_batch_lossy` without ids); such requests do not ride in the shared count batches.
+    async fn count_tokens_lossy(&self, _ctx: &SecurityContext, req: CountTokensRequest) -> Result<Vec<u32>, TokenizerError> {
+        let n = req.offsets.len().saturating_sub(1);
+        let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
+        let native = self.native.clone();
+        tokio::task::spawn_blocking(move || native.count_batch_lossy(&req.bytes, &req.offsets, vid.as_deref()))
+            .await
+            .map_err(|e| TokenizerError::Internal(e.to_string()))?
+            .map_err(map_native)
     }
 
     /// The device path (`cfbpe_encode_batch_char_starts`): the unit starts are computed where the ids and byte starts are.
@@ -132,7 +161,10 @@ impl TokenizerPluginClient for Service {
         self.encode_batch(ctx, EncodeBatchRequest { with_starts: true, ..req }).await
     }
 
-    async fn count_tokens(&self, _ctx: &SecurityContext, req: CountTokensRequest) -> Result<Vec<u32>, TokenizerError> {
+    async fn count_tokens(&self, ctx: &SecurityContext, req: CountTokensRequest) -> Result<Vec<u32>, TokenizerError> {
+        if req.invalid_utf8 == InvalidUtf8::Replace {
+            return self.count_tokens_lossy(ctx, req).await;
+        }
         let n = req.offsets.len().saturating_sub(1);
         let vid = self.vocab_ids(&req.vocab, req.vocabs_per_prompt.as_deref(), req.vocab_index.as_deref(), n)?;
         // small requests (a chat message is a few KB) ride in a shared device batch; large ones go straight through
@@ -221,7 +253,7 @@ impl TokenizerPluginClient for Service {
         .await
         .map_err(|e| TokenizerError::Internal(e.to_string()))?
         .map_err(map_native)?;
-        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts: None, lens: None })
+        Ok(EncodeBatchResponse { ids: out.ids, offsets: out.offsets, counts: out.counts, starts: None, lens: None, replaced: None })
     }
 }
 

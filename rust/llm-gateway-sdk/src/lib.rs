@@ -19,7 +19,7 @@ pub use api::TokenizerClient;
 pub use error::TokenizerError;
 pub use gts::TokenizerPluginSpecV1;
 pub use models::{
-    chunk_spans, truncate_cut, unit_starts, ChatTemplate, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, OffsetUnit, SpecialTokens,
+    chunk_spans, truncate_cut, unit_starts, ChatTemplate, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse, InvalidUtf8, OffsetUnit, SpecialTokens,
     TruncateBatchResponse, TruncateKeep, Usage, VocabRef,
 };
-pub use plugin_api::TokenizerPluginClient;
+pub use plugin_api::{repair_utf8, TokenizerPluginClient};

@@ -30,6 +30,21 @@ pub struct EncodeBatchRequest {
     /// with `with_starts`: the unit of the starts (`OffsetUnit::Byte` for byte offsets; a character unit also fills
     /// `EncodeBatchResponse::lens`)
     pub starts_unit: OffsetUnit,
+    /// bytes that are not valid UTF-8: `Reject` fails the request, `Replace` encodes every prompt as `String::from_utf8_lossy`
+    /// would have it and fills `EncodeBatchResponse::replaced` (not with `with_starts`)
+    pub invalid_utf8: InvalidUtf8,
+}
+
+/// What a request does with bytes that are not valid UTF-8 (`include/cfbpe.h`, `cfbpe_encode_batch_lossy`).
+#[derive(Debug, Clone, Copy, PartialEq, Eq, Default, Serialize, Deserialize, schemars::JsonSchema)]
+#[serde(rename_all = "lowercase")]
+pub enum InvalidUtf8 {
+    /// fail the request (tiktoken only accepts valid text)
+    #[default]
+    Reject,
+    /// replace each maximal subpart of an ill-formed sequence with U+FFFD (`String::from_utf8_lossy`, Python's
+    /// `decode("utf-8", "replace")`, the WHATWG decoder)
+    Replace,
 }
 
 #[derive(Debug, Clone, Default, Serialize, Deserialize)]
@@ -46,6 +61,9 @@ pub struct EncodeBatchResponse {
     /// with a character `starts_unit`: every prompt's length in that unit (closes the last token's span)
     #[serde(default, skip_serializing_if = "Option::is_none")]
     pub lens: Option<Vec<u32>>,
+    /// with `InvalidUtf8::Replace`: every prompt's U+FFFD inserted by the repair (0: valid UTF-8)
+    #[serde(default, skip_serializing_if = "Option::is_none")]
+    pub replaced: Option<Vec<u32>>,
 }
 
 /// What a token start counts (`include/cfbpe.h`, `cfbpe_encode_batch_char_starts`).
@@ -168,6 +186,8 @@ pub struct CountTokensRequest {
     pub offsets: Vec<u64>,
     pub vocabs_per_prompt: Option<Vec<VocabRef>>,
     pub vocab_index: Option<Vec<u8>>,
+    /// as `EncodeBatchRequest::invalid_utf8`
+    pub invalid_utf8: InvalidUtf8,
 }
 
 #[derive(Debug, Clone)]

@@ -5,7 +5,7 @@ use modkit_security::SecurityContext;
 
 use crate::error::TokenizerError;
 use crate::models::{chunk_spans, truncate_cut, unit_starts, ChunkBatchResponse, CountTokensRequest, DecodeBatchRequest, DecodeBatchResponse, EncodeBatchRequest, EncodeBatchResponse,
-                    OffsetUnit, SpecialTokens, TruncateBatchResponse, TruncateKeep, VocabRef};
+                    InvalidUtf8, OffsetUnit, SpecialTokens, TruncateBatchResponse, TruncateKeep, VocabRef};
 
 /// Each plugin registers this trait with a scoped `ClientHub` entry using its GTS instance id as the scope.  Clients are
 /// `Arc<dyn … + Send + Sync>` shared by all tokio tasks (`libs/modkit/src/client_hub.rs:142-165`): calls are concurrent and
@@ -70,6 +70,26 @@ pub trait TokenizerPluginClient: Send + Sync {
             out.chunk_offsets.push(out.spans.len() as u64);
         }
         Ok(out)
+    }
+
+    /// `encode_batch` of a request with `InvalidUtf8::Replace`: every prompt encoded as `String::from_utf8_lossy` would have it,
+    /// and `EncodeBatchResponse::replaced` -- `include/cfbpe.h`, `cfbpe_encode_batch_lossy`.  The default works on any plugin: it
+    /// repairs every prompt on the host and sends the repaired batch through one strict `encode_batch`.
+    /// `gpu-bpe-tokenizer-plugin` overrides it with the device call.
+    async fn encode_batch_lossy(&self, ctx: &SecurityContext, req: EncodeBatchRequest) -> Result<EncodeBatchResponse, TokenizerError> {
+        if req.with_starts {
+            return Err(TokenizerError::InvalidInput("InvalidUtf8::Replace returns no starts: they would index the repaired text".to_owned()));
+        }
+        let (bytes, offsets, replaced) = repair_utf8(&req.bytes, &req.offsets);
+        let mut enc = self.encode_batch(ctx, EncodeBatchRequest { bytes: bytes.into(), offsets, invalid_utf8: InvalidUtf8::Reject, ..req }).await?;
+        enc.replaced = Some(replaced);
+        Ok(enc)
+    }
+
+    /// `count_tokens` of a request with `InvalidUtf8::Replace`; this default repairs on the host, as `encode_batch_lossy`.
+    async fn count_tokens_lossy(&self, ctx: &SecurityContext, req: CountTokensRequest) -> Result<Vec<u32>, TokenizerError> {
+        let (bytes, offsets, _) = repair_utf8(&req.bytes, &req.offsets);
+        self.count_tokens(ctx, CountTokensRequest { bytes: bytes.into(), offsets, invalid_utf8: InvalidUtf8::Reject, ..req }).await
     }
 
     /// `encode_batch` with every token's start in `req.starts_unit` and, for a character unit, every prompt's length in it
@@ -141,14 +161,14 @@ pub trait TokenizerPluginClient: Send + Sync {
             plan.push(steps);
         }
         let enc = if stretches.is_empty() {
-            EncodeBatchResponse { ids: Vec::new(), offsets: vec![0], counts: Vec::new(), starts: None, lens: None }
+            EncodeBatchResponse { ids: Vec::new(), offsets: vec![0], counts: Vec::new(), starts: None, lens: None, replaced: None }
         } else {
             let mut bytes = Vec::new();
             let mut offsets = vec![0u64];
             for s in &stretches { bytes.extend_from_slice(s.as_bytes()); offsets.push(bytes.len() as u64); }
-            self.encode_batch(ctx, EncodeBatchRequest { vocab: req.vocab.clone(), bytes: bytes.into(), offsets, vocabs_per_prompt: per.take(), vocab_index: None, with_starts: false, starts_unit: OffsetUnit::Byte }).await?
+            self.encode_batch(ctx, EncodeBatchRequest { vocab: req.vocab.clone(), bytes: bytes.into(), offsets, vocabs_per_prompt: per.take(), vocab_index: None, with_starts: false, starts_unit: OffsetUnit::Byte, invalid_utf8: InvalidUtf8::Reject }).await?
         };
-        let mut out = EncodeBatchResponse { ids: Vec::new(), offsets: vec![0u64], counts: Vec::with_capacity(n), starts: None, lens: None };
+        let mut out = EncodeBatchResponse { ids: Vec::new(), offsets: vec![0u64], counts: Vec::with_capacity(n), starts: None, lens: None, replaced: None };
         for steps in plan {
             let start = out.ids.len();
             for s in steps {
@@ -162,4 +182,22 @@ pub trait TokenizerPluginClient: Send + Sync {
         }
         Ok(out)
     }
+}
+
+/// Every prompt of a packed batch as `String::from_utf8_lossy` makes it: `(bytes, offsets, replaced)`, `replaced[i]` the U+FFFD the
+/// repair inserted into prompt `i` (one per maximal subpart of an ill-formed sequence; a U+FFFD already in the text does not count).
+pub fn repair_utf8(bytes: &[u8], offsets: &[u64]) -> (Vec<u8>, Vec<u64>, Vec<u32>) {
+    let n = offsets.len().saturating_sub(1);
+    let (mut out, mut out_offsets, mut replaced) = (Vec::with_capacity(bytes.len()), Vec::with_capacity(n + 1), Vec::with_capacity(n));
+    out_offsets.push(0u64);
+    for i in 0..n {
+        let prompt = &bytes[offsets[i] as usize..offsets[i + 1] as usize];
+        let text = String::from_utf8_lossy(prompt);
+        let had = text.matches('\u{FFFD}').count();
+        let kept = prompt.windows(3).filter(|w| *w == "\u{FFFD}".as_bytes()).count();
+        replaced.push((had - kept) as u32);
+        out.extend_from_slice(text.as_bytes());
+        out_offsets.push(out.len() as u64);
+    }
+    (out, out_offsets, replaced)
 }

@@ -7,7 +7,7 @@ use std::sync::Arc;
 use async_trait::async_trait;
 use bytes::Bytes;
 use llm_gateway_sdk::{
-    ChatTemplate, CountTokensRequest, EncodeBatchRequest, OffsetUnit, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1,
+    ChatTemplate, CountTokensRequest, EncodeBatchRequest, InvalidUtf8, OffsetUnit, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1,
     TruncateKeep, Usage, VocabRef,
 };
 use modkit::client_hub::{ClientHub, ClientScope};
@@ -64,7 +64,7 @@ impl TokenizerService {
         -> Result<Vec<(Vec<String>, Vec<[u32; 2]>, u32)>, TokenizerError> {
         let (bytes, offsets) = pack_texts(texts);
         let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
-                                       starts_unit: OffsetUnit::Byte };
+                                       starts_unit: OffsetUnit::Byte, invalid_utf8: InvalidUtf8::Reject };
         let r = self.plugin().await?.chunk_batch(ctx, req, max_tokens, overlap).await?;
         texts.iter().enumerate().map(|(i, t)| {
             let spans = r.spans[r.chunk_offsets[i] as usize..r.chunk_offsets[i + 1] as usize].to_vec();
@@ -92,7 +92,7 @@ impl TokenizerClient for TokenizerService {
     async fn encode(&self, ctx: &SecurityContext, model: &str, texts: &[String]) -> Result<Vec<Vec<u32>>, TokenizerError> {
         let (bytes, offsets) = pack_texts(texts);
         let r = self.plugin().await?.encode_batch(ctx, EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
-                                       starts_unit: OffsetUnit::Byte }).await?;
+                                       starts_unit: OffsetUnit::Byte, invalid_utf8: InvalidUtf8::Reject }).await?;
         Ok((0..texts.len()).map(|i| r.ids[r.offsets[i] as usize..r.offsets[i + 1] as usize].to_vec()).collect())
     }
 
@@ -100,7 +100,7 @@ impl TokenizerClient for TokenizerService {
         -> Result<Vec<(Vec<u32>, Vec<[u64; 2]>)>, TokenizerError> {
         let (bytes, offsets) = pack_texts(texts);
         let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets: offsets.clone(), vocabs_per_prompt: None, vocab_index: None,
-                                       with_starts: true, starts_unit: unit };
+                                       with_starts: true, starts_unit: unit, invalid_utf8: InvalidUtf8::Reject };
         // a character unit: the plugin does the work (the trait's default converts byte starts on the host, the GPU plugin counts on the device)
         let plugin = self.plugin().await?;
         let r = if unit == OffsetUnit::Byte { plugin.encode_batch(ctx, req).await? } else { plugin.encode_batch_unit_starts(ctx, req).await? };
@@ -126,7 +126,7 @@ impl TokenizerClient for TokenizerService {
         }
         let (bytes, offsets) = pack_texts(texts);
         let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
-                                       starts_unit: OffsetUnit::Byte };
+                                       starts_unit: OffsetUnit::Byte, invalid_utf8: InvalidUtf8::Reject };
         let r = self.plugin().await?.truncate_batch(ctx, req, max_tokens, keep).await?;
         texts.iter().enumerate().map(|(i, t)| {
             let cut = r.cut[i] as usize;
@@ -150,7 +150,7 @@ impl TokenizerClient for TokenizerService {
         }
         let (bytes, offsets) = pack_texts(texts);
         let req = EncodeBatchRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, with_starts: false,
-                                       starts_unit: OffsetUnit::Byte };
+                                       starts_unit: OffsetUnit::Byte, invalid_utf8: InvalidUtf8::Reject };
         let r = self.plugin().await?.encode_batch_special(ctx, req, special).await?;
         Ok((0..texts.len()).map(|i| r.ids[r.offsets[i] as usize..r.offsets[i + 1] as usize].to_vec()).collect())
     }
@@ -161,7 +161,7 @@ impl TokenizerClient for TokenizerService {
             return Ok(Usage::default());
         }
         let (bytes, offsets) = pack_texts(&texts);
-        let counts = self.plugin().await?.count_tokens(ctx, CountTokensRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None }).await?;
+        let counts = self.plugin().await?.count_tokens(ctx, CountTokensRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, invalid_utf8: InvalidUtf8::Reject }).await?;
         Ok(Usage { input_tokens: counts.iter().map(|c| u64::from(*c)).sum(), output_tokens: 0 })
     }
 
@@ -215,7 +215,7 @@ impl TokenizerClient for TokenizerService {
             return Ok(Usage { input_tokens: fixed, output_tokens: 0 });
         }
         let (bytes, offsets) = pack_texts(&texts);
-        let counts = self.plugin().await?.count_tokens(ctx, CountTokensRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None }).await?;
+        let counts = self.plugin().await?.count_tokens(ctx, CountTokensRequest { vocab: VocabRef(model.to_owned()), bytes, offsets, vocabs_per_prompt: None, vocab_index: None, invalid_utf8: InvalidUtf8::Reject }).await?;
         Ok(Usage { input_tokens: fixed + counts.iter().map(|c| u64::from(*c)).sum::<u64>(), output_tokens: 0 })
     }
 
