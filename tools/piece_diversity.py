@@ -1,47 +1,28 @@
 #!/usr/bin/env python3
 """Per-kernel times against the DIVERSITY of the pieces (VERDICT r1, weak 10: the bench corpus is ~2 MB of text tiled to 134 MB, so
 its distinct pieces are few and the hash probes hit L1 / L2 more than production text would).  Batches of the same size and prompt
-lengths whose "words" are drawn from the vocabulary itself: the D most common... the first D valid-UTF-8 tokens of the rank file,
-uniformly, joined by spaces and line breaks -- D = 1 000 ... all of them (about 10^5 distinct pieces, every one a table hit or a
-two/three-token merge).  JSON lines: D, per-kernel ms, L1/L2 are in the ncu capture of the same script if run under ncu."""
-import base64, json, os, sys
+lengths whose "words" are drawn from the vocabulary itself: the first D valid-UTF-8 tokens of the rank file, stripped, uniformly --
+D = 1 000 ... all of them (about 10^5 distinct pieces).  The batches are cfbpe.workload.make_vocab_text's "diverse" kind: the words
+joined by spaces, line breaks, punctuation and digit groups, with a share of separator-free runs.  JSON lines: D, per-kernel ms."""
+import json, os, sys
 os.environ.setdefault("CFBPE_ALLOW_STAND_IN", "1")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "cyberfabric-core_b200")):
     sys.path.insert(0, p)
 import numpy as np
 import torch
-from cfbpe import plugin as P, vocabs as V, _native as N
+from cfbpe import plugin as P, vocabs as V, workload as W, _native as N
 
 rv = V.resolve("cl100k_base", allow_stand_in=True)
-toks = []
-for line in rv.file_bytes.splitlines()[:rv.max_ranks or None]:
-    t = base64.b64decode(line.split()[0])
-    try:
-        s = t.decode("utf-8")
-    except UnicodeDecodeError:
-        continue
-    if s.strip() and not any(c.isspace() for c in s.strip()) and "�" not in s:
-        toks.append(s.strip().encode())
+n_words = len(W.vocab_words(W.vocab_tokens(rv.file_bytes, rv.max_ranks)))
 plug = P.GpuBpeTokenizerPlugin(0, ("cl100k_base",), 160 << 20, 1 << 17)
 dev = torch.device("cuda:0")
-rng = np.random.default_rng(7)
-n, target = 65536, 134_000_000
-for D in [int(a) for a in sys.argv[1:]] or [1000, 10000, len(toks)]:
-    D = min(D, len(toks))
-    pool = toks[:D] if D < len(toks) else toks
-    lens = np.array([len(t) + 1 for t in pool])
-    n_words = int(target / lens.mean())
-    pick = rng.integers(0, len(pool), size=n_words)
-    sep = np.where(rng.random(n_words) < 0.05, b"\n"[0], b" "[0]).astype(np.uint8)
-    buf = bytearray()
-    for i, s in zip(pick, sep):
-        buf += pool[i]; buf.append(int(s))
-    data = np.frombuffer(bytes(buf), dtype=np.uint8)
+n = 65536
+for D in [int(a) for a in sys.argv[1:]] or [1000, 10000, n_words]:
+    D = min(D, n_words)
+    # prompts of 8..4096 bytes (like the bench batch), cut at character boundaries
+    data, offs = W.make_vocab_text(rv.file_bytes, rv.max_ranks, 7, "diverse", n_prompts=n, distinct=D)
     total = len(data)
-    # prompts: cut at word boundaries near uniform lengths 8..4096 (like the bench batch)
-    cuts = np.sort(rng.choice(np.nonzero((data == 32) | (data == 10))[0] + 1, size=n - 1, replace=False))
-    offs = np.concatenate([[0], cuts, [total]]).astype(np.uint64)
     d_bytes = torch.zeros(total + 256, dtype=torch.uint8, device=dev); d_bytes[:total] = torch.from_numpy(data.copy()).to(dev)
     d_offs = torch.from_numpy(offs.astype(np.int64)).to(dev)
     d_ids = torch.empty(total + 1, dtype=torch.int32, device=dev)
@@ -63,5 +44,5 @@ for D in [int(a) for a in sys.argv[1:]] or [1000, 10000, len(toks)]:
         plug.ctx.encode_batch_device(n, d_bytes.data_ptr(), total, d_offs.data_ptr(), None, d_ids.data_ptr(), d_ids.numel(), d_off.data_ptr(), d_cnt.data_ptr(), s, sync=False)
     e1.record(); torch.cuda.synchronize(); plug.ctx.device_status(s)
     step = e0.elapsed_time(e1) / 5
-    print(json.dumps({"distinct_words": len(pool), "bytes": total, "tokens": nt, "miss_pieces": pr["n_miss_pieces"], "device_ms": round(step, 3), "GBps": round(total / step / 1e6, 2),
+    print(json.dumps({"distinct_words": D, "bytes": total, "tokens": nt, "miss_pieces": pr["n_miss_pieces"], "device_ms": round(step, 3), "GBps": round(total / step / 1e6, 2),
                       "kernel_ms": {k: round(v, 3) for k, v in acc.items() if v}}), flush=True)
