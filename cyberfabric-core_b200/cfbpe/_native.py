@@ -33,6 +33,7 @@ EXPORTS = [
     "cfbpe_truncate_batch", "cfbpe_truncate_batch_device",
     "cfbpe_chunk_batch", "cfbpe_chunk_batch_device",
     "cfbpe_encode_batch_lossy", "cfbpe_encode_batch_lossy_device",
+    "cfbpe_vocab_set_id_base", "cfbpe_vocab_get_id_base",
 ]
 
 
@@ -128,6 +129,10 @@ def load():
                                            C.POINTER(C.c_uint64), vp]
     L.cfbpe_vocab_set_specials.restype = C.c_int
     L.cfbpe_vocab_set_specials.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, vp, vp]
+    L.cfbpe_vocab_set_id_base.restype = C.c_int
+    L.cfbpe_vocab_set_id_base.argtypes = [vp, C.c_uint32, C.c_uint32]
+    L.cfbpe_vocab_get_id_base.restype = C.c_int
+    L.cfbpe_vocab_get_id_base.argtypes = [vp, C.c_uint32, C.POINTER(C.c_uint32)]
     L.cfbpe_encode_batch_special.restype = C.c_int
     L.cfbpe_encode_batch_special.argtypes = [vp, C.c_uint32, u8p, vp, u8p, vp, vp, C.c_uint64, vp, vp, vp]
     L.cfbpe_encode_batch_special_device.restype = C.c_int
@@ -486,6 +491,15 @@ class Context:
         """register {token string: id} as the special tokens of vocabulary slot `vocab_id` (replaces the earlier set; {} clears it)"""
         data, offs, ids = self.pack_specials(specials)
         self._check(load().cfbpe_vocab_set_specials(self._h, vocab_id, len(specials), data.ctypes.data, offs.ctypes.data, ids.ctypes.data))
+
+    def vocab_set_id_base(self, vocab_id, base):
+        """ordinary token of rank r of slot `vocab_id` -> id base + r in every id a call returns or decode takes (0: ids are ranks)"""
+        self._check(load().cfbpe_vocab_set_id_base(self._h, vocab_id, int(base)))
+
+    def vocab_id_base(self, vocab_id):
+        out = C.c_uint32(0)
+        self._check(load().cfbpe_vocab_get_id_base(self._h, vocab_id, C.byref(out)))
+        return out.value
 
     @staticmethod
     def _modes_arg(modes):

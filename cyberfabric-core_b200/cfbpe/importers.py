@@ -6,9 +6,11 @@ tiktoken/load.py:160-172: base64(token bytes), space, decimal rank, one per line
 
 The two formats describe the same merges differently -- HF lists the merges in order, tiktoken ranks every token's BYTES and
 merges the adjacent pair whose concatenation ranks lowest -- and agree exactly when (a) the vocabulary holds all 256 single
-bytes, (b) the ids of the mergeable tokens are 0..n-1, and (c) the merge list, read in order, produces tokens of increasing id.
+bytes, (b) the ids of the mergeable tokens are base..base+n-1 (rank = id - base), and (c) the merge list, read in order, produces tokens of increasing id.
 The importer checks all three and refuses a file it cannot convert exactly (a wrong count is worse than no count: the numbers
 bill tenants).  Special / added tokens are returned separately: they are not part of the rank file (tiktoken keeps them apart too).
+The base is 0 for GPT-2 / Llama-3 style files; Mistral's Tekken files put their 1000 control tokens first and number the
+mergeable tokens from 1000 -- load such a rank file with that id base (cfbpe_vocab_set_id_base) to get the file's ids.
 """
 from __future__ import annotations
 
@@ -60,7 +62,7 @@ def _find_pattern(node) -> Optional[str]:
 
 
 def hf_tokenizer_json_to_rank_file(data: bytes) -> Tuple[bytes, dict]:
-    """-> (rank file bytes, meta).  meta = {n_ranks, pattern_id or None, pattern, sha256 of the rank file, special_tokens}"""
+    """-> (rank file bytes, meta).  meta = {n_ranks, id_base, pattern_id or None, pattern, sha256 of the rank file, special_tokens}"""
     try:
         j = json.loads(data)
         model = j["model"]
@@ -82,8 +84,10 @@ def hf_tokenizer_json_to_rank_file(data: bytes) -> Tuple[bytes, dict]:
         except KeyError:
             raise ImportError_("token %r is not written in the byte-level alphabet (not a byte-level BPE vocabulary)" % s) from None
     n = len(toks)
-    if sorted(toks) != list(range(n)):
-        raise ImportError_("mergeable token ids are not 0..%d" % (n - 1))
+    base = min(toks) if toks else 0
+    if sorted(toks) != list(range(base, base + n)):
+        raise ImportError_("mergeable token ids are not %d..%d" % (base, base + n - 1))
+    toks = {i - base: b for i, b in toks.items()}
     rank = {b: i for i, b in toks.items()}
     if len(rank) != n:
         raise ImportError_("two ids share the same bytes")
@@ -106,7 +110,7 @@ def hf_tokenizer_json_to_rank_file(data: bytes) -> Tuple[bytes, dict]:
         raise ImportError_("%d merges for %d multi-byte tokens: some tokens are not reachable by merges" % (len(merges), n - 256))
     out = b"".join(base64.b64encode(toks[i]) + b" " + str(i).encode() + b"\n" for i in range(n))
     pattern = _find_pattern(j.get("pre_tokenizer"))
-    meta = {"n_ranks": n, "pattern": pattern, "pattern_id": _KNOWN_PATTERNS.get(pattern), "sha256": hashlib.sha256(out).hexdigest(),
+    meta = {"n_ranks": n, "id_base": base, "pattern": pattern, "pattern_id": _KNOWN_PATTERNS.get(pattern), "sha256": hashlib.sha256(out).hexdigest(),
             "special_tokens": added}
     return out, meta
 

@@ -312,14 +312,16 @@ class Usage:
 @dataclass(frozen=True)
 class ChatTemplate:
     """How a provider frames a list of chat messages into the token stream it bills as `Usage.input_tokens`
-    (SURVEY.md section 8(f) item 2: "chat-template overhead accounting").  Two kinds:
+    (SURVEY.md section 8(f) item 2: "chat-template overhead accounting").  Three kinds:
 
     "overhead"  a fixed number of framing tokens a message (OpenAI's ChatML accounting: every message is
                 <|start|>{role/name}\n{content}<|end|>\n = `tokens_per_message` tokens beside role and content, a `name` costs
                 `tokens_per_name` more, the reply is primed with `reply_priming` tokens);
     "rendered"  the conversation is rendered to text around control tokens (Llama 3, Mistral): `bos`, then per message
                 `message_prefix.format(role=...)` + content + `message_suffix`, then `generation_prompt`; the strings in
-                `special_tokens` count one token each, the text between them is tokenised as ordinary text.
+                `special_tokens` count one token each, the text between them is tokenised as ordinary text;
+    "mistral"   mistral_common's InstructTokenizerV3 on a text-only conversation (Tekken models: Mistral NeMo, Pixtral 12B):
+                mistral_instruct_texts gives the rules.  Every message's text is tokenised on its own, between control tokens.
 
     Message CONTENT is always ordinary text: a message that spells a control token gets the pieces of that spelling, never the
     control token (the gateway does not let user text forge framing)."""
@@ -340,11 +342,63 @@ CHAT_TEMPLATES = {
     # https://cookbook.openai.com "How to count tokens with tiktoken": gpt-3.5-turbo-0613 / gpt-4 and later
     "openai-chatml": ChatTemplate("overhead", tokens_per_message=3, tokens_per_name=1, reply_priming=3),
     # Meta Llama 3 instruct
+    # Mistral's Tekken models (mistral_common InstructTokenizerV3): <s>, then [INST] user [/INST] and assistant </s>
+    "mistral-v3": ChatTemplate("mistral"),
     "llama3-instruct": ChatTemplate("rendered", bos="<|begin_of_text|>",
                                     message_prefix="<|start_header_id|>{role}<|end_header_id|>\n\n", message_suffix="<|eot_id|>",
                                     generation_prompt="<|start_header_id|>assistant<|end_header_id|>\n\n",
                                     special_tokens=("<|begin_of_text|>", "<|start_header_id|>", "<|end_header_id|>", "<|eot_id|>")),
 }
+
+
+def mistral_instruct_texts(messages: Sequence[dict]) -> Tuple[List[str], int]:
+    """A text-only conversation as mistral_common 1.11's InstructTokenizerV3 encodes it (encode_chat_completion with its request
+    normalizer): (the ordinary texts in order, the number of control tokens).  The token count is the control tokens plus the
+    sum of the texts' token counts (Tekkenizer.encode(text, bos=False, eos=False), each text on its own).
+      - a message's text is its text parts joined with "\n\n"; other parts (images ...) are not counted here;
+      - system messages leave the sequence; the non-empty system texts, joined with "\n\n", are the system prompt;
+      - consecutive user (or assistant) messages merge into one, their texts joined with "\n\n" (a system message between two
+        messages of one role keeps them apart);
+      - when the first message left is not a user message, an empty user message goes first;
+      - <s>; then per message: user -> [INST] text [/INST], where the LAST user message's text is the system prompt + "\n\n" +
+        its text (when there is a system prompt); assistant -> its text without trailing spaces, then </s>.
+    What mistral_common's validator refuses raises InvalidInput: no message, a system message right after an assistant message,
+    an assistant message last (system messages aside), an assistant message without text."""
+    def text(m):
+        return "\n\n".join(str(p["text"]) for p in m.get("content", []) if p.get("type") == "text")
+    system = "\n\n".join(t for t in (text(m) for m in messages if m.get("role") == "system") if t)
+    if not messages:
+        raise InvalidInput("a conversation for the mistral template has at least one message")
+    turns: List[list] = []              # [role, text] after merging
+    prev = None
+    for m in messages:
+        role = m.get("role")
+        if role not in ("system", "user", "assistant"):
+            raise InvalidInput("the mistral template counts system, user and assistant messages, not %r" % role)
+        if role == "system" and prev == "assistant":
+            raise InvalidInput("a system message follows an assistant message")
+        if role != "system":
+            if role == prev:
+                turns[-1][1] += "\n\n" + text(m)
+            else:
+                turns.append([role, text(m)])
+        prev = role
+    if not turns or turns[0][0] != "user":
+        turns.insert(0, ["user", ""])
+    if turns[-1][0] != "user":
+        raise InvalidInput("a conversation for the mistral template ends with a user message")
+    last_user = max(i for i, t in enumerate(turns) if t[0] == "user")
+    texts, controls = [], 1             # <s>
+    for i, (role, t) in enumerate(turns):
+        if role == "user":
+            texts.append(system + "\n\n" + t if i == last_user and system else t)
+            controls += 2               # [INST] [/INST]
+        else:
+            if not t:
+                raise InvalidInput("an assistant message without text")
+            texts.append(t.rstrip(" "))
+            controls += 1               # </s>
+    return texts, controls
 
 
 # --------------------------------------------------------------------------- plugin trait
@@ -558,6 +612,10 @@ class GpuBpeTokenizerPlugin(TokenizerPluginClient):
                     self.ctx.vocab_import(slot, blob)
                 else:
                     self.ctx.vocab_load(slot, rv.file_bytes, rv.spec.fmt, rv.pattern_id, rv.max_ranks)
+                if rv.spec.id_base:         # the model's own ids: control tokens first, the ordinary tokens after them
+                    self.ctx.vocab_set_id_base(slot, rv.spec.id_base)
+                    self.ctx.vocab_set_specials(slot, rv.control_tokens)
+                    self._specials[slot] = dict(rv.control_tokens)
             except N.NativeError as e:
                 raise _map_native(e) from e
             self._slot[name] = slot
@@ -893,6 +951,8 @@ class LlmGatewayTokenizerService:
                 feed_framing(template.message_suffix)
             feed_framing(template.generation_prompt)
             texts = [t for t in run if t]
+        elif template.kind == "mistral":
+            texts, fixed = mistral_instruct_texts(messages)
         else:
             raise InvalidInput("unknown chat template kind %r" % template.kind)
         texts = [t for t in texts if t]

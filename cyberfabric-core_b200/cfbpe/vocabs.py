@@ -11,10 +11,14 @@ therefore resolves in this order:
      Mistral Tekken rank file truncated to the same vocabulary size, used with the requested pattern -- labelled
      `stand_in=True` so that every benchmark line and the plugin instance's properties say so.  Otherwise: VocabUnavailable.
 
-Tekken ids here are raw ranks 0..n-1 of the rank file; mistral_common shifts them by its 1000 reserved special-token ids
-(`id = rank + 1000`).  A gateway that serves Mistral models adds that offset above this layer.
+The "tekken" vocabulary speaks raw ranks 0..n-1 of the rank file (the stand-in slot every benchmark and test uses as such).
+"mistral_tekken" is the same ranks as mistral_common numbers them for Mistral's Tekken models: its 1000 control tokens first
+(<unk> 0, <s> 1, </s> 2, [INST] 3, [/INST] 4, ...; vocabs/tekken_controls.json) and the ordinary token of rank r at id 1000 + r
+(the plugin loads it with cfbpe_vocab_set_id_base(1000) and registers the control tokens as its special tokens).  Mistral NeMo's
+tekken_240718 and Pixtral's tekken_240911 hold the same first 130072 ranks, so both models use the committed 240911 file.
 """
 import hashlib
+import json
 import os
 from dataclasses import dataclass
 
@@ -23,6 +27,7 @@ from . import _native as N
 _ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 VOCAB_DIR = os.path.join(_ROOT, "vocabs")
 TEKKEN_FILE = os.path.join(VOCAB_DIR, "tekken_240911.tiktoken")
+TEKKEN_CONTROLS_FILE = os.path.join(VOCAB_DIR, "tekken_controls.json")
 
 # published sha256 of the OpenAI files (tiktoken_ext/openai_public.py)
 KNOWN_SHA256 = {
@@ -38,6 +43,8 @@ class VocabSpec:
     n_ranks: int          # vocabulary size of the real thing
     real_file: str = ""   # file name of the real rank file, if one exists publicly
     fmt: int = N.FORMAT_TIKTOKEN
+    id_base: int = 0      # id of the ordinary token of rank 0 (cfbpe_vocab_set_id_base)
+    controls: str = ""    # file under vocabs/ that lists the control tokens in id order (ids 0 .. id_base - 1), if any
 
 
 SPECS = {
@@ -45,6 +52,7 @@ SPECS = {
     "o200k_base": VocabSpec("o200k_base", "o200k", 199998, "o200k_base.tiktoken"),
     "llama3": VocabSpec("llama3", "llama3", 128000, "llama3.tiktoken"),
     "tekken": VocabSpec("tekken", "tekken", 130072, "tekken_240911.tiktoken"),
+    "mistral_tekken": VocabSpec("mistral_tekken", "tekken", 130072, "tekken_240911.tiktoken", id_base=1000, controls="tekken_controls.json"),
 }
 
 # canonical model id -> vocab (provider_slug::provider_model_id, modules/model-registry/docs/PRD.md:197)
@@ -52,7 +60,7 @@ MODEL_VOCABS = {
     "openai::gpt-4": "cl100k_base", "openai::gpt-3.5-turbo": "cl100k_base", "openai::text-embedding-3-small": "cl100k_base",
     "openai::gpt-4o": "o200k_base", "openai::gpt-4o-mini": "o200k_base", "openai::o1": "o200k_base",
     "meta::llama-3-8b-instruct": "llama3", "meta::llama-3.1-70b-instruct": "llama3",
-    "mistral::mistral-nemo": "tekken", "mistral::pixtral-12b": "tekken",
+    "mistral::mistral-nemo": "mistral_tekken", "mistral::pixtral-12b": "mistral_tekken",
 }
 
 
@@ -68,6 +76,21 @@ class ResolvedVocab:
     @property
     def pattern_id(self):
         return N.PATTERN_IDS[self.spec.pattern]
+
+    @property
+    def control_tokens(self) -> dict:
+        """{token string: id} of the vocabulary's control tokens (empty for a vocabulary without them)"""
+        return control_tokens(self.spec)
+
+
+def control_tokens(spec: VocabSpec) -> dict:
+    if not spec.controls:
+        return {}
+    with open(os.path.join(VOCAB_DIR, spec.controls), encoding="utf-8") as f:
+        toks = json.load(f)
+    if len(toks) != spec.id_base:
+        raise ValueError("%s lists %d control tokens for id base %d" % (spec.controls, len(toks), spec.id_base))
+    return {t: i for i, t in enumerate(toks)}
 
 
 def _read(path):
@@ -85,9 +108,10 @@ def resolve(name: str, allow_stand_in: bool = False) -> ResolvedVocab:
     if name not in SPECS:
         raise VocabUnavailable("unknown vocabulary %r" % name)
     spec = SPECS[name]
-    if name == "tekken":
+    if name in ("tekken", "mistral_tekken"):
         data = _read(TEKKEN_FILE)
-        return ResolvedVocab(spec, data, spec.n_ranks, False, "tekken_240911[:130072]", hashlib.sha256(data).hexdigest())
+        return ResolvedVocab(spec, data, spec.n_ranks, False, "tekken_240911[:130072]" + (" + 1000" if spec.id_base else ""),
+                             hashlib.sha256(data).hexdigest())
     for d in filter(None, [os.environ.get("CFBPE_VOCAB_DIR"), VOCAB_DIR]):
         p = os.path.join(d, spec.real_file)
         if os.path.exists(p):

@@ -1738,6 +1738,40 @@ starts_emit_kernel(BatchView b, const uint64_t* __restrict__ out_offsets, uint64
     }
 }
 
+// Id bases (cfbpe_vocab_set_id_base): the ordinary token of rank r of vocabulary v has the id v[v] + r.  Every kernel of the encode
+// path works on ranks; the rebase kernel turns the ranks a call returns into ids, and decode maps ids back to ranks.
+struct IdBases { uint32_t v[kMaxVocabs]; };
+
+// ids[r] += the base of the vocabulary of r's prompt, for the ranks [tok_end - n_tokens, min(tok_end, out_cap)) of the (sub-)batch
+// (status, as starts_len reads them).  A CTA takes kStartsTile ids.  Without per-prompt vocabularies the base is one constant and a
+// thread takes every 256th id of the tile (coalesced); else a thread takes 8 consecutive ids, finds the prompt of the first by rank
+// in out_offsets and steps on.
+__global__ void __launch_bounds__(256)
+id_rebase_kernel(BatchView b, IdBases ib, uint32_t* __restrict__ ids, const uint64_t* __restrict__ out_offsets, uint64_t out_cap,
+                 const DeviceStatus* status) {
+    const uint64_t n = status->n_tokens, r0 = status->tok_end - n;
+    const uint64_t lim = r0 + n < out_cap ? r0 + n : out_cap;
+    const uint64_t tile = r0 + static_cast<uint64_t>(blockIdx.x) * kStartsTile;
+    if (!b.vocab_ids) {
+        const uint32_t base = ib.v[0];
+#pragma unroll
+        for (uint32_t k = 0; k < kStartsTile / 256; ++k) {
+            const uint64_t r = tile + 256u * k + threadIdx.x;
+            if (r < lim) ids[r] += base;
+        }
+        return;
+    }
+    const uint64_t r = tile + 8u * threadIdx.x;
+    if (r >= lim) return;
+    const uint32_t m = lim - r < 8 ? static_cast<uint32_t>(lim - r) : 8u;
+    uint32_t p = find_prompt(out_offsets, b.n_prompts, r);
+    for (uint32_t k = 0; k < m; ++k) {
+        p = starts_prompt(out_offsets, p, r + k);
+        const uint32_t vid = b.vocab_ids[p];
+        ids[r + k] += ib.v[vid < kMaxVocabs ? vid : 0u];      // (a slot past the table is reported as bad_vocab by the pass)
+    }
+}
+
 // Truncation (pipeline.cuh, enqueue_emit): where to cut prompt p so that it keeps the first (head) or the last (tail) k = min(budget, c)
 // of its c tokens, moved to a character boundary; kept = the tokens wholly inside the kept span.  The boundary is token j (head:
 // j = k, tail: j = c - k) and its byte position is the sum of the lengths of the tokens before it -- or the prompt's length minus
@@ -2098,7 +2132,7 @@ struct DecodeView {
 
 __global__ void __launch_bounds__(256)
 decode_len_kernel(DecodeView d, VocabSet vs, uint32_t* __restrict__ lens, uint32_t* __restrict__ tile_sums, DeviceStatus* status,
-                  SpecialSet sp = SpecialSet{}) {
+                  SpecialSet sp = SpecialSet{}, IdBases ib = IdBases{}) {
     __shared__ uint32_t s_tmp[8];
     const uint64_t base = static_cast<uint64_t>(blockIdx.x) * kDecodeTile;
     uint32_t sum = 0;
@@ -2108,9 +2142,9 @@ decode_len_kernel(DecodeView d, VocabSet vs, uint32_t* __restrict__ lens, uint32
         uint32_t vid = 0;
         if (d.vocab_ids) vid = d.vocab_ids[find_prompt(d.id_offsets, d.n_seqs, i)];
         const TablesView& T = vs.v[vid];
-        const uint32_t id = d.ids[i];
+        const uint32_t id = d.ids[i], rank = id - ib.v[vid];   // (an id below the base wraps past n_ranks: base + n_ranks < 2^32)
         uint32_t len = 0;
-        if (id < T.n_ranks) len = T.tokoff[id + 1] - T.tokoff[id];
+        if (rank < T.n_ranks) len = T.tokoff[rank + 1] - T.tokoff[rank];
         else {                                          // not an ordinary token: a special token of the vocabulary, or unknown
             const int k = sp_by_id(sp.v[vid], id);
             if (k >= 0) len = sp_len(sp.v[vid], static_cast<uint32_t>(k));
@@ -2125,7 +2159,7 @@ decode_len_kernel(DecodeView d, VocabSet vs, uint32_t* __restrict__ lens, uint32
 
 __global__ void __launch_bounds__(256)
 decode_copy_kernel(DecodeView d, VocabSet vs, const uint32_t* __restrict__ lens, const uint64_t* __restrict__ tile_base,
-                   uint8_t* __restrict__ out, uint64_t out_cap, SpecialSet sp = SpecialSet{}) {
+                   uint8_t* __restrict__ out, uint64_t out_cap, SpecialSet sp = SpecialSet{}, IdBases ib = IdBases{}) {
     __shared__ uint32_t s_warp[8];
     const uint64_t base = static_cast<uint64_t>(blockIdx.x) * kDecodeTile + 4ull * threadIdx.x;   // my four consecutive tokens
     uint32_t l[4], mine = 0;
@@ -2146,8 +2180,8 @@ decode_copy_kernel(DecodeView d, VocabSet vs, const uint32_t* __restrict__ lens,
         uint32_t vid = 0;
         if (d.vocab_ids) vid = d.vocab_ids[find_prompt(d.id_offsets, d.n_seqs, base + t)];
         const TablesView& T = vs.v[vid];
-        const uint32_t id = d.ids[base + t];
-        const uint8_t* src = id < T.n_ranks ? T.blob + T.tokoff[id]
+        const uint32_t id = d.ids[base + t], rank = id - ib.v[vid];
+        const uint8_t* src = rank < T.n_ranks ? T.blob + T.tokoff[rank]
                                             : sp_bytes(sp.v[vid]) + sp.v[vid].w[sp.v[vid].o_offs + sp_by_id(sp.v[vid], id)];   // a special token
         for (uint32_t k = 0; k < l[t]; ++k) if (o + k < out_cap) out[o + k] = src[k];
         o += l[t];

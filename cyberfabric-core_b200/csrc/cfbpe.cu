@@ -189,6 +189,7 @@ struct DeviceCtx {
     VocabSet vs{};
     DevPtr<uint32_t> d_specials[CFBPE_MAX_VOCABS];   // each vocabulary's special-token table (specials.h), or empty
     SpecialSet specials{};                          // their views (modes NULL): what decode reads
+    IdBases bases{};                                // each vocabulary's id base (cfbpe_vocab_set_id_base): kernel arguments, no device memory
     std::vector<std::unique_ptr<Lane>> lanes;
     std::atomic<uint32_t> next_lane{0};
     void* comm = nullptr;                 // ncclComm_t of this device in the context's communicator
@@ -362,7 +363,8 @@ int install_blob(cfbpe_ctx* ctx, uint32_t vocab_id, std::vector<uint8_t>&& blob)
         for (size_t d = 0; d < G; ++d) { cudaSetDevice(ctx->devs[d]->device); if (cudaStreamSynchronize(ctx->devs[d]->lanes[0]->stream.get()) != cudaSuccess && rc == 0) rc = -1; }
         if (rc != 0) return fail(ctx, CFBPE_EIO, std::string("ncclBroadcast of the vocabulary tables: ") + (rc > 0 ? nc.GetErrorString(rc) : "stream error"));
     }
-    clear_specials(ctx, vocab_id);           // a new vocabulary starts without special tokens
+    clear_specials(ctx, vocab_id);           // a new vocabulary starts without special tokens, and with ids = ranks
+    for (auto& dvp : ctx->devs) dvp->bases.v[vocab_id] = 0;
     HostVocab& hv = ctx->vocabs[vocab_id];
     hv.h_blob = std::move(blob);
     std::memcpy(&hv.hdr, hv.h_blob.data(), sizeof(TablesHeader));
@@ -425,6 +427,23 @@ int ensure_call_buffers(cfbpe_ctx* ctx, Lane* ln, bool starts, bool trunc, bool 
     if (!rc && chunk) rc = ensure_lane_buffer(ctx, ln->d_chunk_offs, lane_offsets_alloc(mp, kMaxPipeChunks) + CFBPE_MAX_DEVICES, "the chunk offsets");
     if (!rc && lens) rc = ensure_lane_buffer(ctx, ln->d_unit_lens, mp + 1, "the unit lengths");
     return rc;
+}
+
+// The id bases the rebase of a host call (or of one of its sub-batches or shards) adds: &dv->bases, or nullptr when no vocabulary
+// its n prompts name (vocab_ids, host memory; NULL: vocabulary 0) has a base above 0 -- then the rebase is not launched at all.
+const IdBases* call_bases(const DeviceCtx* dv, const uint8_t* vocab_ids, uint32_t n) {
+    uint32_t based = 0;
+    for (uint32_t v = 0; v < CFBPE_MAX_VOCABS; ++v) if (dv->bases.v[v]) based |= 1u << v;
+    if (!based) return nullptr;
+    if (!vocab_ids) return (based & 1u) ? &dv->bases : nullptr;
+    for (uint32_t i = 0; i < n; ++i) if ((based >> vocab_ids[i]) & 1u) return &dv->bases;
+    return nullptr;
+}
+// ... of a device-path call, whose vocabulary ids the host does not read: with d_vocab_ids, every vocabulary may be touched
+const IdBases* device_call_bases(const DeviceCtx* dv, const uint8_t* d_vocab_ids) {
+    if (!d_vocab_ids) return call_bases(dv, nullptr, 0);
+    for (uint32_t v = 0; v < CFBPE_MAX_VOCABS; ++v) if (dv->bases.v[v]) return &dv->bases;
+    return nullptr;
 }
 
 // A host unit-start call (cfbpe_encode_batch_char_starts): the starts go where byte starts go (the lane's starts buffer, then
@@ -595,6 +614,9 @@ int run_host_pipelined(cfbpe_ctx* ctx, DeviceCtx* const* dvs, Lane* const* lns, 
         enqueue_emit(b, w, want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get() + q0, ln->d_out_counts.get() + p0,
                      ss, static_cast<ProfEvents*>(nullptr), (out_starts || chunk) ? ln->d_out_starts.get() : nullptr, &dv->vs, trunc ? &tv : nullptr,
                      chunk ? &cv : nullptr, unit ? &uv : nullptr);
+        if (want_ids && !trunc && !chunk)      // (truncate and chunk calls keep their ranks in the lane)
+            enqueue_rebase(b, call_bases(dv, vocab_ids ? vocab_ids + p0 : nullptr, nk), ln->d_out_ids.get(), ln->d_out_offsets.get() + q0,
+                           ctx->max_bytes, w.status, ss);
         if (chunk) CK(cudaEventRecord(ln->ev_chain[k].get(), ss));       // (the chunk scan read the previous chunk_end: the chain ends here)
         CK(cudaGetLastError());
         status_publish_kernel<<<1, 64, 0, ss>>>(ln->d_status_arr.get() + k, ln->h_status_arr.get() + k);
@@ -696,6 +718,7 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
                    ln->d_out_counts.get(), static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
                    ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, (out_starts || chunk) ? ln->d_out_starts.get() : nullptr, trunc ? &tv : nullptr,
                    chunk ? &cv : nullptr, unit ? &uv : nullptr);
+    if (want_ids && !trunc && !chunk) enqueue_rebase(b, call_bases(dv, vocab_ids, n), ln->d_out_ids.get(), ln->d_out_offsets.get(), ctx->max_bytes, ln->ws.status, s);
     CK(cudaGetLastError());
     if (prof) cudaEventRecord(prof->d2h[0].get(), s);
     CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
@@ -798,7 +821,7 @@ struct EncodeOut { uint32_t* ids; uint64_t cap; uint64_t* offsets; uint32_t* cou
 // special) and what it found, then the ordinary path on the prompts as they are, into `plain`, or on the stretches followed by the
 // splice, into `spliced` (the stretches' own ids, offsets and counts go to the lane's d_out_* buffers).  *did_splice: which ran.
 int enqueue_special_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchView& b, const SpecialSet& sp, bool scan, cudaStream_t s,
-                         const EncodeOut& plain, const EncodeOut& spliced, uint32_t* out_bad, bool* did_splice) {
+                         const EncodeOut& plain, const EncodeOut& spliced, uint32_t* out_bad, bool* did_splice, const IdBases* bases) {
     const SpecialWork sw = special_work(ln);
     uint64_t n_str = b.n_prompts;
     if (scan) {       // the one synchronisation of the call: the host needs the number of stretches for the launch geometry
@@ -817,10 +840,12 @@ int enqueue_special_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchVie
     if (!*did_splice) {
         enqueue_encode(b, dv->vs, dv->uc, ln->ws, plain.ids, plain.cap, plain.offsets, plain.counts, grid,
                        s, ln->aux_stream.get(), ln->aux2_stream.get(), ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), static_cast<ProfEvents*>(nullptr));
+        enqueue_rebase(b, bases, plain.ids, plain.offsets, plain.cap, ln->ws.status, s);
     } else {
         enqueue_encode_special(b, sp, dv->vs, dv->uc, ln->ws, sw, static_cast<uint32_t>(n_str), ln->d_out_ids.get(), ctx->max_bytes, ln->d_out_offsets.get(),
                                ln->d_out_counts.get(), spliced.ids, spliced.cap, spliced.offsets, spliced.counts,
-                               grid, s, ln->aux_stream.get(), ln->aux2_stream.get(), ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), static_cast<ProfEvents*>(nullptr));
+                               grid, s, ln->aux_stream.get(), ln->aux2_stream.get(), ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), static_cast<ProfEvents*>(nullptr),
+                               bases);
     }
     CK(cudaGetLastError());
     return CFBPE_OK;
@@ -1038,7 +1063,7 @@ int run_lane_special(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const 
     if ((rc = special_set(ctx, dv, ln, modes, &sp, &scan, s)) || (rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b))) return rc;
     const EncodeOut plain{want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get(), ln->d_out_counts.get()};
     const EncodeOut fin{want_ids ? ln->ws.lscratch.rank : nullptr, ctx->max_bytes, ln->sp.fin_offsets.get(), ln->sp.fin_counts.get()};
-    if ((rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, plain, fin, out_bad, &spliced))) return rc;
+    if ((rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, plain, fin, out_bad, &spliced, call_bases(dv, vocab_ids, n)))) return rc;
     if (spliced) CK(cudaMemcpyAsync(ln->sp.h_status.get(), ln->sp.status.get(), sizeof(SpecialStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -1113,7 +1138,7 @@ int ensure_lossy_lane(cfbpe_ctx* ctx, Lane* ln) {
 // invalid byte) or on the repaired batch, which goes to the lane's byte buffer.  When b.bytes IS that buffer (a host call), the
 // bytes are first copied to ids_by_pos (4 bytes a byte, dead until the ordinary pass starts).  The prompts' U+FFFD counts are left
 // in the lane's replaced buffer.  A repaired batch over max_batch_bytes fails with CFBPE_EINVAL before anything is written to `out`.
-int enqueue_lossy_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, const EncodeOut& out) {
+int enqueue_lossy_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, const EncodeOut& out, const IdBases* bases) {
     const LossyWork lw{ln->lossy.replaced.get(), ln->lossy.offsets.get(), ln->lossy.status.get()};
     enqueue_utf8_scan(b, dv->vs, ln->ws, lw, s);
     CK(cudaGetLastError());
@@ -1135,6 +1160,7 @@ int enqueue_lossy_call(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, const BatchView&
     }
     enqueue_encode(eb, dv->vs, dv->uc, ln->ws, out.ids, out.cap, out.offsets, out.counts, static_cast<uint32_t>(dv->sm_count * 4),
                    s, ln->aux_stream.get(), ln->aux2_stream.get(), ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), static_cast<ProfEvents*>(nullptr));
+    enqueue_rebase(eb, bases, out.ids, out.offsets, out.cap, ln->ws.status, s);
     CK(cudaGetLastError());
     return CFBPE_OK;
 }
@@ -1153,7 +1179,7 @@ int run_lane_lossy(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const ui
     BatchView b;
     if ((rc = upload_batch(ctx, ln, n, bytes, offsets, vocab_ids, total, s, &b))) return rc;
     const EncodeOut out{want_ids ? ln->d_out_ids.get() : nullptr, ctx->max_bytes, ln->d_out_offsets.get(), ln->d_out_counts.get()};
-    if ((rc = enqueue_lossy_call(ctx, dv, ln, b, s, out))) return rc;
+    if ((rc = enqueue_lossy_call(ctx, dv, ln, b, s, out, call_bases(dv, vocab_ids, n)))) return rc;
     CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     if (!defer) {
         if (out_offsets) CK(cudaMemcpyAsync(out_offsets, ln->d_out_offsets.get(), (static_cast<uint64_t>(n) + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
@@ -1375,6 +1401,7 @@ int run_device(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint6
                        static_cast<uint32_t>(dv->sm_count * 4), s, prof ? s : ln->aux_stream.get(), prof ? s : ln->aux2_stream.get(),
                        ln->ev_fork.get(), ln->ev_join.get(), ln->ev_join2.get(), prof, nullptr, d_out_starts, nullptr, nullptr,
                        unit);   // profiling: one stream, so that the per-kernel times do not overlap
+        enqueue_rebase(b, device_call_bases(dv, d_vocab_ids), d_out_ids, d_out_offsets, out_cap, ln->ws.status, s);
         CK(cudaGetLastError());
         return CFBPE_OK;
     });
@@ -1390,7 +1417,7 @@ int run_device_special(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_byte
         bool scan = false, spliced = false;
         const EncodeOut out{d_out_ids, out_cap, d_out_offsets, d_out_counts};
         int rc = special_set(ctx, dv, ln, modes, &sp, &scan, s);
-        if (!rc) rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, out, out, out_bad, &spliced);
+        if (!rc) rc = enqueue_special_call(ctx, dv, ln, b, sp, scan, s, out, out, out_bad, &spliced, device_call_bases(dv, d_vocab_ids));
         // the lane's status carries the call's id count (cfbpe_device_status checks it against out_cap): n_tokens and tok_end
         if (!rc && spliced) CK(cudaMemcpyAsync(&ln->ws.status->n_tokens, &ln->sp.status->fin.n_tokens, 2 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, s));
         return rc;
@@ -1405,7 +1432,7 @@ int run_device_lossy(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes,
     return device_call(ctx, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_out_offsets, d_out_ids != nullptr, out_cap, n_tokens, stream, false,
                        [&](DeviceCtx* dv, Lane* ln, const BatchView& b, cudaStream_t s, ProfEvents*) {
         int rc = ensure_lossy_lane(ctx, ln);
-        if (!rc) rc = enqueue_lossy_call(ctx, dv, ln, b, s, EncodeOut{d_out_ids, out_cap, d_out_offsets, d_out_counts});
+        if (!rc) rc = enqueue_lossy_call(ctx, dv, ln, b, s, EncodeOut{d_out_ids, out_cap, d_out_offsets, d_out_counts}, device_call_bases(dv, d_vocab_ids));
         if (!rc && d_out_replaced && n_prompts)
             CK(cudaMemcpyAsync(d_out_replaced, ln->lossy.replaced.get(), static_cast<uint64_t>(n_prompts) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
         return rc;
@@ -1684,9 +1711,9 @@ int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, con
     CK(cudaMemsetAsync(ln->ws.status, 0, sizeof(DeviceStatus), s));
     DecodeView d{ln->d_out_ids.get(), ln->d_offsets.get(), vocab_ids ? ln->d_vocab_ids.get() : nullptr, n_seqs, n_ids};
     const uint32_t n_tiles = static_cast<uint32_t>((n_ids + kDecodeTile - 1) / kDecodeTile);
-    if (n_tiles) decode_len_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_sums.get(), ln->ws.status, dv->specials);
+    if (n_tiles) decode_len_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_sums.get(), ln->ws.status, dv->specials, dv->bases);
     tile_scan_kernel<<<1, n_tiles ? 1024 : 32, 0, s>>>(ln->d_dec_sums.get(), n_tiles, ln->d_dec_base.get(), ln->ws.status, nullptr);
-    if (n_tiles) decode_copy_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_base.get(), ln->d_bytes.get(), ctx->max_bytes, dv->specials);
+    if (n_tiles) decode_copy_kernel<<<n_tiles, 256, 0, s>>>(d, dv->vs, ln->ws.ids_by_pos, ln->d_dec_base.get(), ln->d_bytes.get(), ctx->max_bytes, dv->specials, dv->bases);
     decode_offsets_kernel<<<static_cast<unsigned>((static_cast<uint64_t>(n_seqs) + 1 + 255) / 256), 256, 0, s>>>(d, ln->ws.ids_by_pos, ln->d_dec_base.get(), ln->d_out_offsets.get(), ln->ws.status);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
@@ -1774,6 +1801,8 @@ int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, cons
     if (rc) return fail(ctx, rc, e);
     std::unique_lock<std::shared_mutex> lock(ctx->vocab_mu);
     if (!ctx->vocabs[vocab_id].loaded) return fail(ctx, CFBPE_ENOENT, "vocab " + std::to_string(vocab_id) + " is not loaded");
+    if (const int k = special_in_id_range(words, ctx->devs[0]->bases.v[vocab_id], ctx->vocabs[vocab_id].hdr.n_ranks); k >= 0)
+        return fail(ctx, CFBPE_EINVAL, "special token " + std::to_string(k) + " has an id of an ordinary token (the vocabulary's id base is set)");
     const size_t G = ctx->devs.size();
     std::vector<DevPtr<uint32_t>> nt(G);      // the new tables, one a device: released on return unless installed
     if (!words.empty()) {
@@ -1794,6 +1823,29 @@ int cfbpe_vocab_set_specials(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t n, cons
         dv->d_specials[vocab_id] = std::move(nt[d]);
         dv->specials.v[vocab_id] = make_special_view(dv->d_specials[vocab_id].get(), ctx->specials[vocab_id]);
     }
+    return CFBPE_OK;
+}
+
+int cfbpe_vocab_set_id_base(cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t base) {
+    DeviceGuard restore_device;
+    if (!ctx) return CFBPE_EINVAL;
+    tl_err.clear();
+    if (vocab_id >= CFBPE_MAX_VOCABS) return fail(ctx, CFBPE_EINVAL, "vocab_id out of range");
+    std::unique_lock<std::shared_mutex> lock(ctx->vocab_mu);
+    if (!ctx->vocabs[vocab_id].loaded) return fail(ctx, CFBPE_ENOENT, "vocab " + std::to_string(vocab_id) + " is not loaded");
+    const uint32_t n_ranks = ctx->vocabs[vocab_id].hdr.n_ranks;
+    if (static_cast<uint64_t>(base) + n_ranks > 0xFFFFFFFFull)
+        return fail(ctx, CFBPE_EINVAL, "base + n_ranks (" + std::to_string(static_cast<uint64_t>(base) + n_ranks) + ") must not exceed 0xFFFFFFFF");
+    if (const int k = special_in_id_range(ctx->specials[vocab_id], base, n_ranks); k >= 0)
+        return fail(ctx, CFBPE_EINVAL, "registered special token " + std::to_string(k) + " has an id in [base, base + n_ranks)");
+    for (auto& dv : ctx->devs) dv->bases.v[vocab_id] = base;     // a kernel argument: calls that follow pass the new value
+    return CFBPE_OK;
+}
+
+int cfbpe_vocab_get_id_base(const cfbpe_ctx* ctx, uint32_t vocab_id, uint32_t* out) {
+    if (!ctx || !out || vocab_id >= CFBPE_MAX_VOCABS) return CFBPE_EINVAL;
+    if (!ctx->vocabs[vocab_id].loaded) return CFBPE_ENOENT;
+    *out = ctx->devs[0]->bases.v[vocab_id];
     return CFBPE_OK;
 }
 

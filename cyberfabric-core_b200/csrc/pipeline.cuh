@@ -333,6 +333,17 @@ inline void enqueue_back(const BatchView& b, const Workspace& w, uint32_t* out_i
     enqueue_emit(b, w, out_ids, out_cap, out_offsets, out_counts, stream, prof, out_starts, vs, trunc, chunk, unit);
 }
 
+// The ids of a (sub-)batch from its ranks (id_rebase_kernel), once every kernel that reads them as ranks has run.  bases: the id bases
+// of the vocabularies, or nullptr when none the call can touch has a base above 0 (nothing is launched).  status, out_offsets and
+// out_cap: those of the pass that emitted the ranks into ids.
+template <typename Stream>
+inline void enqueue_rebase(const BatchView& b, const IdBases* bases, uint32_t* ids, const uint64_t* out_offsets, uint64_t out_cap,
+                           const DeviceStatus* status, Stream stream) {
+    if (!bases || !ids || !b.total_bytes) return;
+    const uint32_t n_tiles = static_cast<uint32_t>((b.total_bytes + kStartsTile - 1) / kStartsTile);   // (at most one id a byte)
+    CFBPE_LAUNCH(id_rebase_kernel, n_tiles, 256, stream, b, *bases, ids, out_offsets, out_cap, status);
+}
+
 // The whole path.  `aux` / `aux2` are streams of their own for the two long-piece kernels (pass the main stream to run everything
 // in order); CFBPE_FORK / CFBPE_JOIN order them.  out_ids may be nullptr (count only); out_starts (nullable, with out_ids): the
 // tokens' byte offsets within their prompts; trunc (nullable, with out_ids): the prompts' cuts to their token budgets; chunk

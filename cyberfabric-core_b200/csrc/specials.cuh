@@ -241,10 +241,12 @@ template <typename Stream, typename Ev, typename Prof>
 inline void enqueue_encode_special(const BatchView& b, const SpecialSet& sp, const VocabSet& vs, const UcTables& uc, const Workspace& w,
                                    const SpecialWork& sw, uint32_t n_stretches, uint32_t* ord_ids, uint64_t ord_cap, uint64_t* ord_offsets,
                                    uint32_t* ord_counts, uint32_t* out_ids, uint64_t out_cap, uint64_t* out_offsets, uint32_t* out_counts,
-                                   uint32_t long_grid, Stream stream, Stream aux, Stream aux2, Ev ev_fork, Ev ev_join, Ev ev_join2, Prof* prof) {
+                                   uint32_t long_grid, Stream stream, Stream aux, Stream aux2, Ev ev_fork, Ev ev_join, Ev ev_join2, Prof* prof,
+                                   const IdBases* bases = nullptr) {
     CFBPE_LAUNCH(special_layout_kernel, static_cast<unsigned>((static_cast<uint64_t>(b.n_prompts) + 7) / 8), 256, stream, b, sp, w.tok_bits, w.ids_by_pos, sw, n_stretches);
     const BatchView st{b.bytes, sw.st_off, b.vocab_ids ? sw.st_vocab : nullptr, n_stretches, b.total_bytes};
     enqueue_encode(st, vs, uc, w, out_ids ? ord_ids : nullptr, ord_cap, ord_offsets, ord_counts, long_grid, stream, aux, aux2, ev_fork, ev_join, ev_join2, prof);
+    enqueue_rebase(st, bases, out_ids ? ord_ids : nullptr, ord_offsets, ord_cap, w.status, stream);   // the text's ids; a special's id is spliced as registered
     const unsigned g = static_cast<unsigned>((static_cast<uint64_t>(n_stretches) + 255) / 256);
     CFBPE_LAUNCH(special_mark_kernel, g, 256, stream, sw.st_id, n_stretches, ord_counts);
     CFBPE_LAUNCH(tile_scan_kernel, 1u, 1024, stream, ord_counts, n_stretches, sw.st_base, &sw.status->fin, static_cast<const uint64_t*>(nullptr));

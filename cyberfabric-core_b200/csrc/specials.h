@@ -205,4 +205,16 @@ inline int build_special_table(uint32_t n, const uint8_t* bytes, const uint64_t*
     return 0;
 }
 
+// The index of a special in the table `words` (build_special_table) whose id lies in [base, base + n_ranks), the ids of the ordinary
+// tokens under an id base (cfbpe_vocab_set_id_base), or -1.  A base of 0 reserves no range: an id below n_ranks then stays the
+// ordinary token, as it always was.
+inline int special_in_id_range(const std::vector<uint32_t>& words, uint32_t base, uint32_t n_ranks) {
+    if (!base || words.empty()) return -1;
+    for (uint32_t k = 0; k < words[0]; ++k) {
+        const uint32_t id = words[words[7] + k];
+        if (id >= base && id - base < n_ranks) return static_cast<int>(k);
+    }
+    return -1;
+}
+
 }  // namespace cfbpe

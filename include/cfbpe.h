@@ -245,7 +245,8 @@ CFBPE_API int cfbpe_chunk_batch(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_
  * ids: the packed token ids of n_seqs sequences, id_offsets[n_seqs + 1] their boundaries (in ids), vocab_ids[n_seqs] or NULL.
  * out_offsets[n_seqs + 1]: byte boundaries of the decoded sequences in out_bytes.  CFBPE_ENOSPC if out_cap is too small
  * (out_offsets[n_seqs] = bytes needed), CFBPE_EINVAL for an id outside its vocabulary or a batch beyond the context's limits
- * (at most max_batch_bytes ids and max_batch_bytes decoded bytes).  An id past the vocabulary's ranks that is one of its
+ * (at most max_batch_bytes ids and max_batch_bytes decoded bytes).  Ids are ranks, or base + rank with an id base set
+ * (cfbpe_vocab_set_id_base).  An id past the vocabulary's ranks that is one of its
  * registered special tokens (cfbpe_vocab_set_specials) decodes to that token's bytes.  Host buffers; no reference interface exists for it
  * (the reference ships no tokenizer: SURVEY.md F1). */
 CFBPE_API int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t* ids, const uint64_t* id_offsets,
@@ -257,9 +258,26 @@ CFBPE_API int cfbpe_decode_batch(cfbpe_ctx* ctx, uint32_t n_seqs, const uint32_t
  * 0xFFFFFFFF), at most CFBPE_MAX_SPECIALS of them: else CFBPE_EINVAL.  CFBPE_ENOENT for a slot that is not loaded.  The table
  * is copied to every device of the context; it is not part of the exported blob (a multi-process deployment registers the
  * specials on each rank).  Waits for running calls, as a vocabulary load does.  Decode then turns these ids into their bytes
- * (an id below the vocabulary's n_ranks is always the ordinary token). */
+ * (an id below the vocabulary's n_ranks is always the ordinary token; with an id base set, see cfbpe_vocab_set_id_base). */
 CFBPE_API int cfbpe_vocab_set_specials(cfbpe_ctx *ctx, uint32_t vocab_id, uint32_t n, const uint8_t *bytes, const uint64_t *offsets,
                                        const uint32_t *ids);
+
+/* Give the ordinary tokens of a vocabulary the ids base + rank (rank 0 .. n_ranks - 1) instead of their ranks: mistral_common's
+ * Tekken numbers its ordinary tokens from 1000, after its control tokens (<unk> 0, <s> 1, </s> 2, [INST] 3, ...).  Every id an
+ * encode call returns (cfbpe_encode_batch and its _starts, _char_starts, _special, _lossy and _device forms) is then
+ * base(v) + rank for its prompt's vocabulary v; a special token's id (cfbpe_encode_batch_special) is written as registered.  Decode
+ * takes an id in [base, base + n_ranks) as the ordinary token id - base; any other id must be a registered special token
+ * (else CFBPE_EINVAL).  Counts, offsets, starts, truncation and chunks do not depend on the base.
+ * The base is 0 until set, and cfbpe_vocab_load and cfbpe_vocab_import reset it to 0.  base + n_ranks must not exceed 0xFFFFFFFF
+ * (CFBPE_EINVAL).  With a base above 0, no special token may have an id in [base, base + n_ranks): this call refuses a base that
+ * would put a registered special there, and cfbpe_vocab_set_specials refuses such a special (CFBPE_EINVAL); with base 0 the rules
+ * of cfbpe_vocab_set_specials are unchanged.  CFBPE_ENOENT for a slot that is not loaded.  The base is copied to every device of
+ * the context; it is not part of the exported blob (a multi-process deployment sets it on each rank).  Waits for running calls, as
+ * a vocabulary load does.  Costs: a call that returns ids for a vocabulary with a base above 0 runs one more small kernel (a read
+ * and a write of every id); other calls run nothing more. */
+CFBPE_API int cfbpe_vocab_set_id_base(cfbpe_ctx *ctx, uint32_t vocab_id, uint32_t base);
+/* the id base of a loaded vocabulary (cfbpe_vocab_set_id_base): CFBPE_EINVAL for a NULL pointer or a bad slot, CFBPE_ENOENT if not loaded */
+CFBPE_API int cfbpe_vocab_get_id_base(const cfbpe_ctx *ctx, uint32_t vocab_id, uint32_t *out);
 
 /* Encode as tiktoken's Encoding.encode(text, allowed_special=..., disallowed_special=...) does, per prompt:
  *  1. if a DISALLOWED special occurs anywhere in the prompt's bytes (inside or across an allowed one too), the call fails with

@@ -115,6 +115,8 @@ extern "C" {
                                      d_out_offsets: *mut u64, d_out_counts: *mut u32, n_tokens: *mut u64,
                                      stream: *mut c_void) -> c_int;
     pub fn cfbpe_vocab_set_specials(ctx: *mut cfbpe_ctx, vocab_id: u32, n: u32, bytes: *const u8, offsets: *const u64, ids: *const u32) -> c_int;
+    pub fn cfbpe_vocab_set_id_base(ctx: *mut cfbpe_ctx, vocab_id: u32, base: u32) -> c_int;
+    pub fn cfbpe_vocab_get_id_base(ctx: *const cfbpe_ctx, vocab_id: u32, out: *mut u32) -> c_int;
     pub fn cfbpe_encode_batch_special(ctx: *mut cfbpe_ctx, n_prompts: u32, bytes: *const u8, offsets: *const u64, vocab_ids: *const u8,
                                       modes: *const *const u8, out_ids: *mut u32, out_cap: u64, out_offsets: *mut u64, out_counts: *mut u32,
                                       out_bad: *mut u32) -> c_int;
@@ -310,6 +312,20 @@ impl Ctx {
 
     /// Register `(token, id)` pairs as the special tokens of a vocabulary slot (the pair order is the special index the
     /// per-call modes refer to); an empty slice clears them.
+    /// The ordinary token of rank `r` gets the id `base + r` in every id a call returns or decode takes (`cfbpe_vocab_set_id_base`;
+    /// 0: ids are ranks).  Mistral's Tekken numbers its ordinary tokens from 1000, after its control tokens.
+    pub fn vocab_set_id_base(&self, vocab_id: u32, base: u32) -> Result<(), NativeError> {
+        // SAFETY: plain values.
+        self.check(unsafe { cfbpe_vocab_set_id_base(self.0.as_ptr(), vocab_id, base) })
+    }
+
+    pub fn vocab_id_base(&self, vocab_id: u32) -> Result<u32, NativeError> {
+        let mut out = 0u32;
+        // SAFETY: out is a valid destination.
+        self.check(unsafe { cfbpe_vocab_get_id_base(self.0.as_ptr(), vocab_id, &mut out) })?;
+        Ok(out)
+    }
+
     pub fn vocab_set_specials(&self, vocab_id: u32, specials: &[(String, u32)]) -> Result<(), NativeError> {
         let mut bytes = Vec::new();
         let mut offsets = vec![0u64];

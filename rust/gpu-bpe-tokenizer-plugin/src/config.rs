@@ -72,4 +72,11 @@ pub struct VocabConfig {
     /// canonical model ids `{provider_slug}::{provider_model_id}` served by this vocabulary
     #[serde(default)]
     pub models: Vec<String>,
+    /// id of the ordinary token of rank 0 (0 = ids are ranks; Mistral's Tekken: 1000, after its control tokens)
+    #[serde(default)]
+    pub id_base: u32,
+    /// JSON list of the control tokens in id order, ids 0 .. id_base - 1 (`vocabs/tekken_controls.json`), registered as the
+    /// vocabulary's special tokens
+    #[serde(default)]
+    pub controls_path: Option<String>,
 }

@@ -58,6 +58,15 @@ impl Service {
                 Pattern::Tekken => 3,
             };
             native.vocab_load(slot as u32, &file, format, pattern, v.max_ranks).map_err(|e| anyhow::anyhow!("{}: {e}", v.name))?;
+            if v.id_base > 0 {       // the model's own ids: control tokens first, the ordinary tokens after them
+                native.vocab_set_id_base(slot as u32, v.id_base).map_err(|e| anyhow::anyhow!("{}: {e}", v.name))?;
+                if let Some(path) = &v.controls_path {
+                    let controls: Vec<String> = serde_json::from_slice(&std::fs::read(path)?)?;
+                    anyhow::ensure!(controls.len() == v.id_base as usize, "{path}: {} control tokens for id base {}", controls.len(), v.id_base);
+                    let specials: Vec<(String, u32)> = controls.into_iter().zip(0u32..).collect();
+                    native.vocab_set_specials(slot as u32, &specials).map_err(|e| anyhow::anyhow!("{}: {e}", v.name))?;
+                }
+            }
             slots.insert(v.name.clone(), slot as u8);
             for m in &v.models {
                 slots.insert(m.clone(), slot as u8);

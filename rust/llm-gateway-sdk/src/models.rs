@@ -226,6 +226,10 @@ pub enum ChatTemplate {
     /// `message_prefix` (with `{role}`) + content + `message_suffix`, then `generation_prompt`; every string of
     /// `special_tokens` counts one token, the text between two of them is tokenised as ONE stretch of ordinary text
     Rendered { bos: String, message_prefix: String, message_suffix: String, generation_prompt: String, special_tokens: Vec<String> },
+    /// mistral_common's InstructTokenizerV3 on a text-only conversation (Tekken models: Mistral NeMo, Pixtral 12B); the rules are
+    /// those of `cfbpe/plugin.py:mistral_instruct_texts`: system texts join the last user message, runs of one role merge with
+    /// "\n\n", `<s>` + `[INST]` text `[/INST]` per user message + text `</s>` per assistant message, each text encoded on its own
+    Mistral,
 }
 
 /// `gts.x.llmgw.core.usage.v1~` (`llm-gateway-sdk/schemas/core/usage.v1.schema.json:8-12`)

@@ -98,6 +98,7 @@ pub struct ChunkResponse {
 pub enum ChatTemplateDto {
     Overhead { tokens_per_message: u32, tokens_per_name: u32, reply_priming: u32 },
     Rendered { bos: String, message_prefix: String, message_suffix: String, generation_prompt: String, special_tokens: Vec<String> },
+    Mistral,
 }
 
 #[derive(Debug, Deserialize, JsonSchema)]

@@ -92,6 +92,7 @@ pub async fn count_tokens(
                 ChatTemplateDto::Rendered { bos, message_prefix, message_suffix, generation_prompt, special_tokens } => {
                     ChatTemplate::Rendered { bos, message_prefix, message_suffix, generation_prompt, special_tokens }
                 }
+                ChatTemplateDto::Mistral => ChatTemplate::Mistral,
             };
             service.count_chat_tokens(&ctx, &req.model, &req.messages, &template).await
         }

@@ -209,6 +209,47 @@ impl TokenizerClient for TokenizerService {
                 feed(generation_prompt, &mut fixed, &mut run);
                 texts = run;
             }
+            ChatTemplate::Mistral => {
+                let text = |m: &Value| Self::text_parts(std::slice::from_ref(m)).join("\n\n");
+                let bad = |msg: &str| TokenizerError::InvalidInput(msg.to_owned());
+                if messages.is_empty() {
+                    return Err(bad("a conversation for the mistral template has at least one message"));
+                }
+                let system = messages.iter().filter(|m| role(m) == "system").map(text).filter(|t| !t.is_empty()).collect::<Vec<_>>().join("\n\n");
+                let mut turns: Vec<(String, String)> = Vec::new();
+                let mut prev = String::new();
+                for m in messages {
+                    let r = role(m);
+                    match r.as_str() {
+                        "system" if prev == "assistant" => return Err(bad("a system message follows an assistant message")),
+                        "system" => {}
+                        "user" | "assistant" if r == prev => { let last = turns.last_mut().expect("a turn of this role"); last.1.push_str("\n\n"); last.1.push_str(&text(m)); }
+                        "user" | "assistant" => turns.push((r.clone(), text(m))),
+                        _ => return Err(bad("the mistral template counts system, user and assistant messages")),
+                    }
+                    prev = r;
+                }
+                if turns.first().map_or(true, |t| t.0 != "user") {
+                    turns.insert(0, ("user".to_owned(), String::new()));
+                }
+                if turns.last().map_or(true, |t| t.0 != "user") {
+                    return Err(bad("a conversation for the mistral template ends with a user message"));
+                }
+                let last_user = turns.iter().rposition(|t| t.0 == "user").expect("a user turn");
+                fixed = 1;                                                  // <s>
+                for (i, (r, t)) in turns.into_iter().enumerate() {
+                    if r == "user" {
+                        texts.push(if i == last_user && !system.is_empty() { format!("{system}\n\n{t}") } else { t });
+                        fixed += 2;                                         // [INST] [/INST]
+                    } else {
+                        if t.is_empty() {
+                            return Err(bad("an assistant message without text"));
+                        }
+                        texts.push(t.trim_end_matches(' ').to_owned());
+                        fixed += 1;                                         // </s>
+                    }
+                }
+            }
         }
         texts.retain(|t| !t.is_empty());
         if texts.is_empty() {
