@@ -23,6 +23,8 @@ Prompt text is never logged (modules/llm-gateway/docs/DESIGN.md:120-124): only s
 """
 from __future__ import annotations
 
+import json
+import re
 import threading
 import uuid
 from dataclasses import dataclass, field
@@ -320,8 +322,11 @@ class ChatTemplate:
     "rendered"  the conversation is rendered to text around control tokens (Llama 3, Mistral): `bos`, then per message
                 `message_prefix.format(role=...)` + content + `message_suffix`, then `generation_prompt`; the strings in
                 `special_tokens` count one token each, the text between them is tokenised as ordinary text;
-    "mistral"   mistral_common's InstructTokenizerV3 on a text-only conversation (Tekken models: Mistral NeMo, Pixtral 12B):
-                mistral_instruct_texts gives the rules.  Every message's text is tokenised on its own, between control tokens.
+    "mistral"   mistral_common's InstructTokenizerV3 (Tekken models: Mistral NeMo, Pixtral 12B) on a conversation of text, tool
+                calls and tool results, with the request's tools: mistral_instruct_texts gives the rules and the refusals.  Every
+                message's text, the tools' JSON, each assistant turn's calls and each tool result are tokenised on their own, between
+                control tokens ([AVAILABLE_TOOLS] before the last [INST], [TOOL_CALLS], [TOOL_RESULTS]).  The other kinds refuse
+                tools; they pass over tool_call and tool_result parts.
 
     Message CONTENT is always ordinary text: a message that spells a control token gets the pieces of that spelling, never the
     control token (the gateway does not let user text forge framing)."""
@@ -351,53 +356,158 @@ CHAT_TEMPLATES = {
 }
 
 
-def mistral_instruct_texts(messages: Sequence[dict]) -> Tuple[List[str], int]:
-    """A text-only conversation as mistral_common 1.11's InstructTokenizerV3 encodes it (encode_chat_completion with its request
-    normalizer): (the ordinary texts in order, the number of control tokens).  The token count is the control tokens plus the
-    sum of the texts' token counts (Tekkenizer.encode(text, bos=False, eos=False), each text on its own).
+# the roles mistral_common's validator lets follow each role
+MISTRAL_NEXT_ROLES = {"system": ("user", "assistant", "system"), "user": ("assistant", "system", "user"),
+                      "assistant": ("assistant", "user", "tool"), "tool": ("assistant", "tool", "user")}
+# its name and call-id rules, re.match(r"^...$"): "$" also matches before a final "\n", so one trailing "\n" passes
+MISTRAL_NAME = re.compile(r"[a-zA-Z0-9_-]{1,64}\n?")
+MISTRAL_CALL_ID = re.compile(r"[a-zA-Z0-9]{9}\n?")
+
+
+def _mistral_json(value) -> str:
+    """JSON as mistral_common writes it into the prompt: json.dumps(value, ensure_ascii=False)"""
+    return json.dumps(value, ensure_ascii=False)
+
+
+def _mistral_tool_content(content: str):
+    """a tool result's content as mistral_common embeds it: the JSON value when the text parses as JSON, else the text; "" is {}"""
+    if not content:
+        return {}
+    try:
+        return json.loads(content)
+    except json.JSONDecodeError:
+        return content
+
+
+def _mistral_tools(tools: Sequence[dict]) -> List[dict]:
+    """the gateway's tools (schemas/tools/tool.v1) as mistral_common's Tool.model_dump() without `strict`"""
+    out = []
+    for t in tools:
+        if t.get("type") != "unified":
+            raise InvalidInput("the mistral template counts unified tools (name, description, parameters), not %r" % t.get("type"))
+        name, description, params = t.get("name"), t.get("description"), t.get("parameters")
+        schema = params.get("json_schema") if isinstance(params, dict) else None
+        if not isinstance(name, str) or not isinstance(description, str) or not isinstance(schema, dict):
+            raise InvalidInput("a unified tool has a string name and description and parameters {json_schema: object}")
+        if not MISTRAL_NAME.fullmatch(name):
+            raise InvalidInput("a tool name is 1 to 64 of a-z, A-Z, 0-9, '_' and '-'")
+        out.append({"type": "function", "function": {"name": name, "description": description, "parameters": schema}})
+    return out
+
+
+def _mistral_message(m: dict) -> Tuple[str, str, List[dict], Optional[dict]]:
+    """(role, text, tool calls, tool result) of one gateway message; text is its text parts joined with "\n\n", other parts
+    (images ...) are not counted here.  A call is {"name", "arguments", "id"} as mistral_common prints it (no "id" for "null")."""
+    role, parts = m.get("role"), m.get("content", [])
+    if role not in MISTRAL_NEXT_ROLES:
+        raise InvalidInput("the mistral template counts system, user, assistant and tool messages, not %r" % role)
+    text = "\n\n".join(str(p["text"]) for p in parts if p.get("type") == "text")
+    calls, results = [], [p.get("tool_result") for p in parts if p.get("type") == "tool_result"]
+    for p in parts:
+        if p.get("type") != "tool_call":
+            continue
+        c = p.get("tool_call")
+        if role != "assistant" or not isinstance(c, dict):
+            raise InvalidInput("a tool_call part belongs to an assistant message")
+        cid, name, args = c.get("id"), c.get("name"), c.get("arguments")
+        if not isinstance(cid, str) or not isinstance(name, str) or not isinstance(args, dict):
+            raise InvalidInput("a tool call has a string id and name and object arguments")
+        if cid != "null" and not MISTRAL_CALL_ID.fullmatch(cid):
+            raise InvalidInput("a tool call id is 9 of a-z, A-Z and 0-9")
+        if not MISTRAL_NAME.fullmatch(name):
+            raise InvalidInput("a tool call's name is 1 to 64 of a-z, A-Z, 0-9, '_' and '-'")
+        calls.append({"name": name, "arguments": args, **({} if cid == "null" else {"id": cid})})
+    if role == "assistant" and bool(text) == bool(calls):
+        raise InvalidInput("an assistant message holds text or tool calls, one of the two" if text else "an assistant message without text or tool calls")
+    if (role == "tool") != bool(results):
+        raise InvalidInput("a tool_result part belongs to a tool message" if results else "a tool message holds a tool_result part")
+    result = None
+    if role == "tool":
+        r = results[0]
+        if len(results) != 1 or text or not isinstance(r, dict) or not isinstance(r.get("content"), str) \
+                or not isinstance(r.get("tool_call_id"), str):
+            raise InvalidInput("a tool message holds one tool_result {tool_call_id: string, content: string} and no text")
+        if not MISTRAL_CALL_ID.fullmatch(r["tool_call_id"]):
+            raise InvalidInput("a tool result's tool_call_id is 9 of a-z, A-Z and 0-9")
+        result = {"content": _mistral_tool_content(r["content"]), "call_id": r["tool_call_id"]}
+    return role, text, calls, result
+
+
+def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[dict]] = None) -> Tuple[List[str], int]:
+    """A conversation as mistral_common 1.11's InstructTokenizerV3 encodes it (encode_chat_completion with its request validator
+    in its default mode and its request normalizer): (the ordinary texts in order, the number of control tokens).  The token count
+    is the control tokens plus the sum of the texts' token counts (Tekkenizer.encode(text, bos=False, eos=False), each text on its
+    own).  JSON below is json.dumps(..., ensure_ascii=False): ", " and ": " between items, key order kept, non-ASCII as is.
       - a message's text is its text parts joined with "\n\n"; other parts (images ...) are not counted here;
+      - an assistant message holds text or tool_call parts {id, name, arguments}; a tool message holds one tool_result part
+        {tool_call_id, content};
       - system messages leave the sequence; the non-empty system texts, joined with "\n\n", are the system prompt;
-      - consecutive user (or assistant) messages merge into one, their texts joined with "\n\n" (a system message between two
-        messages of one role keeps them apart);
+      - consecutive user (or assistant) messages merge into one, their texts joined with "\n\n" and their tool calls listed in
+        order (a system message between two messages of one role keeps them apart); tool messages stay one each;
       - when the first message left is not a user message, an empty user message goes first;
       - <s>; then per message: user -> [INST] text [/INST], where the LAST user message's text is the system prompt + "\n\n" +
-        its text (when there is a system prompt); assistant -> its text without trailing spaces, then </s>.
-    What mistral_common's validator refuses raises InvalidInput: no message, a system message right after an assistant message,
-    an assistant message last (system messages aside), an assistant message without text."""
-    def text(m):
-        return "\n\n".join(str(p["text"]) for p in m.get("content", []) if p.get("type") == "text")
-    system = "\n\n".join(t for t in (text(m) for m in messages if m.get("role") == "system") if t)
+        its text (when there is a system prompt), and [AVAILABLE_TOOLS] the tools [/AVAILABLE_TOOLS] go before that [INST]
+        (when there are tools: a list of {"type": "function", "function": {"name", "description", "parameters"}});
+        assistant -> its text without trailing spaces, or [TOOL_CALLS] the list of its calls {"name", "arguments", "id"}; then
+        </s>; tool -> [TOOL_RESULTS] {"content": the result, "call_id": its id} [/TOOL_RESULTS], the result being the JSON value
+        its content parses to, else the content as a string ("" is {}).
+    What mistral_common refuses raises InvalidInput: no message; one message that is not a user or system message; an assistant
+    message last; a system message after an assistant or tool message, a tool message after a system or user message; an
+    assistant message without text and tool calls, or with both (also once merged); an assistant message while the tool calls of
+    the one before it do not have exactly one tool message each (the first message is not checked); a tool name or tool-call name
+    that is not 1-64 of [a-zA-Z0-9_-], a call id that is not 9 of [a-zA-Z0-9] (a call id may be "null": it is then not printed);
+    a tool that is not a unified one.  A tool's parameters are taken as a valid JSON Schema (mistral_common checks them against
+    Draft 7; this does not)."""
+    tool_defs = _mistral_tools(tools or ())
     if not messages:
         raise InvalidInput("a conversation for the mistral template has at least one message")
-    turns: List[list] = []              # [role, text] after merging
+    msgs = [_mistral_message(m) for m in messages]
+    roles = [m[0] for m in msgs]
+    if len(roles) == 1 and roles[0] not in ("user", "system"):
+        raise InvalidInput("a conversation of one message for the mistral template is a user or system message")
+    if len(roles) > 1 and roles[-1] == "assistant":
+        raise InvalidInput("a conversation for the mistral template ends with a user or tool message")
+    for prev, role in zip(roles, roles[1:]):
+        if role not in MISTRAL_NEXT_ROLES[prev]:
+            raise InvalidInput("a message of role %r follows one of role %r" % (role, prev))
+    pending = 0                         # tool messages the last tool-calling assistant message still waits for
+    for role, _, calls, _ in msgs[1:]:
+        if role == "tool":
+            pending -= 1
+        elif role == "assistant":
+            if pending:
+                raise InvalidInput("an assistant message follows tool calls without exactly one tool message each")
+            pending = len(calls)
+    system = "\n\n".join(t for role, t, _, _ in msgs if role == "system" and t)
+    turns: List[list] = []              # [role, text, calls, result] after merging
     prev = None
-    for m in messages:
-        role = m.get("role")
-        if role not in ("system", "user", "assistant"):
-            raise InvalidInput("the mistral template counts system, user and assistant messages, not %r" % role)
-        if role == "system" and prev == "assistant":
-            raise InvalidInput("a system message follows an assistant message")
-        if role != "system":
-            if role == prev:
-                turns[-1][1] += "\n\n" + text(m)
-            else:
-                turns.append([role, text(m)])
+    for role, text, calls, result in msgs:
+        if role in ("user", "assistant") and role == prev:
+            if not calls:               # (a message with tool calls has no text to merge)
+                turns[-1][1] += "\n\n" + text
+            turns[-1][2] += calls
+            if turns[-1][1] and turns[-1][2]:
+                raise InvalidInput("merged assistant messages hold both text and tool calls")
+        elif role != "system":
+            turns.append([role, text, list(calls), result])
         prev = role
     if not turns or turns[0][0] != "user":
-        turns.insert(0, ["user", ""])
-    if turns[-1][0] != "user":
-        raise InvalidInput("a conversation for the mistral template ends with a user message")
+        turns.insert(0, ["user", "", [], None])
     last_user = max(i for i, t in enumerate(turns) if t[0] == "user")
     texts, controls = [], 1             # <s>
-    for i, (role, t) in enumerate(turns):
+    for i, (role, t, calls, result) in enumerate(turns):
         if role == "user":
+            if i == last_user and tool_defs:
+                texts.append(_mistral_json(tool_defs))
+                controls += 2           # [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
             texts.append(system + "\n\n" + t if i == last_user and system else t)
             controls += 2               # [INST] [/INST]
+        elif role == "assistant":
+            texts.append(_mistral_json(calls) if calls else t.rstrip(" "))
+            controls += 2 if calls else 1   # ([TOOL_CALLS]) </s>
         else:
-            if not t:
-                raise InvalidInput("an assistant message without text")
-            texts.append(t.rstrip(" "))
-            controls += 1               # </s>
+            texts.append(_mistral_json(result))
+            controls += 2               # [TOOL_RESULTS] [/TOOL_RESULTS]
     return texts, controls
 
 
@@ -909,11 +1019,16 @@ class LlmGatewayTokenizerService:
         counts = self._plugin().count_tokens(ctx, CountTokensRequest(VocabRef(model), data, offs))
         return Usage(int(counts.sum()))
 
-    def count_chat_tokens(self, ctx: SecurityContext, model: str, messages: Sequence[dict], template: ChatTemplate) -> Usage:
+    def count_chat_tokens(self, ctx: SecurityContext, model: str, messages: Sequence[dict], template: ChatTemplate,
+                          tools: Optional[Sequence[dict]] = None) -> Usage:
         """`Usage.input_tokens` of one chat request as the provider counts it: content AND framing (ChatTemplate).
         messages: [{"role": "user", "name": optional, "content": [{"type": "text", "text": ...}, ...]}, ...]; parts that are
-        not text (images ...) are priced elsewhere.  Every stretch of text of the whole request goes to the device in ONE batch."""
+        not text (images ...) are priced elsewhere.  tools: the request's `tools` (schemas/tools/tool.v1), counted by the "mistral"
+        kind only, which also counts tool_call and tool_result parts (mistral_instruct_texts); the other kinds refuse tools and
+        pass over those parts.  Every stretch of text of the whole request, tool JSON included, goes to the device in ONE batch."""
         import re
+        if tools and template.kind != "mistral":
+            raise InvalidInput("the %r chat template does not count tools" % template.kind)
         texts: List[str] = []
         fixed = 0
         if template.kind == "overhead":
@@ -952,7 +1067,7 @@ class LlmGatewayTokenizerService:
             feed_framing(template.generation_prompt)
             texts = [t for t in run if t]
         elif template.kind == "mistral":
-            texts, fixed = mistral_instruct_texts(messages)
+            texts, fixed = mistral_instruct_texts(messages, tools)
         else:
             raise InvalidInput("unknown chat template kind %r" % template.kind)
         texts = [t for t in texts if t]

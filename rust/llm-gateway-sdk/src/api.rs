@@ -41,5 +41,17 @@ pub trait TokenizerClient: Send + Sync {
     /// Pre-call estimate against a remaining budget (`docs/DESIGN.md:833-855`).
     /// `Usage.input_tokens` as the provider counts it: content AND the framing of `template`
     async fn count_chat_tokens(&self, ctx: &SecurityContext, model: &str, messages: &[Value], template: &ChatTemplate) -> Result<Usage, TokenizerError>;
+
+    /// `count_chat_tokens` of a request that also carries `tools` (`schemas/core/request.v1.schema.json`, `tools`): the
+    /// `ChatTemplate::Mistral` kind counts the tool definitions as mistral_common does; the other kinds refuse a non-empty `tools`
+    /// with `InvalidInput`.  This default counts requests without tools only.
+    async fn count_chat_tokens_with_tools(&self, ctx: &SecurityContext, model: &str, messages: &[Value], tools: &[Value], template: &ChatTemplate)
+        -> Result<Usage, TokenizerError> {
+        if !tools.is_empty() {
+            return Err(TokenizerError::InvalidInput("this tokenizer client does not count tools".to_owned()));
+        }
+        self.count_chat_tokens(ctx, model, messages, template).await
+    }
+
     async fn check_budget(&self, ctx: &SecurityContext, model: &str, messages: &[Value], remaining_tokens: u64) -> Result<bool, TokenizerError>;
 }

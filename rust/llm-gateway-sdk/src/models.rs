@@ -226,9 +226,12 @@ pub enum ChatTemplate {
     /// `message_prefix` (with `{role}`) + content + `message_suffix`, then `generation_prompt`; every string of
     /// `special_tokens` counts one token, the text between two of them is tokenised as ONE stretch of ordinary text
     Rendered { bos: String, message_prefix: String, message_suffix: String, generation_prompt: String, special_tokens: Vec<String> },
-    /// mistral_common's InstructTokenizerV3 on a text-only conversation (Tekken models: Mistral NeMo, Pixtral 12B); the rules are
-    /// those of `cfbpe/plugin.py:mistral_instruct_texts`: system texts join the last user message, runs of one role merge with
-    /// "\n\n", `<s>` + `[INST]` text `[/INST]` per user message + text `</s>` per assistant message, each text encoded on its own
+    /// mistral_common's InstructTokenizerV3 (Tekken models: Mistral NeMo, Pixtral 12B) on a conversation of text, tool calls and
+    /// tool results, with the request's tools (`TokenizerClient::count_chat_tokens_with_tools`); the rules and refusals are those
+    /// of `cfbpe/plugin.py:mistral_instruct_texts`: system texts join the last user message, runs of one role merge with "\n\n",
+    /// `<s>` + `[INST]` text `[/INST]` per user message (the tools' JSON between `[AVAILABLE_TOOLS]` and `[/AVAILABLE_TOOLS]`
+    /// before the last one) + text `</s>` or `[TOOL_CALLS]` calls `</s>` per assistant message + `[TOOL_RESULTS]` result
+    /// `[/TOOL_RESULTS]` per tool message, each text and JSON encoded on its own
     Mistral,
 }
 

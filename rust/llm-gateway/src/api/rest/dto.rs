@@ -110,6 +110,10 @@ pub struct CountTokensRequest {
     pub messages: Vec<serde_json::Value>,
     /// the provider's framing; absent: the sum over the text parts
     pub template: Option<ChatTemplateDto>,
+    /// the request's tools (`llm-gateway-sdk/schemas/tools/tool.v1.schema.json`): counted by the `mistral` template (unified tools
+    /// only); any other template, or none, refuses them
+    #[serde(default)]
+    pub tools: Vec<serde_json::Value>,
 }
 
 /// `gts.x.llmgw.core.usage.v1~` restricted to what a pre-call estimate knows

@@ -83,8 +83,9 @@ pub async fn count_tokens(
     Extension(service): Extension<Arc<TokenizerService>>,
     Json(req): Json<CountTokensRequest>,
 ) -> Result<Json<CountTokensResponse>, Problem> {
-    tracing::debug!(model = %req.model, messages = req.messages.len(), "count_tokens");
+    tracing::debug!(model = %req.model, messages = req.messages.len(), tools = req.tools.len(), "count_tokens");
     let usage = match req.template {
+        None if !req.tools.is_empty() => Err(TokenizerError::InvalidInput("tools are counted with the mistral template".to_owned())),
         None => service.count_tokens(&ctx, &req.model, &req.messages).await,
         Some(t) => {
             let template = match t {
@@ -94,7 +95,7 @@ pub async fn count_tokens(
                 }
                 ChatTemplateDto::Mistral => ChatTemplate::Mistral,
             };
-            service.count_chat_tokens(&ctx, &req.model, &req.messages, &template).await
+            service.count_chat_tokens_with_tools(&ctx, &req.model, &req.messages, &req.tools, &template).await
         }
     }
     .map_err(problem)?;

@@ -2,7 +2,8 @@
 //! Plugin resolution is lazy and single-flight (`libs/modkit/src/plugins/mod.rs:44-78`): vendor match, lowest priority wins
 //! (`:136-191`).  Prompt text is never logged (`docs/DESIGN.md:120-124`): only sizes and counts.
 
-use std::sync::Arc;
+use std::io;
+use std::sync::{Arc, LazyLock};
 
 use async_trait::async_trait;
 use bytes::Bytes;
@@ -13,8 +14,95 @@ use llm_gateway_sdk::{
 use modkit::client_hub::{ClientHub, ClientScope};
 use modkit::plugins::{choose_plugin_instance, GtsPluginSelector};
 use modkit_security::SecurityContext;
-use serde_json::Value;
+use regex::Regex;
+use serde::Serialize;
+use serde_json::{json, Value};
 use types_registry_sdk::{ListQuery, TypesRegistryClient};
+
+/// the roles mistral_common's validator lets follow each role (none: not a role the mistral template counts)
+fn mistral_next_roles(role: &str) -> &'static [&'static str] {
+    match role {
+        "system" => &["user", "assistant", "system"],
+        "user" => &["assistant", "system", "user"],
+        "assistant" => &["assistant", "user", "tool"],
+        "tool" => &["assistant", "tool", "user"],
+        _ => &[],
+    }
+}
+
+// mistral_common's name and call-id rules, Python's re.match(r"^...$"): "$" also matches before a final "\n", so one trailing "\n"
+// passes (the regex crate's "$" matches only at the end, hence the explicit "\n?")
+static MISTRAL_NAME: LazyLock<Regex> = LazyLock::new(|| Regex::new(r"^[a-zA-Z0-9_-]{1,64}\n?$").expect("a valid pattern"));
+static MISTRAL_CALL_ID: LazyLock<Regex> = LazyLock::new(|| Regex::new(r"^[a-zA-Z0-9]{9}\n?$").expect("a valid pattern"));
+static NULL: Value = Value::Null;
+
+/// one gateway message as the mistral template reads it: a tool call is `{"name", "arguments"[, "id"]}`, a tool result
+/// `{"content", "call_id"}`
+struct MistralMessage {
+    role: String,
+    text: String,
+    calls: Vec<Value>,
+    result: Option<Value>,
+}
+
+/// JSON as mistral_common writes it into the prompt, Python's `json.dumps(value, ensure_ascii=False)`: ", " and ": " between
+/// items, keys in their order (serde_json's `preserve_order`), non-ASCII as is, floats as Python's `repr`.  Numbers that serde_json
+/// reads otherwise than Python's `json` (NaN, Infinity, -0, integers past 64 bits) are the one known difference from the Python
+/// mirror.
+fn mistral_json(value: &Value) -> String {
+    let mut out = Vec::new();
+    value.serialize(&mut serde_json::Serializer::with_formatter(&mut out, PythonJson)).expect("a Value always serializes");
+    String::from_utf8(out).expect("serde_json writes UTF-8")
+}
+
+/// a tool result's content as mistral_common embeds it: the JSON value when the text parses as JSON, else the text; "" is {}
+fn mistral_tool_content(content: &str) -> Value {
+    if content.is_empty() {
+        return json!({});
+    }
+    serde_json::from_str(content).unwrap_or_else(|_| Value::from(content))
+}
+
+struct PythonJson;
+
+impl serde_json::ser::Formatter for PythonJson {
+    fn begin_array_value<W: ?Sized + io::Write>(&mut self, writer: &mut W, first: bool) -> io::Result<()> {
+        if first { Ok(()) } else { writer.write_all(b", ") }
+    }
+
+    fn begin_object_key<W: ?Sized + io::Write>(&mut self, writer: &mut W, first: bool) -> io::Result<()> {
+        if first { Ok(()) } else { writer.write_all(b", ") }
+    }
+
+    fn begin_object_value<W: ?Sized + io::Write>(&mut self, writer: &mut W) -> io::Result<()> {
+        writer.write_all(b": ")
+    }
+
+    fn write_f64<W: ?Sized + io::Write>(&mut self, writer: &mut W, value: f64) -> io::Result<()> {
+        writer.write_all(python_float_repr(value).as_bytes())
+    }
+}
+
+/// Python's `repr` of a finite float: the shortest digits that read back to it, positional when the decimal exponent is in
+/// -4 ..= 15 (at least one digit after the point), else `d[.ddd]e±XX`
+fn python_float_repr(x: f64) -> String {
+    let sci = format!("{x:e}");                                             // shortest digits: "-1.5e-7", "1e16", "0e0"
+    let (mantissa, exp) = sci.split_once('e').expect("an exponent");
+    let exp: i32 = exp.parse().expect("an integer exponent");
+    let (sign, mantissa) = mantissa.strip_prefix('-').map_or(("", mantissa), |m| ("-", m));
+    if !(-4..16).contains(&exp) {
+        return format!("{sign}{mantissa}e{}{:02}", if exp < 0 { '-' } else { '+' }, exp.abs());
+    }
+    let digits: String = mantissa.chars().filter(|c| *c != '.').collect();
+    let point = exp + 1;                                                    // digits before the decimal point
+    if point <= 0 {
+        format!("{sign}0.{}{digits}", "0".repeat(point.unsigned_abs() as usize))
+    } else if point as usize >= digits.len() {
+        format!("{sign}{digits}{}.0", "0".repeat(point as usize - digits.len()))
+    } else {
+        format!("{sign}{}.{}", &digits[..point as usize], &digits[point as usize..])
+    }
+}
 
 pub struct TokenizerService {
     hub: Arc<ClientHub>,
@@ -73,6 +161,83 @@ impl TokenizerService {
                 .ok_or_else(|| TokenizerError::Internal(format!("the plugin cut text {i} inside a character")))).collect::<Result<Vec<_>, _>>()?;
             Ok((chunks, spans, r.counts[i]))
         }).collect()
+    }
+
+    /// the gateway's tools (`schemas/tools/tool.v1.schema.json`) as mistral_common's `Tool.model_dump()` without `strict`
+    /// (Python mirror: `cfbpe/plugin.py:_mistral_tools`)
+    fn mistral_tools(tools: &[Value]) -> Result<Vec<Value>, TokenizerError> {
+        let bad = |msg: &str| TokenizerError::InvalidInput(msg.to_owned());
+        tools.iter().map(|t| {
+            let kind = t.get("type").and_then(Value::as_str);
+            if kind != Some("unified") {
+                return Err(TokenizerError::InvalidInput(format!("the mistral template counts unified tools (name, description, parameters), not {kind:?}")));
+            }
+            let name = t.get("name").and_then(Value::as_str);
+            let description = t.get("description").and_then(Value::as_str);
+            let schema = t.get("parameters").and_then(|p| p.get("json_schema")).filter(|s| s.is_object());
+            let (Some(name), Some(description), Some(schema)) = (name, description, schema) else {
+                return Err(bad("a unified tool has a string name and description and parameters {json_schema: object}"));
+            };
+            if !MISTRAL_NAME.is_match(name) {
+                return Err(bad("a tool name is 1 to 64 of a-z, A-Z, 0-9, '_' and '-'"));
+            }
+            Ok(json!({"type": "function", "function": {"name": name, "description": description, "parameters": schema}}))
+        }).collect()
+    }
+
+    /// role, text, tool calls and tool result of one gateway message (Python mirror: `cfbpe/plugin.py:_mistral_message`); text is
+    /// its text parts joined with "\n\n", other parts (images ...) are not counted here.  A call is {"name", "arguments", "id"} as
+    /// mistral_common prints it (no "id" for "null").
+    fn mistral_message(m: &Value) -> Result<MistralMessage, TokenizerError> {
+        let bad = |msg: &str| TokenizerError::InvalidInput(msg.to_owned());
+        let role = m.get("role").and_then(Value::as_str).unwrap_or("");
+        if mistral_next_roles(role).is_empty() {
+            return Err(TokenizerError::InvalidInput(format!("the mistral template counts system, user, assistant and tool messages, not {role:?}")));
+        }
+        let parts: &[Value] = m.get("content").and_then(Value::as_array).map_or(&[], Vec::as_slice);
+        let of_type = |p: &&Value, t: &str| p.get("type").and_then(Value::as_str) == Some(t);
+        let text = Self::text_parts(std::slice::from_ref(m)).join("\n\n");
+        let results: Vec<&Value> = parts.iter().filter(|p| of_type(p, "tool_result")).map(|p| p.get("tool_result").unwrap_or(&NULL)).collect();
+        let mut calls = Vec::new();
+        for p in parts.iter().filter(|p| of_type(p, "tool_call")) {
+            let Some(c) = p.get("tool_call").filter(|c| role == "assistant" && c.is_object()) else {
+                return Err(bad("a tool_call part belongs to an assistant message"));
+            };
+            let (id, name, args) = (c.get("id").and_then(Value::as_str), c.get("name").and_then(Value::as_str), c.get("arguments").filter(|a| a.is_object()));
+            let (Some(id), Some(name), Some(args)) = (id, name, args) else {
+                return Err(bad("a tool call has a string id and name and object arguments"));
+            };
+            if id != "null" && !MISTRAL_CALL_ID.is_match(id) {
+                return Err(bad("a tool call id is 9 of a-z, A-Z and 0-9"));
+            }
+            if !MISTRAL_NAME.is_match(name) {
+                return Err(bad("a tool call's name is 1 to 64 of a-z, A-Z, 0-9, '_' and '-'"));
+            }
+            let mut call = json!({"name": name, "arguments": args});
+            if id != "null" {
+                call["id"] = Value::from(id);
+            }
+            calls.push(call);
+        }
+        if role == "assistant" && text.is_empty() == calls.is_empty() {
+            return Err(bad(if text.is_empty() { "an assistant message without text or tool calls" } else { "an assistant message holds text or tool calls, one of the two" }));
+        }
+        if (role == "tool") == results.is_empty() {
+            return Err(bad(if results.is_empty() { "a tool message holds a tool_result part" } else { "a tool_result part belongs to a tool message" }));
+        }
+        let mut result = None;
+        if role == "tool" {
+            let r = results[0];
+            let (content, id) = (r.get("content").and_then(Value::as_str), r.get("tool_call_id").and_then(Value::as_str));
+            let (Some(content), Some(id), 1, true) = (content, id, results.len(), text.is_empty()) else {
+                return Err(bad("a tool message holds one tool_result {tool_call_id: string, content: string} and no text"));
+            };
+            if !MISTRAL_CALL_ID.is_match(id) {
+                return Err(bad("a tool result's tool_call_id is 9 of a-z, A-Z and 0-9"));
+            }
+            result = Some(json!({"content": mistral_tool_content(content), "call_id": id}));
+        }
+        Ok(MistralMessage { role: role.to_owned(), text, calls, result })
     }
 
     /// the `TextContent.text` parts of a request's messages (`schemas/core/message.v1.schema.json`)
@@ -166,7 +331,16 @@ impl TokenizerClient for TokenizerService {
     }
 
     async fn count_chat_tokens(&self, ctx: &SecurityContext, model: &str, messages: &[Value], template: &ChatTemplate) -> Result<Usage, TokenizerError> {
-        // every stretch of ordinary text of the whole request goes to the device in ONE batch; control tokens count one each
+        self.count_chat_tokens_with_tools(ctx, model, messages, &[], template).await
+    }
+
+    async fn count_chat_tokens_with_tools(&self, ctx: &SecurityContext, model: &str, messages: &[Value], tools: &[Value], template: &ChatTemplate)
+        -> Result<Usage, TokenizerError> {
+        // every stretch of ordinary text of the whole request, tool JSON included, goes to the device in ONE batch; control tokens
+        // count one each
+        if !tools.is_empty() && *template != ChatTemplate::Mistral {
+            return Err(TokenizerError::InvalidInput("only the mistral chat template counts tools".to_owned()));
+        }
         let content = |m: &Value| -> String {
             m.get("content").and_then(Value::as_array).map(|parts| {
                 parts.iter().filter(|p| p.get("type").and_then(Value::as_str) == Some("text")).filter_map(|p| p.get("text").and_then(Value::as_str)).collect::<String>()
@@ -210,43 +384,80 @@ impl TokenizerClient for TokenizerService {
                 texts = run;
             }
             ChatTemplate::Mistral => {
-                let text = |m: &Value| Self::text_parts(std::slice::from_ref(m)).join("\n\n");
                 let bad = |msg: &str| TokenizerError::InvalidInput(msg.to_owned());
+                let mut tool_defs = Self::mistral_tools(tools)?;
                 if messages.is_empty() {
                     return Err(bad("a conversation for the mistral template has at least one message"));
                 }
-                let system = messages.iter().filter(|m| role(m) == "system").map(text).filter(|t| !t.is_empty()).collect::<Vec<_>>().join("\n\n");
-                let mut turns: Vec<(String, String)> = Vec::new();
-                let mut prev = String::new();
-                for m in messages {
-                    let r = role(m);
-                    match r.as_str() {
-                        "system" if prev == "assistant" => return Err(bad("a system message follows an assistant message")),
-                        "system" => {}
-                        "user" | "assistant" if r == prev => { let last = turns.last_mut().expect("a turn of this role"); last.1.push_str("\n\n"); last.1.push_str(&text(m)); }
-                        "user" | "assistant" => turns.push((r.clone(), text(m))),
-                        _ => return Err(bad("the mistral template counts system, user and assistant messages")),
+                let msgs = messages.iter().map(Self::mistral_message).collect::<Result<Vec<_>, _>>()?;
+                let roles: Vec<String> = msgs.iter().map(|m| m.role.clone()).collect();
+                if roles.len() == 1 && !matches!(roles[0].as_str(), "user" | "system") {
+                    return Err(bad("a conversation of one message for the mistral template is a user or system message"));
+                }
+                if roles.len() > 1 && roles[roles.len() - 1] == "assistant" {
+                    return Err(bad("a conversation for the mistral template ends with a user or tool message"));
+                }
+                for w in roles.windows(2) {
+                    if !mistral_next_roles(&w[0]).contains(&w[1].as_str()) {
+                        return Err(TokenizerError::InvalidInput(format!("a message of role {:?} follows one of role {:?}", w[1], w[0])));
                     }
-                    prev = r;
                 }
-                if turns.first().map_or(true, |t| t.0 != "user") {
-                    turns.insert(0, ("user".to_owned(), String::new()));
+                let mut pending = 0i64;                                     // tool messages the last tool-calling assistant message still waits for
+                for m in &msgs[1..] {
+                    match m.role.as_str() {
+                        "tool" => pending -= 1,
+                        "assistant" if pending != 0 => return Err(bad("an assistant message follows tool calls without exactly one tool message each")),
+                        "assistant" => pending = m.calls.len() as i64,
+                        _ => {}
+                    }
                 }
-                if turns.last().map_or(true, |t| t.0 != "user") {
-                    return Err(bad("a conversation for the mistral template ends with a user message"));
-                }
-                let last_user = turns.iter().rposition(|t| t.0 == "user").expect("a user turn");
-                fixed = 1;                                                  // <s>
-                for (i, (r, t)) in turns.into_iter().enumerate() {
-                    if r == "user" {
-                        texts.push(if i == last_user && !system.is_empty() { format!("{system}\n\n{t}") } else { t });
-                        fixed += 2;                                         // [INST] [/INST]
-                    } else {
-                        if t.is_empty() {
-                            return Err(bad("an assistant message without text"));
+                let system = msgs.iter().filter(|m| m.role == "system" && !m.text.is_empty()).map(|m| m.text.as_str()).collect::<Vec<_>>().join("\n\n");
+                let mut turns: Vec<MistralMessage> = Vec::new();            // after merging
+                let mut prev = String::new();
+                for m in msgs {
+                    let role = m.role.clone();
+                    if (role == "user" || role == "assistant") && role == prev {
+                        let last = turns.last_mut().expect("a turn of this role");
+                        if m.calls.is_empty() {                             // (a message with tool calls has no text to merge)
+                            last.text.push_str("\n\n");
+                            last.text.push_str(&m.text);
                         }
-                        texts.push(t.trim_end_matches(' ').to_owned());
-                        fixed += 1;                                         // </s>
+                        last.calls.extend(m.calls);
+                        if !last.text.is_empty() && !last.calls.is_empty() {
+                            return Err(bad("merged assistant messages hold both text and tool calls"));
+                        }
+                    } else if role != "system" {
+                        turns.push(m);
+                    }
+                    prev = role;
+                }
+                if turns.first().map_or(true, |t| t.role != "user") {
+                    turns.insert(0, MistralMessage { role: "user".to_owned(), text: String::new(), calls: Vec::new(), result: None });
+                }
+                let last_user = turns.iter().rposition(|t| t.role == "user").expect("a user turn");
+                fixed = 1;                                                  // <s>
+                for (i, t) in turns.into_iter().enumerate() {
+                    match t.role.as_str() {
+                        "user" => {
+                            if i == last_user && !tool_defs.is_empty() {
+                                texts.push(mistral_json(&Value::Array(std::mem::take(&mut tool_defs))));
+                                fixed += 2;                                 // [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
+                            }
+                            texts.push(if i == last_user && !system.is_empty() { format!("{system}\n\n{}", t.text) } else { t.text });
+                            fixed += 2;                                     // [INST] [/INST]
+                        }
+                        "assistant" if !t.calls.is_empty() => {
+                            texts.push(mistral_json(&Value::Array(t.calls)));
+                            fixed += 2;                                     // [TOOL_CALLS] </s>
+                        }
+                        "assistant" => {
+                            texts.push(t.text.trim_end_matches(' ').to_owned());
+                            fixed += 1;                                     // </s>
+                        }
+                        _ => {
+                            texts.push(mistral_json(t.result.as_ref().expect("a tool message has its result")));
+                            fixed += 2;                                     // [TOOL_RESULTS] [/TOOL_RESULTS]
+                        }
                     }
                 }
             }

@@ -6,6 +6,8 @@
   tests/golden/mistral_tekken.npz    Tekkenizer.encode(s, bos=False, eos=False) of tests/mistral_ref.fuzz_texts(), and the token
                                      count of encode_chat_completion of every conversation of tests/mistral_ref.conversations()
                                      (the reference of the Tekken tests on a machine without mistral_common)
+  tests/golden/mistral_tools.npz     the token count of encode_chat_completion of every tool conversation of
+                                     tests/mistral_tools_ref.tool_conversations() with its tools (-1: mistral_common refuses it)
 
   python tools/gen_mistral_data.py
 """
@@ -18,6 +20,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import mistral_ref  # noqa: E402
+import mistral_tools_ref  # noqa: E402
 
 
 def main():
@@ -42,7 +45,12 @@ def main():
         id_offsets=np.concatenate([[0], np.cumsum([len(x) for x in ids])]).astype(np.uint64),
         conversations=np.frombuffer(mistral_ref.conversations_json(convs).encode("utf-8"), dtype=np.uint8),
         conversation_counts=np.asarray([mistral_ref.mistral_count(mt, c) for c in convs], dtype=np.int64))
-    print("wrote vocabs/tekken_controls.json and", os.path.relpath(mistral_ref.GOLDEN, ROOT))
+    tool_convs = mistral_tools_ref.tool_conversations()
+    np.savez_compressed(
+        mistral_tools_ref.GOLDEN,
+        conversations=np.frombuffer(mistral_ref.conversations_json(tool_convs).encode("utf-8"), dtype=np.uint8),
+        conversation_counts=np.asarray([mistral_tools_ref.mistral_count(mt, c, t) for c, t in tool_convs], dtype=np.int64))
+    print("wrote vocabs/tekken_controls.json,", os.path.relpath(mistral_ref.GOLDEN, ROOT), "and", os.path.relpath(mistral_tools_ref.GOLDEN, ROOT))
 
 
 if __name__ == "__main__":
