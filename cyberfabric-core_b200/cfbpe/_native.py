@@ -461,7 +461,7 @@ class Context:
     def truncate_batch_device(self, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_budgets, mode, d_out_cut, d_out_kept,
                               d_out_counts, stream=0):
         """cfbpe_truncate_batch_device on raw device pointers (uint32 budgets, cuts, kept counts, counts: n_prompts each; counts
-        may be None).  Asynchronous: errors come from the next synchronising call or device_status."""
+        may be None).  Asynchronous: its errors come from device_status, called from the same thread before its next device call."""
         self._check(load().cfbpe_truncate_batch_device(self._h, n_prompts, d_bytes, total_bytes, d_offsets, d_vocab_ids, d_budgets,
                                                        mode, d_out_cut, d_out_kept, d_out_counts, stream))
 
@@ -587,6 +587,8 @@ class Context:
         return nt.value if sync else None
 
     def device_status(self, stream=0):
+        """sync `stream` and raise the error of this thread's last device call on this context (sync=False calls report only here);
+        host calls, decode and other threads' calls do not change it"""
         self._check(load().cfbpe_device_status(self._h, stream))
 
     def pinned(self, shape, dtype):

@@ -13,6 +13,7 @@
 #include <mutex>
 #include <string>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/cfbpe.h"
@@ -129,8 +130,6 @@ struct Lane {
     Event ev_list[kMaxPipeChunks];
     Event ev_ws;                         // recorded at the end of an asynchronous device-path call: the workspace is busy until then
     bool ws_pending = false;             // ... and whether one is outstanding
-    uint64_t dev_out_cap = 0;            // out_cap of the last device-path call (cfbpe_device_status reports ENOSPC against it)
-    bool dev_want_ids = false;
     Event ev_scan[kMaxPipeChunks];
     Stream front[kFrontStreams];         // front streams 1.. of a pipelined host call (0 = stream)
     Stream pool[kPrioLevels][kPoolSlots];   // CFBPE_PIPE_PRIO=1|2 (experiment): streams by priority level
@@ -199,6 +198,17 @@ struct DeviceCtx {
 
 struct HostVocab { bool loaded = false; std::vector<uint8_t> h_blob; TablesHeader hdr{}; };
 
+// What cfbpe_device_status reports for one thread on one context: the status word of the thread's last device-path call, copied
+// on the call's stream right after its work (before the lane is free again), so no later call on the lane, from this thread or
+// another, can rewrite it.
+struct DeviceCallRecord {
+    HostPtr<DeviceStatus> status;         // pinned: the copy
+    Event ev;                             // recorded on the call's stream after the copy; made on `device`
+    int device = -1;
+    uint64_t out_cap = 0;                 // the call's out_cap (or chunk_cap): ENOSPC is reported against it ...
+    bool want_ids = false;                // ... when the call returned ids (or chunks)
+};
+
 // the few NCCL entry points the library uses, resolved at cfbpe_create of a multi-device context
 struct NcclApi {
     void* lib = nullptr;
@@ -225,6 +235,8 @@ struct cfbpe_ctx {
     std::atomic<bool> profiling{false};
     NcclApi nccl;
     bool peer_ok = false;      // several devices, each maps the memory of all the others (NVLink): sub-batches may go round-robin
+    std::mutex records_mu;     // guards the map; a record itself is only touched by its thread
+    std::unordered_map<uint64_t, std::unique_ptr<DeviceCallRecord>> records;   // by tl_thread: each thread's last device-path call
 };
 
 namespace {
@@ -233,7 +245,8 @@ namespace {
 thread_local std::string tl_err;
 thread_local cfbpe_profile tl_profile{};
 thread_local bool tl_profile_ready = false;
-thread_local Lane* tl_device_lane = nullptr;      // the lane of this thread's last device-path call (cfbpe_device_status)
+std::atomic<uint64_t> g_threads{0};
+thread_local const uint64_t tl_thread = ++g_threads;   // the calling thread's key in cfbpe_ctx::records (never reused, unlike a thread id)
 
 int fail(cfbpe_ctx*, int code, const std::string& msg) {
     tl_err = msg;
@@ -385,7 +398,7 @@ int install_blob(cfbpe_ctx* ctx, uint32_t vocab_id, std::vector<uint8_t>&& blob)
     return CFBPE_OK;
 }
 
-void fill_profile(Lane* ln, uint64_t n_bytes) {
+void fill_profile(Lane* ln, const DeviceStatus& st, uint64_t n_bytes) {
     cfbpe_profile& p = tl_profile;
     std::memset(&p, 0, sizeof p);
     for (int k = 0; k < CFBPE_NUM_KERNELS; ++k) {
@@ -398,15 +411,15 @@ void fill_profile(Lane* ln, uint64_t n_bytes) {
     if (cudaEventElapsedTime(&ms, ln->prof.h2d[0].get(), ln->prof.h2d[1].get()) == cudaSuccess) p.h2d_ms = ms;
     if (cudaEventElapsedTime(&ms, ln->prof.d2h[0].get(), ln->prof.d2h[1].get()) == cudaSuccess) p.d2h_ms = ms;
     if (cudaEventElapsedTime(&ms, ln->prof.total[0].get(), ln->prof.total[1].get()) == cudaSuccess) p.total_ms = ms;
-    p.n_tokens = ln->h_status->n_tokens;
-    p.n_long_pieces = static_cast<uint64_t>(ln->h_status->n_long) + ln->h_status->n_big;
+    p.n_tokens = st.n_tokens;
+    p.n_long_pieces = static_cast<uint64_t>(st.n_long) + st.n_big;
     p.n_bytes = n_bytes;
-    p.n_long_bytes = ln->h_status->long_bytes;
-    p.n_long_tokens = ln->h_status->long_tokens;
-    p.n_miss_pieces = static_cast<uint64_t>(ln->h_status->miss_n[0]) + ln->h_status->miss_n[1] + ln->h_status->miss_n[2];
-    p.n_list_pieces = ln->h_status->defer_n;
-    p.n_list_parts = ln->h_status->defer_parts;
-    p.n_extra_tokens = ln->h_status->extra_n;
+    p.n_long_bytes = st.long_bytes;
+    p.n_long_tokens = st.long_tokens;
+    p.n_miss_pieces = static_cast<uint64_t>(st.miss_n[0]) + st.miss_n[1] + st.miss_n[2];
+    p.n_list_pieces = st.defer_n;
+    p.n_list_parts = st.defer_parts;
+    p.n_extra_tokens = st.extra_n;
     tl_profile_ready = true;
 }
 
@@ -749,7 +762,7 @@ int run_lane(cfbpe_ctx* ctx, DeviceCtx* dv, Lane* ln, uint32_t n, const uint8_t*
     }
     if (prof) { cudaEventRecord(prof->d2h[1].get(), s); cudaEventRecord(prof->total[1].get(), s); }
     CK(cudaStreamSynchronize(s));
-    if (prof) fill_profile(ln, total);
+    if (prof) fill_profile(ln, *ln->h_status, total);
     return CFBPE_OK;
 }
 
@@ -1341,11 +1354,44 @@ bool load_nccl(NcclApi* n) {
     return n->CommInitAll && n->CommDestroy && n->GroupStart && n->GroupEnd && n->Broadcast && n->AllGather && n->GetErrorString;
 }
 
-// what the lane's last device-path call reports, once its status is in h_status: the status, then ENOSPC against its out_cap
-int device_call_status(cfbpe_ctx* ctx, const Lane* ln) {
-    const DeviceStatus& st = *ln->h_status;
+// what a device-path call reports, once its record's copy has landed: the status, then ENOSPC against its out_cap
+int device_call_status(cfbpe_ctx* ctx, const DeviceCallRecord& rec) {
+    const DeviceStatus& st = *rec.status;
     if (const int rc = fail_status(ctx, st)) return rc;
-    if (ln->dev_want_ids && st.n_tokens > ln->dev_out_cap) return fail_nospace(ctx, st.n_tokens);
+    if (rec.want_ids && st.n_tokens > rec.out_cap) return fail_nospace(ctx, st.n_tokens);
+    return CFBPE_OK;
+}
+
+// the calling thread's record on the context, or nullptr when it has made no device-path call there
+DeviceCallRecord* find_call_record(cfbpe_ctx* ctx) {
+    std::lock_guard<std::mutex> lock(ctx->records_mu);
+    const auto it = ctx->records.find(tl_thread);
+    return it == ctx->records.end() ? nullptr : it->second.get();
+}
+
+// Copy the lane's status into the calling thread's record, on s after the call's work (made on the thread's first device-path call
+// on the context; the caller has selected the lane's device).  s first waits for the record's previous copy, which may be on
+// another lane and stream, so that the copies land in call order.
+int record_device_call(cfbpe_ctx* ctx, int device, Lane* ln, cudaStream_t s, uint64_t out_cap, bool want_ids, DeviceCallRecord** out) {
+    DeviceCallRecord* rec = find_call_record(ctx);
+    if (!rec) {
+        auto r = std::make_unique<DeviceCallRecord>();
+        if (hmalloc(r->status, 1) != cudaSuccess) { cudaGetLastError(); return fail(ctx, CFBPE_ENOMEM, "no pinned memory for the call status"); }
+        std::memset(r->status.get(), 0, sizeof(DeviceStatus));
+        rec = r.get();
+        std::lock_guard<std::mutex> lock(ctx->records_mu);
+        ctx->records.emplace(tl_thread, std::move(r));
+    }
+    if (rec->ev) CK(cudaStreamWaitEvent(s, rec->ev.get(), 0));
+    if (rec->device != device) {             // an event is recorded on a stream of the device it was made on
+        CK(make_event(rec->ev, cudaEventDisableTiming));
+        rec->device = device;
+    }
+    CK(cudaMemcpyAsync(rec->status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaEventRecord(rec->ev.get(), s));
+    rec->out_cap = out_cap;
+    rec->want_ids = want_ids;
+    *out = rec;
     return CFBPE_OK;
 }
 
@@ -1374,20 +1420,18 @@ int device_call(cfbpe_ctx* ctx, uint32_t n_prompts, const uint8_t* d_bytes, uint
     if (ln->ws_pending) CK(cudaStreamWaitEvent(s, ln->ev_ws.get(), 0));
     ProfEvents* prof = profiled && ctx->profiling.load() ? &ln->prof : nullptr;
     if (prof) { std::memset(prof->launched, 0, sizeof prof->launched); cudaEventRecord(prof->total[0].get(), s); cudaEventRecord(prof->h2d[0].get(), s); cudaEventRecord(prof->h2d[1].get(), s); }
-    const int rc = enqueue(dv, ln, BatchView{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes}, s, prof);
+    int rc = enqueue(dv, ln, BatchView{d_bytes, d_offsets, d_vocab_ids, n_prompts, total_bytes}, s, prof);
+    DeviceCallRecord* rec = nullptr;
+    if (!rc) rc = record_device_call(ctx, dv->device, ln, s, out_cap, want_ids, &rec);   // before ev_ws: the status is the call's until then
     if (rc) return rc;
     CK(cudaEventRecord(ln->ev_ws.get(), s));
     ln->ws_pending = true;
-    ln->dev_out_cap = out_cap;
-    ln->dev_want_ids = want_ids;
-    tl_device_lane = ln;
     if (prof) { cudaEventRecord(prof->d2h[0].get(), s); cudaEventRecord(prof->d2h[1].get(), s); cudaEventRecord(prof->total[1].get(), s); }
     if (!n_tokens && !prof) return CFBPE_OK;
-    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    if (prof) fill_profile(ln, total_bytes);
-    if (n_tokens) *n_tokens = ln->h_status->n_tokens;
-    return device_call_status(ctx, ln);
+    if (prof) fill_profile(ln, *rec->status, total_bytes);
+    if (n_tokens) *n_tokens = rec->status->n_tokens;
+    return device_call_status(ctx, *rec);
 }
 
 // shared body of encode_batch_device / encode_batch_starts_device / encode_batch_char_starts_device: d_out_starts (nullable) gets the
@@ -1563,6 +1607,7 @@ void cfbpe_destroy(cfbpe_ctx* ctx) {
         if (dv->comm && ctx->nccl.CommDestroy) ctx->nccl.CommDestroy(dv->comm);
         dv.reset();                          // its lanes, then its tables
     }
+    ctx->records.clear();                    // every thread's device-call record: none outlives the context
     delete ctx;
 }
 
@@ -1887,14 +1932,12 @@ int cfbpe_encode_batch_lossy_device(cfbpe_ctx* ctx, uint32_t n_prompts, const ui
 int cfbpe_device_status(cfbpe_ctx* ctx, void* stream) {
     DeviceGuard restore_device;
     if (!ctx) return CFBPE_EINVAL;
-    Lane* ln = tl_device_lane;      // the lane of this thread's last device-path call
-    if (!ln) return CFBPE_OK;
-    std::lock_guard<std::mutex> lock(ln->mu);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    CK(cudaSetDevice(ln->device));
-    CK(cudaMemcpyAsync(ln->h_status.get(), ln->ws.status, sizeof(DeviceStatus), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return device_call_status(ctx, ln);
+    const DeviceCallRecord* rec = find_call_record(ctx);      // this thread's last device-path call on this context
+    if (!rec) return CFBPE_OK;
+    CK(cudaSetDevice(rec->device));
+    CK(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
+    CK(cudaEventSynchronize(rec->ev.get()));                  // (the call may have run on another stream)
+    return device_call_status(ctx, *rec);
 }
 
 void* cfbpe_host_alloc(cfbpe_ctx* ctx, size_t size) {

@@ -308,8 +308,8 @@ CFBPE_API int cfbpe_encode_batch_special_device(cfbpe_ctx *ctx, uint32_t n_promp
  * default stream).  d_bytes must be readable for 32 bytes past total_bytes (the kernels read whole 16-byte
  * groups); the contents of that padding do not matter.  d_out_ids may be NULL (count only).  n_tokens (host, may be NULL) is written
  * after an internal stream sync; with n_tokens == NULL the call is fully asynchronous and
- * d_out_offsets[n_prompts] holds the total.  Malformed UTF-8 is reported by the next call that
- * synchronises (or cfbpe_device_status). */
+ * d_out_offsets[n_prompts] holds the total.  Then malformed UTF-8 and an out_cap that is too small are reported by
+ * cfbpe_device_status only: no other call reports them, whatever it synchronises. */
 CFBPE_API int cfbpe_encode_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
                               const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t *d_out_ids,
                               uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
@@ -331,8 +331,7 @@ CFBPE_API int cfbpe_encode_batch_char_starts_device(cfbpe_ctx *ctx, uint32_t n_p
 /* cfbpe_truncate_batch on device-resident buffers, enqueued on `stream` as cfbpe_encode_batch_device (d_bytes readable for 32
  * bytes past total_bytes).  d_budgets, d_out_cut, d_out_kept and d_out_counts (may be NULL) are device memory.  Fully
  * asynchronous: nothing has to come back to the host, and the ids, which never exceed max_batch_bytes, stay in the lane's
- * buffers (no CFBPE_ENOSPC).  Malformed UTF-8 and an unloaded vocabulary are reported by the next call that synchronises (or
- * cfbpe_device_status). */
+ * buffers (no CFBPE_ENOSPC).  Malformed UTF-8 and an unloaded vocabulary are reported by cfbpe_device_status only. */
 CFBPE_API int cfbpe_truncate_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
                                           const uint64_t *d_offsets, const uint8_t *d_vocab_ids, const uint32_t *d_budgets, uint32_t mode,
                                           uint32_t *d_out_cut, uint32_t *d_out_kept, uint32_t *d_out_counts, void *stream);
@@ -340,8 +339,8 @@ CFBPE_API int cfbpe_truncate_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, co
  * past total_bytes).  d_out_spans (room for chunk_cap chunks), d_out_chunk_offsets and d_out_counts (may be NULL) are device
  * memory.  n_chunks (host, may be NULL) is written after an internal stream sync, and then CFBPE_ENOSPC is returned when the
  * chunks exceed chunk_cap; with n_chunks == NULL the call is fully asynchronous, d_out_chunk_offsets[n_prompts] holds the total,
- * and CFBPE_ENOSPC, malformed UTF-8 and an unloaded vocabulary are reported by the next call that synchronises (or
- * cfbpe_device_status).  Chunks at or past chunk_cap are not written. */
+ * and CFBPE_ENOSPC, malformed UTF-8 and an unloaded vocabulary are reported by cfbpe_device_status only.  Chunks at or past
+ * chunk_cap are not written. */
 CFBPE_API int cfbpe_chunk_batch_device(cfbpe_ctx *ctx, uint32_t n_prompts, const uint8_t *d_bytes, uint64_t total_bytes,
                                        const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t chunk_tokens,
                                        uint32_t overlap_tokens, uint32_t *d_out_spans, uint64_t chunk_cap,
@@ -378,7 +377,13 @@ CFBPE_API int cfbpe_encode_batch_lossy_device(cfbpe_ctx *ctx, uint32_t n_prompts
                                               const uint64_t *d_offsets, const uint8_t *d_vocab_ids, uint32_t *d_out_ids,
                                               uint64_t out_cap, uint64_t *d_out_offsets, uint32_t *d_out_counts,
                                               uint32_t *d_out_replaced, uint64_t *n_tokens, void *stream);
-/* Synchronise `stream` and return the status word of the last device call (0, CFBPE_EILSEQ, CFBPE_ENOSPC). */
+/* Synchronise `stream`, wait for the CALLING THREAD's last device-path call (cfbpe_*_device) on this context, and return that
+ * call's status: 0, CFBPE_EILSEQ, CFBPE_ENOENT (an unloaded vocabulary) or CFBPE_ENOSPC (against its out_cap or chunk_cap); 0
+ * when the thread has made none there.  Only a later device-path call of the same thread on the same context replaces it: host
+ * calls, decode, other threads' calls and calls on other contexts do not.  A device-path call that fails before its work is
+ * queued (a bad argument, a disallowed special token, a repaired batch that does not fit) replaces nothing.  Each device-path
+ * call copies its status into a record of the thread when its work ends (one small device-to-host copy on its stream); the
+ * context frees the records in cfbpe_destroy. */
 CFBPE_API int cfbpe_device_status(cfbpe_ctx *ctx, void *stream);
 
 /* page-locked host memory the DMA engines can read without a staging copy */
