@@ -322,11 +322,12 @@ class ChatTemplate:
     "rendered"  the conversation is rendered to text around control tokens (Llama 3, Mistral): `bos`, then per message
                 `message_prefix.format(role=...)` + content + `message_suffix`, then `generation_prompt`; the strings in
                 `special_tokens` count one token each, the text between them is tokenised as ordinary text;
-    "mistral"   mistral_common's InstructTokenizerV3 (Tekken models: Mistral NeMo, Pixtral 12B) on a conversation of text, tool
-                calls and tool results, with the request's tools: mistral_instruct_texts gives the rules and the refusals.  Every
-                message's text, the tools' JSON, each assistant turn's calls and each tool result are tokenised on their own, between
-                control tokens ([AVAILABLE_TOOLS] before the last [INST], [TOOL_CALLS], [TOOL_RESULTS]).  The other kinds refuse
-                tools; they pass over tool_call and tool_result parts.
+    "mistral"   mistral_common's InstructTokenizer of `instruct_version` 3 (Tekken models: Mistral NeMo, Pixtral 12B) or 7 (Mistral
+                Large 2411, Pixtral Large 2411, Mistral Small 2501 and 2503) on a conversation of text, tool calls and tool results,
+                with the request's tools: mistral_instruct_texts gives the rules and the refusals.  Every message's text, the tools'
+                JSON, each assistant turn's calls and each tool result are tokenised on their own, between control tokens
+                ([AVAILABLE_TOOLS] before the last [INST], [TOOL_CALLS], [TOOL_RESULTS]; V7 also [SYSTEM_PROMPT], [TOOL_CONTENT]).
+                The other kinds refuse tools; they pass over tool_call and tool_result parts.
 
     Message CONTENT is always ordinary text: a message that spells a control token gets the pieces of that spelling, never the
     control token (the gateway does not let user text forge framing)."""
@@ -339,6 +340,7 @@ class ChatTemplate:
     message_suffix: str = ""
     generation_prompt: str = ""
     special_tokens: Tuple[str, ...] = ()
+    instruct_version: int = 3           # "mistral": mistral_common's instruct tokenizer version, 3 or 7
 
 
 # templates of the model families the stand-in vocabularies cover; a deployment lists its own next to the model's tokenizer
@@ -349,6 +351,9 @@ CHAT_TEMPLATES = {
     # Meta Llama 3 instruct
     # Mistral's Tekken models (mistral_common InstructTokenizerV3): <s>, then [INST] user [/INST] and assistant </s>
     "mistral-v3": ChatTemplate("mistral"),
+    # Mistral's V7 Tekken models (InstructTokenizerV7): system messages in place as [SYSTEM_PROMPT] text [/SYSTEM_PROMPT], tool
+    # results as [TOOL_RESULTS] call id [TOOL_CONTENT] content [/TOOL_RESULTS]
+    "mistral-v7": ChatTemplate("mistral", instruct_version=7),
     "llama3-instruct": ChatTemplate("rendered", bos="<|begin_of_text|>",
                                     message_prefix="<|start_header_id|>{role}<|end_header_id|>\n\n", message_suffix="<|eot_id|>",
                                     generation_prompt="<|start_header_id|>assistant<|end_header_id|>\n\n",
@@ -379,6 +384,17 @@ def _mistral_tool_content(content: str):
         return content
 
 
+def _mistral_normalized_content(content: str) -> str:
+    """a tool result's content as mistral_common's V7 request normalizer leaves it: the JSON value it parses to, written again by
+    _mistral_json, else the text as given; "" is "{}" """
+    if not content:
+        return "{}"
+    try:
+        return _mistral_json(json.loads(content))
+    except json.JSONDecodeError:
+        return content
+
+
 def _mistral_tools(tools: Sequence[dict]) -> List[dict]:
     """the gateway's tools (schemas/tools/tool.v1) as mistral_common's Tool.model_dump() without `strict`"""
     out = []
@@ -395,13 +411,18 @@ def _mistral_tools(tools: Sequence[dict]) -> List[dict]:
     return out
 
 
-def _mistral_message(m: dict) -> Tuple[str, str, List[dict], Optional[dict]]:
-    """(role, text, tool calls, tool result) of one gateway message; text is its text parts joined with "\n\n", other parts
-    (images ...) are not counted here.  A call is {"name", "arguments", "id"} as mistral_common prints it (no "id" for "null")."""
+def _mistral_message(m: dict, version: int = 3) -> Tuple[str, List[str], List[dict], Optional[Tuple[str, str]], bool]:
+    """(role, text parts, tool calls, tool result (call id, content), prefix) of one gateway message; other parts (images ...)
+    are not counted here.  A call is {"name", "arguments", "id"} as mistral_common prints it (no "id" for "null").  prefix is
+    the `prefix` flag of an assistant message (Mistral's chat API: the reply continues this message), read under V7 only."""
     role, parts = m.get("role"), m.get("content", [])
     if role not in MISTRAL_NEXT_ROLES:
         raise InvalidInput("the mistral template counts system, user, assistant and tool messages, not %r" % role)
-    text = "\n\n".join(str(p["text"]) for p in parts if p.get("type") == "text")
+    texts = [str(p["text"]) for p in parts if p.get("type") == "text"]
+    text = "\n\n".join(texts)
+    prefix = m.get("prefix", False) if version == 7 else False
+    if not isinstance(prefix, bool) or (prefix and role != "assistant"):
+        raise InvalidInput("prefix is a boolean of an assistant message")
     calls, results = [], [p.get("tool_result") for p in parts if p.get("type") == "tool_result"]
     for p in parts:
         if p.get("type") != "tool_call":
@@ -417,7 +438,7 @@ def _mistral_message(m: dict) -> Tuple[str, str, List[dict], Optional[dict]]:
         if not MISTRAL_NAME.fullmatch(name):
             raise InvalidInput("a tool call's name is 1 to 64 of a-z, A-Z, 0-9, '_' and '-'")
         calls.append({"name": name, "arguments": args, **({} if cid == "null" else {"id": cid})})
-    if role == "assistant" and bool(text) == bool(calls):
+    if version == 3 and role == "assistant" and bool(text) == bool(calls):     # (V7: text, calls or both, once merged)
         raise InvalidInput("an assistant message holds text or tool calls, one of the two" if text else "an assistant message without text or tool calls")
     if (role == "tool") != bool(results):
         raise InvalidInput("a tool_result part belongs to a tool message" if results else "a tool message holds a tool_result part")
@@ -429,15 +450,16 @@ def _mistral_message(m: dict) -> Tuple[str, str, List[dict], Optional[dict]]:
             raise InvalidInput("a tool message holds one tool_result {tool_call_id: string, content: string} and no text")
         if not MISTRAL_CALL_ID.fullmatch(r["tool_call_id"]):
             raise InvalidInput("a tool result's tool_call_id is 9 of a-z, A-Z and 0-9")
-        result = {"content": _mistral_tool_content(r["content"]), "call_id": r["tool_call_id"]}
-    return role, text, calls, result
+        result = (r["tool_call_id"], r["content"])
+    return role, texts, calls, result, prefix
 
 
-def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[dict]] = None) -> Tuple[List[str], int]:
-    """A conversation as mistral_common 1.11's InstructTokenizerV3 encodes it (encode_chat_completion with its request validator
-    in its default mode and its request normalizer): (the ordinary texts in order, the number of control tokens).  The token count
-    is the control tokens plus the sum of the texts' token counts (Tekkenizer.encode(text, bos=False, eos=False), each text on its
-    own).  JSON below is json.dumps(..., ensure_ascii=False): ", " and ": " between items, key order kept, non-ASCII as is.
+def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[dict]] = None, version: int = 3) -> Tuple[List[str], int]:
+    """A conversation as mistral_common 1.11's InstructTokenizerV3 (version 3) or InstructTokenizerV7 (version 7) encodes it
+    (encode_chat_completion with its request validator in its default mode and its request normalizer): (the ordinary texts in
+    order, the number of control tokens).  The token count is the control tokens plus the sum of the texts' token counts
+    (Tekkenizer.encode(text, bos=False, eos=False), each text on its own).  JSON below is json.dumps(..., ensure_ascii=False):
+    ", " and ": " between items, key order kept, non-ASCII as is.  Version 3:
       - a message's text is its text parts joined with "\n\n"; other parts (images ...) are not counted here;
       - an assistant message holds text or tool_call parts {id, name, arguments}; a tool message holds one tool_result part
         {tool_call_id, content};
@@ -457,31 +479,54 @@ def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[di
     the one before it do not have exactly one tool message each (the first message is not checked); a tool name or tool-call name
     that is not 1-64 of [a-zA-Z0-9_-], a call id that is not 9 of [a-zA-Z0-9] (a call id may be "null": it is then not printed);
     a tool that is not a unified one.  A tool's parameters are taken as a valid JSON Schema (mistral_common checks them against
-    Draft 7; this does not)."""
+    Draft 7; this does not).
+
+    Version 7 (MistralRequestValidatorV5, InstructRequestNormalizerV7) keeps the roles that may follow each role, the names, the
+    call ids, the count of tool messages and the calls' JSON, and differs in this:
+      - each system message stays where it is, as [SYSTEM_PROMPT] its text [/SYSTEM_PROMPT] (an empty one too); system messages
+        in a row stay one each; nothing joins the user messages, and no empty user message goes first;
+      - consecutive user (or assistant) messages merge into one whose text is all their text parts joined with "\n\n" (a message
+        without text parts adds nothing);
+      - an assistant message may hold text and tool calls: its turn is its text without trailing spaces, then [TOOL_CALLS] the
+        list of its calls, then </s>; a turn with neither is refused (a message with neither passes when merged with one that
+        has either);
+      - tool -> [TOOL_RESULTS] call id [TOOL_CONTENT] content [/TOOL_RESULTS], the content being the JSON value it parses to
+        written again, else the text as given ("" is "{}");
+      - the last message may be an assistant message with "prefix": true, the start of the reply: its turn has no </s>.  prefix on
+        any other message is refused;
+      - the tools go before the last user message's [INST]; a conversation without a user message does not show them."""
+    if version not in (3, 7):
+        raise InvalidInput("the mistral template counts instruct versions 3 and 7, not %r" % (version,))
     tool_defs = _mistral_tools(tools or ())
     if not messages:
         raise InvalidInput("a conversation for the mistral template has at least one message")
-    msgs = [_mistral_message(m) for m in messages]
+    msgs = [_mistral_message(m, version) for m in messages]
     roles = [m[0] for m in msgs]
+    if any(m[4] for m in msgs[:-1]):
+        raise InvalidInput("an assistant message with prefix is the last message")
     if len(roles) == 1 and roles[0] not in ("user", "system"):
         raise InvalidInput("a conversation of one message for the mistral template is a user or system message")
-    if len(roles) > 1 and roles[-1] == "assistant":
-        raise InvalidInput("a conversation for the mistral template ends with a user or tool message")
+    if len(roles) > 1 and roles[-1] == "assistant" and not msgs[-1][4]:
+        raise InvalidInput("a conversation for the mistral template ends with a user or tool message" +
+                           (" or an assistant message with prefix" if version == 7 else ""))
     for prev, role in zip(roles, roles[1:]):
         if role not in MISTRAL_NEXT_ROLES[prev]:
             raise InvalidInput("a message of role %r follows one of role %r" % (role, prev))
     pending = 0                         # tool messages the last tool-calling assistant message still waits for
-    for role, _, calls, _ in msgs[1:]:
+    for role, _, calls, _, _ in msgs[1:]:
         if role == "tool":
             pending -= 1
         elif role == "assistant":
             if pending:
                 raise InvalidInput("an assistant message follows tool calls without exactly one tool message each")
             pending = len(calls)
-    system = "\n\n".join(t for role, t, _, _ in msgs if role == "system" and t)
+    if version == 7:
+        return _mistral_v7_texts(msgs, tool_defs)
+    system = "\n\n".join(t for t in ("\n\n".join(parts) for role, parts, _, _, _ in msgs if role == "system") if t)
     turns: List[list] = []              # [role, text, calls, result] after merging
     prev = None
-    for role, text, calls, result in msgs:
+    for role, parts, calls, result, _ in msgs:
+        text = "\n\n".join(parts)
         if role in ("user", "assistant") and role == prev:
             if not calls:               # (a message with tool calls has no text to merge)
                 turns[-1][1] += "\n\n" + text
@@ -506,8 +551,50 @@ def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[di
             texts.append(_mistral_json(calls) if calls else t.rstrip(" "))
             controls += 2 if calls else 1   # ([TOOL_CALLS]) </s>
         else:
-            texts.append(_mistral_json(result))
+            call_id, content = result
+            texts.append(_mistral_json({"content": _mistral_tool_content(content), "call_id": call_id}))
             controls += 2               # [TOOL_RESULTS] [/TOOL_RESULTS]
+    return texts, controls
+
+
+def _mistral_v7_texts(msgs: Sequence[tuple], tool_defs: List[dict]) -> Tuple[List[str], int]:
+    """mistral_instruct_texts under version 7, on messages _mistral_message read and mistral_instruct_texts checked"""
+    turns: List[list] = []              # [role, text parts, calls, result] after merging
+    prev = None
+    for role, parts, calls, result, _ in msgs:
+        if role in ("user", "assistant") and role == prev:
+            turns[-1][1] += parts
+            turns[-1][2] += calls
+        else:
+            turns.append([role, list(parts), list(calls), result])
+        prev = role
+    last_user = max((i for i, t in enumerate(turns) if t[0] == "user"), default=-1)
+    prefix = msgs[-1][4]
+    texts, controls = [], 1             # <s>
+    for i, (role, parts, calls, result) in enumerate(turns):
+        text = "\n\n".join(parts)
+        if role == "system":
+            texts.append(text)
+            controls += 2               # [SYSTEM_PROMPT] [/SYSTEM_PROMPT]
+        elif role == "user":
+            if i == last_user and tool_defs:
+                texts.append(_mistral_json(tool_defs))
+                controls += 2           # [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
+            texts.append(text)
+            controls += 2               # [INST] [/INST]
+        elif role == "assistant":
+            if not text and not calls:
+                raise InvalidInput("an assistant message without text or tool calls (also once merged)")
+            texts.append(text.rstrip(" "))
+            if calls:
+                texts.append(_mistral_json(calls))
+                controls += 1           # [TOOL_CALLS]
+            if not (prefix and i == len(turns) - 1):
+                controls += 1           # </s>
+        else:
+            call_id, content = result
+            texts += [call_id, _mistral_normalized_content(content)]
+            controls += 3               # [TOOL_RESULTS] [TOOL_CONTENT] [/TOOL_RESULTS]
     return texts, controls
 
 
@@ -1024,8 +1111,8 @@ class LlmGatewayTokenizerService:
         """`Usage.input_tokens` of one chat request as the provider counts it: content AND framing (ChatTemplate).
         messages: [{"role": "user", "name": optional, "content": [{"type": "text", "text": ...}, ...]}, ...]; parts that are
         not text (images ...) are priced elsewhere.  tools: the request's `tools` (schemas/tools/tool.v1), counted by the "mistral"
-        kind only, which also counts tool_call and tool_result parts (mistral_instruct_texts); the other kinds refuse tools and
-        pass over those parts.  Every stretch of text of the whole request, tool JSON included, goes to the device in ONE batch."""
+        kind only, which also counts tool_call and tool_result parts (mistral_instruct_texts, by the template's instruct version);
+        the other kinds refuse tools and pass over those parts.  Every stretch of text of the whole request, tool JSON included, goes to the device in ONE batch."""
         import re
         if tools and template.kind != "mistral":
             raise InvalidInput("the %r chat template does not count tools" % template.kind)
@@ -1067,7 +1154,7 @@ class LlmGatewayTokenizerService:
             feed_framing(template.generation_prompt)
             texts = [t for t in run if t]
         elif template.kind == "mistral":
-            texts, fixed = mistral_instruct_texts(messages, tools)
+            texts, fixed = mistral_instruct_texts(messages, tools, template.instruct_version)
         else:
             raise InvalidInput("unknown chat template kind %r" % template.kind)
         texts = [t for t in texts if t]

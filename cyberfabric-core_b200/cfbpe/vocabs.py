@@ -16,6 +16,9 @@ The "tekken" vocabulary speaks raw ranks 0..n-1 of the rank file (the stand-in s
 (<unk> 0, <s> 1, </s> 2, [INST] 3, [/INST] 4, ...; vocabs/tekken_controls.json) and the ordinary token of rank r at id 1000 + r
 (the plugin loads it with cfbpe_vocab_set_id_base(1000) and registers the control tokens as its special tokens).  Mistral NeMo's
 tekken_240718 and Pixtral's tekken_240911 hold the same first 130072 ranks, so both models use the committed 240911 file.
+Mistral's instruct-V7 models (Large 2411, Pixtral Large 2411, Small 2501 and 2503) map to "mistral_tekken" too, as a stand-in:
+their own tekken.json files are not here (MODEL_TOKENIZERS labels them stand_in=True).  A model's chat template sits in its
+MODEL_TOKENIZERS entry, beside its vocabulary, so the gateway never infers it from the model's name.
 """
 import hashlib
 import json
@@ -55,13 +58,34 @@ SPECS = {
     "mistral_tekken": VocabSpec("mistral_tekken", "tekken", 130072, "tekken_240911.tiktoken", id_base=1000, controls="tekken_controls.json"),
 }
 
-# canonical model id -> vocab (provider_slug::provider_model_id, modules/model-registry/docs/PRD.md:197)
-MODEL_VOCABS = {
-    "openai::gpt-4": "cl100k_base", "openai::gpt-3.5-turbo": "cl100k_base", "openai::text-embedding-3-small": "cl100k_base",
-    "openai::gpt-4o": "o200k_base", "openai::gpt-4o-mini": "o200k_base", "openai::o1": "o200k_base",
-    "meta::llama-3-8b-instruct": "llama3", "meta::llama-3.1-70b-instruct": "llama3",
-    "mistral::mistral-nemo": "mistral_tekken", "mistral::pixtral-12b": "mistral_tekken",
+@dataclass(frozen=True)
+class ModelTokenizer:
+    """How the gateway counts one model's requests: the vocabulary (SPECS) and the chat template (plugin.CHAT_TEMPLATES; "" when
+    none is registered for the model) that frames its conversations.  stand_in: the vocabulary is not the model's own tokenizer
+    file but stands in for it, so its counts are the stand-in's and may differ from the provider's."""
+    vocab: str
+    chat_template: str = ""
+    stand_in: bool = False
+
+
+# canonical model id -> its tokenizer (provider_slug::provider_model_id, modules/model-registry/docs/PRD.md:197)
+MODEL_TOKENIZERS = {
+    "openai::gpt-4": ModelTokenizer("cl100k_base"), "openai::gpt-3.5-turbo": ModelTokenizer("cl100k_base"),
+    "openai::text-embedding-3-small": ModelTokenizer("cl100k_base"),
+    "openai::gpt-4o": ModelTokenizer("o200k_base"), "openai::gpt-4o-mini": ModelTokenizer("o200k_base"), "openai::o1": ModelTokenizer("o200k_base"),
+    "meta::llama-3-8b-instruct": ModelTokenizer("llama3"), "meta::llama-3.1-70b-instruct": ModelTokenizer("llama3"),
+    # instruct V3: their own tekken files hold the committed file's first 130072 ranks
+    "mistral::mistral-nemo": ModelTokenizer("mistral_tekken", "mistral-v3"),
+    "mistral::pixtral-12b": ModelTokenizer("mistral_tekken", "mistral-v3"),
+    # instruct V7: STAND-IN -- their own tekken.json files are not in this repository; tekken_240911 and its control tokens stand
+    # in for them (the V7 rules are checked against mistral_common on tekken_240911, not on these models' files)
+    "mistral::mistral-large-2411": ModelTokenizer("mistral_tekken", "mistral-v7", stand_in=True),
+    "mistral::pixtral-large-2411": ModelTokenizer("mistral_tekken", "mistral-v7", stand_in=True),
+    "mistral::mistral-small-2501": ModelTokenizer("mistral_tekken", "mistral-v7", stand_in=True),
+    "mistral::mistral-small-2503": ModelTokenizer("mistral_tekken", "mistral-v7", stand_in=True),
 }
+# canonical model id -> vocab
+MODEL_VOCABS = {model: t.vocab for model, t in MODEL_TOKENIZERS.items()}
 
 
 @dataclass
@@ -132,7 +156,12 @@ def resolve(name: str, allow_stand_in: bool = False) -> ResolvedVocab:
 
 def for_model(canonical_id: str) -> str:
     """vocab name for a model-registry canonical id; VocabUnavailable if the model is unknown"""
+    return tokenizer_for_model(canonical_id).vocab
+
+
+def tokenizer_for_model(canonical_id: str) -> ModelTokenizer:
+    """vocabulary, chat template and stand-in flag of a model-registry canonical id; VocabUnavailable if the model is unknown"""
     try:
-        return MODEL_VOCABS[canonical_id]
+        return MODEL_TOKENIZERS[canonical_id]
     except KeyError:
         raise VocabUnavailable("no vocabulary is registered for model %r" % canonical_id) from None

@@ -226,13 +226,45 @@ pub enum ChatTemplate {
     /// `message_prefix` (with `{role}`) + content + `message_suffix`, then `generation_prompt`; every string of
     /// `special_tokens` counts one token, the text between two of them is tokenised as ONE stretch of ordinary text
     Rendered { bos: String, message_prefix: String, message_suffix: String, generation_prompt: String, special_tokens: Vec<String> },
-    /// mistral_common's InstructTokenizerV3 (Tekken models: Mistral NeMo, Pixtral 12B) on a conversation of text, tool calls and
-    /// tool results, with the request's tools (`TokenizerClient::count_chat_tokens_with_tools`); the rules and refusals are those
-    /// of `cfbpe/plugin.py:mistral_instruct_texts`: system texts join the last user message, runs of one role merge with "\n\n",
+    /// mistral_common's instruct tokenizer of version `instruct` (Tekken models) on a conversation of text, tool calls and tool
+    /// results, with the request's tools (`TokenizerClient::count_chat_tokens_with_tools`); the rules and refusals are those of
+    /// `cfbpe/plugin.py:mistral_instruct_texts`.  V3: system texts join the last user message, runs of one role merge with "\n\n",
     /// `<s>` + `[INST]` text `[/INST]` per user message (the tools' JSON between `[AVAILABLE_TOOLS]` and `[/AVAILABLE_TOOLS]`
     /// before the last one) + text `</s>` or `[TOOL_CALLS]` calls `</s>` per assistant message + `[TOOL_RESULTS]` result
-    /// `[/TOOL_RESULTS]` per tool message, each text and JSON encoded on its own
-    Mistral,
+    /// `[/TOOL_RESULTS]` per tool message, each text and JSON encoded on its own.  V7: see [`MistralInstruct::V7`]
+    Mistral { instruct: MistralInstruct },
+}
+
+impl ChatTemplate {
+    /// the templates of the model families the stand-in vocabularies cover, by name (Python mirror: `cfbpe/plugin.py:CHAT_TEMPLATES`)
+    pub fn named(name: &str) -> Option<Self> {
+        match name {
+            "openai-chatml" => Some(Self::Overhead { tokens_per_message: 3, tokens_per_name: 1, reply_priming: 3 }),
+            "mistral-v3" => Some(Self::Mistral { instruct: MistralInstruct::V3 }),
+            "mistral-v7" => Some(Self::Mistral { instruct: MistralInstruct::V7 }),
+            "llama3-instruct" => Some(Self::Rendered {
+                bos: "<|begin_of_text|>".to_owned(),
+                message_prefix: "<|start_header_id|>{role}<|end_header_id|>\n\n".to_owned(),
+                message_suffix: "<|eot_id|>".to_owned(),
+                generation_prompt: "<|start_header_id|>assistant<|end_header_id|>\n\n".to_owned(),
+                special_tokens: ["<|begin_of_text|>", "<|start_header_id|>", "<|end_header_id|>", "<|eot_id|>"].map(str::to_owned).to_vec(),
+            }),
+            _ => None,
+        }
+    }
+}
+
+/// mistral_common's instruct tokenizer version of `ChatTemplate::Mistral` (Python: `ChatTemplate.instruct_version`)
+#[derive(Debug, Clone, Copy, Default, PartialEq, Eq)]
+pub enum MistralInstruct {
+    /// InstructTokenizerV3 (Mistral NeMo, Pixtral 12B)
+    #[default]
+    V3,
+    /// InstructTokenizerV7 (Mistral Large 2411, Pixtral Large 2411, Mistral Small 2501 and 2503): each system message stays in
+    /// place as `[SYSTEM_PROMPT]` text `[/SYSTEM_PROMPT]`; an assistant turn may hold text and then `[TOOL_CALLS]` calls; a tool
+    /// result is `[TOOL_RESULTS]` call id `[TOOL_CONTENT]` content `[/TOOL_RESULTS]` (the content's JSON written again, else as
+    /// given, "" as "{}"); a last assistant message with `"prefix": true` has no `</s>`
+    V7,
 }
 
 /// `gts.x.llmgw.core.usage.v1~` (`llm-gateway-sdk/schemas/core/usage.v1.schema.json:8-12`)

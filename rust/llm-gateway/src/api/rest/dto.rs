@@ -92,13 +92,29 @@ pub struct ChunkResponse {
     pub counts: Vec<u32>,
 }
 
-/// How the provider frames the messages (`llm_gateway_sdk::ChatTemplate`); absent: content only.
+/// How the provider frames the messages (`llm_gateway_sdk::ChatTemplate`): a template's name (`ChatTemplate::named`:
+/// "openai-chatml", "mistral-v3", "mistral-v7", "llama3-instruct") or the template spelled out; absent: content only.
+#[derive(Debug, Deserialize, JsonSchema)]
+#[serde(untagged)]
+pub enum TemplateDto {
+    Named(String),
+    Spec(ChatTemplateDto),
+}
+
 #[derive(Debug, Deserialize, JsonSchema)]
 #[serde(tag = "kind", rename_all = "snake_case", deny_unknown_fields)]
 pub enum ChatTemplateDto {
     Overhead { tokens_per_message: u32, tokens_per_name: u32, reply_priming: u32 },
     Rendered { bos: String, message_prefix: String, message_suffix: String, generation_prompt: String, special_tokens: Vec<String> },
-    Mistral,
+    Mistral {
+        /// mistral_common's instruct tokenizer version, 3 or 7; absent: 3
+        #[serde(default = "mistral_instruct_default")]
+        instruct_version: u8,
+    },
+}
+
+fn mistral_instruct_default() -> u8 {
+    3
 }
 
 #[derive(Debug, Deserialize, JsonSchema)]
@@ -109,7 +125,7 @@ pub struct CountTokensRequest {
     /// chat messages (`llm-gateway-sdk/schemas/core/message.v1.schema.json`): only their `text` content parts are counted
     pub messages: Vec<serde_json::Value>,
     /// the provider's framing; absent: the sum over the text parts
-    pub template: Option<ChatTemplateDto>,
+    pub template: Option<TemplateDto>,
     /// the request's tools (`llm-gateway-sdk/schemas/tools/tool.v1.schema.json`): counted by the `mistral` template (unified tools
     /// only); any other template, or none, refuses them
     #[serde(default)]

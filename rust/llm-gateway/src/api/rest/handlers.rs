@@ -3,12 +3,13 @@
 use std::sync::Arc;
 
 use axum::{Extension, Json};
-use llm_gateway_sdk::{ChatTemplate, TokenizerClient, TokenizerError};
+use llm_gateway_sdk::{ChatTemplate, MistralInstruct, TokenizerClient, TokenizerError};
 use modkit_errors::Problem;
 use modkit_security::SecurityContext;
 
 use crate::api::rest::dto::{
-    ChatTemplateDto, ChunkRequest, ChunkResponse, CountTokensRequest, CountTokensResponse, MaxTokens, TokenizeRequest, TokenizeResponse, TruncateRequest, TruncateResponse,
+    ChatTemplateDto, ChunkRequest, ChunkResponse, CountTokensRequest, CountTokensResponse, MaxTokens, TemplateDto, TokenizeRequest, TokenizeResponse, TruncateRequest,
+    TruncateResponse,
 };
 use crate::domain::service::TokenizerService;
 
@@ -87,17 +88,29 @@ pub async fn count_tokens(
     let usage = match req.template {
         None if !req.tools.is_empty() => Err(TokenizerError::InvalidInput("tools are counted with the mistral template".to_owned())),
         None => service.count_tokens(&ctx, &req.model, &req.messages).await,
-        Some(t) => {
-            let template = match t {
-                ChatTemplateDto::Overhead { tokens_per_message, tokens_per_name, reply_priming } => ChatTemplate::Overhead { tokens_per_message, tokens_per_name, reply_priming },
-                ChatTemplateDto::Rendered { bos, message_prefix, message_suffix, generation_prompt, special_tokens } => {
-                    ChatTemplate::Rendered { bos, message_prefix, message_suffix, generation_prompt, special_tokens }
-                }
-                ChatTemplateDto::Mistral => ChatTemplate::Mistral,
-            };
-            service.count_chat_tokens_with_tools(&ctx, &req.model, &req.messages, &req.tools, &template).await
-        }
+        Some(t) => match chat_template(t) {
+            Ok(template) => service.count_chat_tokens_with_tools(&ctx, &req.model, &req.messages, &req.tools, &template).await,
+            Err(e) => Err(e),
+        },
     }
     .map_err(problem)?;
     Ok(Json(CountTokensResponse { input_tokens: usage.input_tokens }))
+}
+
+/// the template a request names or spells out
+fn chat_template(t: TemplateDto) -> Result<ChatTemplate, TokenizerError> {
+    Ok(match t {
+        TemplateDto::Named(name) => ChatTemplate::named(&name).ok_or_else(|| TokenizerError::InvalidInput(format!("unknown chat template {name:?}")))?,
+        TemplateDto::Spec(ChatTemplateDto::Overhead { tokens_per_message, tokens_per_name, reply_priming }) => ChatTemplate::Overhead { tokens_per_message, tokens_per_name, reply_priming },
+        TemplateDto::Spec(ChatTemplateDto::Rendered { bos, message_prefix, message_suffix, generation_prompt, special_tokens }) => {
+            ChatTemplate::Rendered { bos, message_prefix, message_suffix, generation_prompt, special_tokens }
+        }
+        TemplateDto::Spec(ChatTemplateDto::Mistral { instruct_version }) => ChatTemplate::Mistral {
+            instruct: match instruct_version {
+                3 => MistralInstruct::V3,
+                7 => MistralInstruct::V7,
+                v => return Err(TokenizerError::InvalidInput(format!("the mistral template counts instruct versions 3 and 7, not {v}"))),
+            },
+        },
+    })
 }

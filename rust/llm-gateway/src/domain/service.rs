@@ -8,7 +8,7 @@ use std::sync::{Arc, LazyLock};
 use async_trait::async_trait;
 use bytes::Bytes;
 use llm_gateway_sdk::{
-    ChatTemplate, CountTokensRequest, EncodeBatchRequest, InvalidUtf8, OffsetUnit, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1,
+    ChatTemplate, CountTokensRequest, EncodeBatchRequest, InvalidUtf8, MistralInstruct, OffsetUnit, SpecialTokens, TokenizerClient, TokenizerError, TokenizerPluginClient, TokenizerPluginSpecV1,
     TruncateKeep, Usage, VocabRef,
 };
 use modkit::client_hub::{ClientHub, ClientScope};
@@ -36,13 +36,14 @@ static MISTRAL_NAME: LazyLock<Regex> = LazyLock::new(|| Regex::new(r"^[a-zA-Z0-9
 static MISTRAL_CALL_ID: LazyLock<Regex> = LazyLock::new(|| Regex::new(r"^[a-zA-Z0-9]{9}\n?$").expect("a valid pattern"));
 static NULL: Value = Value::Null;
 
-/// one gateway message as the mistral template reads it: a tool call is `{"name", "arguments"[, "id"]}`, a tool result
-/// `{"content", "call_id"}`
+/// one gateway message as the mistral template reads it: its text parts, its tool calls `{"name", "arguments"[, "id"]}`, its tool
+/// result (call id, content) and its `prefix` flag (V7 only)
 struct MistralMessage {
     role: String,
-    text: String,
+    parts: Vec<String>,
     calls: Vec<Value>,
-    result: Option<Value>,
+    result: Option<(String, String)>,
+    prefix: bool,
 }
 
 /// JSON as mistral_common writes it into the prompt, Python's `json.dumps(value, ensure_ascii=False)`: ", " and ": " between
@@ -61,6 +62,15 @@ fn mistral_tool_content(content: &str) -> Value {
         return json!({});
     }
     serde_json::from_str(content).unwrap_or_else(|_| Value::from(content))
+}
+
+/// a tool result's content as mistral_common's V7 request normalizer leaves it: the JSON value it parses to, written again by
+/// `mistral_json`, else the text as given; "" is "{}"
+fn mistral_normalized_content(content: &str) -> String {
+    if content.is_empty() {
+        return "{}".to_owned();
+    }
+    serde_json::from_str::<Value>(content).map_or_else(|_| content.to_owned(), |v| mistral_json(&v))
 }
 
 struct PythonJson;
@@ -185,10 +195,11 @@ impl TokenizerService {
         }).collect()
     }
 
-    /// role, text, tool calls and tool result of one gateway message (Python mirror: `cfbpe/plugin.py:_mistral_message`); text is
-    /// its text parts joined with "\n\n", other parts (images ...) are not counted here.  A call is {"name", "arguments", "id"} as
-    /// mistral_common prints it (no "id" for "null").
-    fn mistral_message(m: &Value) -> Result<MistralMessage, TokenizerError> {
+    /// role, text parts, tool calls, tool result and prefix flag of one gateway message (Python mirror:
+    /// `cfbpe/plugin.py:_mistral_message`); other parts (images ...) are not counted here.  A call is {"name", "arguments", "id"}
+    /// as mistral_common prints it (no "id" for "null").  `prefix` (Mistral's chat API: the reply continues this assistant
+    /// message) is read under V7 only.
+    fn mistral_message(m: &Value, instruct: MistralInstruct) -> Result<MistralMessage, TokenizerError> {
         let bad = |msg: &str| TokenizerError::InvalidInput(msg.to_owned());
         let role = m.get("role").and_then(Value::as_str).unwrap_or("");
         if mistral_next_roles(role).is_empty() {
@@ -196,7 +207,12 @@ impl TokenizerService {
         }
         let parts: &[Value] = m.get("content").and_then(Value::as_array).map_or(&[], Vec::as_slice);
         let of_type = |p: &&Value, t: &str| p.get("type").and_then(Value::as_str) == Some(t);
-        let text = Self::text_parts(std::slice::from_ref(m)).join("\n\n");
+        let texts = Self::text_parts(std::slice::from_ref(m));
+        let text = texts.join("\n\n");
+        let prefix = match (instruct, m.get("prefix")) {
+            (MistralInstruct::V7, Some(p)) => p.as_bool().filter(|&p| !p || role == "assistant").ok_or_else(|| bad("prefix is a boolean of an assistant message"))?,
+            _ => false,
+        };
         let results: Vec<&Value> = parts.iter().filter(|p| of_type(p, "tool_result")).map(|p| p.get("tool_result").unwrap_or(&NULL)).collect();
         let mut calls = Vec::new();
         for p in parts.iter().filter(|p| of_type(p, "tool_call")) {
@@ -219,7 +235,7 @@ impl TokenizerService {
             }
             calls.push(call);
         }
-        if role == "assistant" && text.is_empty() == calls.is_empty() {
+        if instruct == MistralInstruct::V3 && role == "assistant" && text.is_empty() == calls.is_empty() {       // (V7: text, calls or both, once merged)
             return Err(bad(if text.is_empty() { "an assistant message without text or tool calls" } else { "an assistant message holds text or tool calls, one of the two" }));
         }
         if (role == "tool") == results.is_empty() {
@@ -235,9 +251,71 @@ impl TokenizerService {
             if !MISTRAL_CALL_ID.is_match(id) {
                 return Err(bad("a tool result's tool_call_id is 9 of a-z, A-Z and 0-9"));
             }
-            result = Some(json!({"content": mistral_tool_content(content), "call_id": id}));
+            result = Some((id.to_owned(), content.to_owned()));
         }
-        Ok(MistralMessage { role: role.to_owned(), text, calls, result })
+        Ok(MistralMessage { role: role.to_owned(), parts: texts, calls, result, prefix })
+    }
+
+    /// the texts and control tokens of a conversation under V7, on messages `mistral_message` read and the caller checked (Python
+    /// mirror: `cfbpe/plugin.py:_mistral_v7_texts`)
+    fn mistral_v7_texts(msgs: Vec<MistralMessage>, tool_defs: Vec<Value>) -> Result<(Vec<String>, u64), TokenizerError> {
+        let prefix = msgs.last().is_some_and(|m| m.prefix);
+        let mut turns: Vec<MistralMessage> = Vec::new();                    // after merging
+        let mut prev = String::new();
+        for m in msgs {
+            let role = m.role.clone();
+            if (role == "user" || role == "assistant") && role == prev {
+                let last = turns.last_mut().expect("a turn of this role");
+                last.parts.extend(m.parts);
+                last.calls.extend(m.calls);
+            } else {
+                turns.push(m);
+            }
+            prev = role;
+        }
+        let last_user = turns.iter().rposition(|t| t.role == "user");
+        let n_turns = turns.len();
+        let (mut texts, mut fixed) = (Vec::new(), 1u64);                    // <s>
+        let mut tool_defs = Some(tool_defs);
+        for (i, t) in turns.into_iter().enumerate() {
+            let text = t.parts.join("\n\n");
+            match t.role.as_str() {
+                "system" => {
+                    texts.push(text);
+                    fixed += 2;                                             // [SYSTEM_PROMPT] [/SYSTEM_PROMPT]
+                }
+                "user" => {
+                    if Some(i) == last_user {
+                        if let Some(defs) = tool_defs.take().filter(|d| !d.is_empty()) {
+                            texts.push(mistral_json(&Value::Array(defs)));
+                            fixed += 2;                                     // [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
+                        }
+                    }
+                    texts.push(text);
+                    fixed += 2;                                             // [INST] [/INST]
+                }
+                "assistant" => {
+                    if text.is_empty() && t.calls.is_empty() {
+                        return Err(TokenizerError::InvalidInput("an assistant message without text or tool calls (also once merged)".to_owned()));
+                    }
+                    texts.push(text.trim_end_matches(' ').to_owned());
+                    if !t.calls.is_empty() {
+                        texts.push(mistral_json(&Value::Array(t.calls)));
+                        fixed += 1;                                         // [TOOL_CALLS]
+                    }
+                    if !(prefix && i == n_turns - 1) {
+                        fixed += 1;                                         // </s>
+                    }
+                }
+                _ => {
+                    let (id, content) = t.result.expect("a tool message has its result");
+                    texts.push(id);
+                    texts.push(mistral_normalized_content(&content));
+                    fixed += 3;                                             // [TOOL_RESULTS] [TOOL_CONTENT] [/TOOL_RESULTS]
+                }
+            }
+        }
+        Ok((texts, fixed))
     }
 
     /// the `TextContent.text` parts of a request's messages (`schemas/core/message.v1.schema.json`)
@@ -338,7 +416,7 @@ impl TokenizerClient for TokenizerService {
         -> Result<Usage, TokenizerError> {
         // every stretch of ordinary text of the whole request, tool JSON included, goes to the device in ONE batch; control tokens
         // count one each
-        if !tools.is_empty() && *template != ChatTemplate::Mistral {
+        if !tools.is_empty() && !matches!(template, ChatTemplate::Mistral { .. }) {
             return Err(TokenizerError::InvalidInput("only the mistral chat template counts tools".to_owned()));
         }
         let content = |m: &Value| -> String {
@@ -383,19 +461,26 @@ impl TokenizerClient for TokenizerService {
                 feed(generation_prompt, &mut fixed, &mut run);
                 texts = run;
             }
-            ChatTemplate::Mistral => {
+            ChatTemplate::Mistral { instruct } => {
                 let bad = |msg: &str| TokenizerError::InvalidInput(msg.to_owned());
                 let mut tool_defs = Self::mistral_tools(tools)?;
                 if messages.is_empty() {
                     return Err(bad("a conversation for the mistral template has at least one message"));
                 }
-                let msgs = messages.iter().map(Self::mistral_message).collect::<Result<Vec<_>, _>>()?;
+                let msgs = messages.iter().map(|m| Self::mistral_message(m, *instruct)).collect::<Result<Vec<_>, _>>()?;
                 let roles: Vec<String> = msgs.iter().map(|m| m.role.clone()).collect();
+                if msgs[..msgs.len() - 1].iter().any(|m| m.prefix) {
+                    return Err(bad("an assistant message with prefix is the last message"));
+                }
                 if roles.len() == 1 && !matches!(roles[0].as_str(), "user" | "system") {
                     return Err(bad("a conversation of one message for the mistral template is a user or system message"));
                 }
-                if roles.len() > 1 && roles[roles.len() - 1] == "assistant" {
-                    return Err(bad("a conversation for the mistral template ends with a user or tool message"));
+                if roles.len() > 1 && roles[roles.len() - 1] == "assistant" && !msgs[msgs.len() - 1].prefix {
+                    return Err(bad(if *instruct == MistralInstruct::V7 {
+                        "a conversation for the mistral template ends with a user or tool message or an assistant message with prefix"
+                    } else {
+                        "a conversation for the mistral template ends with a user or tool message"
+                    }));
                 }
                 for w in roles.windows(2) {
                     if !mistral_next_roles(&w[0]).contains(&w[1].as_str()) {
@@ -411,52 +496,59 @@ impl TokenizerClient for TokenizerService {
                         _ => {}
                     }
                 }
-                let system = msgs.iter().filter(|m| m.role == "system" && !m.text.is_empty()).map(|m| m.text.as_str()).collect::<Vec<_>>().join("\n\n");
-                let mut turns: Vec<MistralMessage> = Vec::new();            // after merging
-                let mut prev = String::new();
-                for m in msgs {
-                    let role = m.role.clone();
-                    if (role == "user" || role == "assistant") && role == prev {
-                        let last = turns.last_mut().expect("a turn of this role");
-                        if m.calls.is_empty() {                             // (a message with tool calls has no text to merge)
-                            last.text.push_str("\n\n");
-                            last.text.push_str(&m.text);
-                        }
-                        last.calls.extend(m.calls);
-                        if !last.text.is_empty() && !last.calls.is_empty() {
-                            return Err(bad("merged assistant messages hold both text and tool calls"));
-                        }
-                    } else if role != "system" {
-                        turns.push(m);
-                    }
-                    prev = role;
-                }
-                if turns.first().map_or(true, |t| t.role != "user") {
-                    turns.insert(0, MistralMessage { role: "user".to_owned(), text: String::new(), calls: Vec::new(), result: None });
-                }
-                let last_user = turns.iter().rposition(|t| t.role == "user").expect("a user turn");
-                fixed = 1;                                                  // <s>
-                for (i, t) in turns.into_iter().enumerate() {
-                    match t.role.as_str() {
-                        "user" => {
-                            if i == last_user && !tool_defs.is_empty() {
-                                texts.push(mistral_json(&Value::Array(std::mem::take(&mut tool_defs))));
-                                fixed += 2;                                 // [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
+                if *instruct == MistralInstruct::V7 {
+                    (texts, fixed) = Self::mistral_v7_texts(msgs, tool_defs)?;
+                } else {
+                    // V3: the texts are each message's text parts joined with "\n\n"
+                    let system = msgs.iter().filter(|m| m.role == "system").map(|m| m.parts.join("\n\n")).filter(|t| !t.is_empty()).collect::<Vec<_>>().join("\n\n");
+                    let mut turns: Vec<(String, String, Vec<Value>, Option<(String, String)>)> = Vec::new();   // (role, text, calls, result) after merging
+                    let mut prev = String::new();
+                    for m in msgs {
+                        let role = m.role.clone();
+                        let text = m.parts.join("\n\n");
+                        if (role == "user" || role == "assistant") && role == prev {
+                            let last = turns.last_mut().expect("a turn of this role");
+                            if m.calls.is_empty() {                         // (a message with tool calls has no text to merge)
+                                last.1.push_str("\n\n");
+                                last.1.push_str(&text);
                             }
-                            texts.push(if i == last_user && !system.is_empty() { format!("{system}\n\n{}", t.text) } else { t.text });
-                            fixed += 2;                                     // [INST] [/INST]
+                            last.2.extend(m.calls);
+                            if !last.1.is_empty() && !last.2.is_empty() {
+                                return Err(bad("merged assistant messages hold both text and tool calls"));
+                            }
+                        } else if role != "system" {
+                            turns.push((role.clone(), text, m.calls, m.result));
                         }
-                        "assistant" if !t.calls.is_empty() => {
-                            texts.push(mistral_json(&Value::Array(t.calls)));
-                            fixed += 2;                                     // [TOOL_CALLS] </s>
-                        }
-                        "assistant" => {
-                            texts.push(t.text.trim_end_matches(' ').to_owned());
-                            fixed += 1;                                     // </s>
-                        }
-                        _ => {
-                            texts.push(mistral_json(t.result.as_ref().expect("a tool message has its result")));
-                            fixed += 2;                                     // [TOOL_RESULTS] [/TOOL_RESULTS]
+                        prev = role;
+                    }
+                    if turns.first().map_or(true, |t| t.0 != "user") {
+                        turns.insert(0, ("user".to_owned(), String::new(), Vec::new(), None));
+                    }
+                    let last_user = turns.iter().rposition(|t| t.0 == "user").expect("a user turn");
+                    fixed = 1;                                              // <s>
+                    for (i, (role, text, calls, result)) in turns.into_iter().enumerate() {
+                        match role.as_str() {
+                            "user" => {
+                                if i == last_user && !tool_defs.is_empty() {
+                                    texts.push(mistral_json(&Value::Array(std::mem::take(&mut tool_defs))));
+                                    fixed += 2;                             // [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
+                                }
+                                texts.push(if i == last_user && !system.is_empty() { format!("{system}\n\n{text}") } else { text });
+                                fixed += 2;                                 // [INST] [/INST]
+                            }
+                            "assistant" if !calls.is_empty() => {
+                                texts.push(mistral_json(&Value::Array(calls)));
+                                fixed += 2;                                 // [TOOL_CALLS] </s>
+                            }
+                            "assistant" => {
+                                texts.push(text.trim_end_matches(' ').to_owned());
+                                fixed += 1;                                 // </s>
+                            }
+                            _ => {
+                                let (id, content) = result.expect("a tool message has its result");
+                                texts.push(mistral_json(&json!({"content": mistral_tool_content(&content), "call_id": id})));
+                                fixed += 2;                                 // [TOOL_RESULTS] [/TOOL_RESULTS]
+                            }
                         }
                     }
                 }
