@@ -322,11 +322,12 @@ class ChatTemplate:
     "rendered"  the conversation is rendered to text around control tokens (Llama 3, Mistral): `bos`, then per message
                 `message_prefix.format(role=...)` + content + `message_suffix`, then `generation_prompt`; the strings in
                 `special_tokens` count one token each, the text between them is tokenised as ordinary text;
-    "mistral"   mistral_common's InstructTokenizer of `instruct_version` 3 (Tekken models: Mistral NeMo, Pixtral 12B) or 7 (Mistral
-                Large 2411, Pixtral Large 2411, Mistral Small 2501 and 2503) on a conversation of text, tool calls and tool results,
-                with the request's tools: mistral_instruct_texts gives the rules and the refusals.  Every message's text, the tools'
-                JSON, each assistant turn's calls and each tool result are tokenised on their own, between control tokens
-                ([AVAILABLE_TOOLS] before the last [INST], [TOOL_CALLS], [TOOL_RESULTS]; V7 also [SYSTEM_PROMPT], [TOOL_CONTENT]).
+    "mistral"   mistral_common's InstructTokenizer of `instruct_version` 3 (Tekken models: Mistral NeMo, Pixtral 12B), 7 (Mistral
+                Large 2411, Pixtral Large 2411, Mistral Small 2501 and 2503), 11 or 13 on a conversation of text, tool calls and tool
+                results, with the request's tools: mistral_instruct_texts (V3, V7) and mistral_instruct_texts_v11 (V11, V13) give
+                the rules and the refusals.  Every message's text, the tools' JSON, each assistant turn's calls and each tool result
+                are tokenised on their own, between control tokens ([AVAILABLE_TOOLS] before the last [INST] (V13: the first), [TOOL_CALLS], [TOOL_RESULTS]; V7 and later also
+                [SYSTEM_PROMPT], [TOOL_CONTENT] (not V13); V11 and V13 also [ARGS], and V11 [CALL_ID]).
                 The other kinds refuse tools; they pass over tool_call and tool_result parts.
 
     Message CONTENT is always ordinary text: a message that spells a control token gets the pieces of that spelling, never the
@@ -340,7 +341,7 @@ class ChatTemplate:
     message_suffix: str = ""
     generation_prompt: str = ""
     special_tokens: Tuple[str, ...] = ()
-    instruct_version: int = 3           # "mistral": mistral_common's instruct tokenizer version, 3 or 7
+    instruct_version: int = 3           # "mistral": mistral_common's instruct tokenizer version, 3, 7, 11 or 13
 
 
 # templates of the model families the stand-in vocabularies cover; a deployment lists its own next to the model's tokenizer
@@ -354,6 +355,11 @@ CHAT_TEMPLATES = {
     # Mistral's V7 Tekken models (InstructTokenizerV7): system messages in place as [SYSTEM_PROMPT] text [/SYSTEM_PROMPT], tool
     # results as [TOOL_RESULTS] call id [TOOL_CONTENT] content [/TOOL_RESULTS]
     "mistral-v7": ChatTemplate("mistral", instruct_version=7),
+    # InstructTokenizerV11: V7, with each tool call as [TOOL_CALLS] name [CALL_ID] id [ARGS] arguments
+    "mistral-v11": ChatTemplate("mistral", instruct_version=11),
+    # InstructTokenizerV13: V11 without call ids, tool results as [TOOL_RESULTS] content [/TOOL_RESULTS], tools before the first
+    # user message
+    "mistral-v13": ChatTemplate("mistral", instruct_version=13),
     "llama3-instruct": ChatTemplate("rendered", bos="<|begin_of_text|>",
                                     message_prefix="<|start_header_id|>{role}<|end_header_id|>\n\n", message_suffix="<|eot_id|>",
                                     generation_prompt="<|start_header_id|>assistant<|end_header_id|>\n\n",
@@ -414,13 +420,13 @@ def _mistral_tools(tools: Sequence[dict]) -> List[dict]:
 def _mistral_message(m: dict, version: int = 3) -> Tuple[str, List[str], List[dict], Optional[Tuple[str, str]], bool]:
     """(role, text parts, tool calls, tool result (call id, content), prefix) of one gateway message; other parts (images ...)
     are not counted here.  A call is {"name", "arguments", "id"} as mistral_common prints it (no "id" for "null").  prefix is
-    the `prefix` flag of an assistant message (Mistral's chat API: the reply continues this message), read under V7 only."""
+    the `prefix` flag of an assistant message (Mistral's chat API: the reply continues this message), read under V7 and later."""
     role, parts = m.get("role"), m.get("content", [])
     if role not in MISTRAL_NEXT_ROLES:
         raise InvalidInput("the mistral template counts system, user, assistant and tool messages, not %r" % role)
     texts = [str(p["text"]) for p in parts if p.get("type") == "text"]
     text = "\n\n".join(texts)
-    prefix = m.get("prefix", False) if version == 7 else False
+    prefix = m.get("prefix", False) if version >= 7 else False
     if not isinstance(prefix, bool) or (prefix and role != "assistant"):
         raise InvalidInput("prefix is a boolean of an assistant message")
     calls, results = [], [p.get("tool_result") for p in parts if p.get("type") == "tool_result"]
@@ -435,6 +441,8 @@ def _mistral_message(m: dict, version: int = 3) -> Tuple[str, List[str], List[di
             raise InvalidInput("a tool call has a string id and name and object arguments")
         if cid != "null" and not MISTRAL_CALL_ID.fullmatch(cid):
             raise InvalidInput("a tool call id is 9 of a-z, A-Z and 0-9")
+        if cid == "null" and version == 13:
+            raise InvalidInput("a tool call has an id under instruct V13")
         if not MISTRAL_NAME.fullmatch(name):
             raise InvalidInput("a tool call's name is 1 to 64 of a-z, A-Z, 0-9, '_' and '-'")
         calls.append({"name": name, "arguments": args, **({} if cid == "null" else {"id": cid})})
@@ -494,9 +502,37 @@ def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[di
         written again, else the text as given ("" is "{}");
       - the last message may be an assistant message with "prefix": true, the start of the reply: its turn has no </s>.  prefix on
         any other message is refused;
-      - the tools go before the last user message's [INST]; a conversation without a user message does not show them."""
+      - the tools go before the last user message's [INST]; a conversation without a user message does not show them.
+
+    Other versions are refused; mistral_instruct_texts_v11 gives versions 11 and 13."""
     if version not in (3, 7):
-        raise InvalidInput("the mistral template counts instruct versions 3 and 7, not %r" % (version,))
+        raise InvalidInput("mistral_instruct_texts counts instruct versions 3 and 7 (11 and 13: mistral_instruct_texts_v11), "
+                           "not %r" % (version,))
+    return _mistral_texts(messages, tools, version)
+
+
+def mistral_instruct_texts_v11(messages: Sequence[dict], tools: Optional[Sequence[dict]] = None, version: int = 11) -> Tuple[List[str], int]:
+    """mistral_instruct_texts for mistral_common 1.11's InstructTokenizerV11 (version 11) or InstructTokenizerV13 (version 13),
+    both with MistralRequestValidatorV13 (default mode) and InstructRequestNormalizerV13: (the ordinary texts in order, the
+    number of control tokens).  They are version 7, except:
+      - V11: each call of an assistant turn is [TOOL_CALLS] its name, then [CALL_ID] its id when the id is not "null", then
+        [ARGS] its arguments' JSON (no list);
+      - V13: as V11 without [CALL_ID] and its id, and a call's id is required ("null" is refused); a tool result is
+        [TOOL_RESULTS] content [/TOOL_RESULTS] (no call id, no [TOOL_CONTENT]); the tools go before the FIRST user message;
+      - both: the tool messages after an assistant message answer its calls by id: a result whose id is not among the ids of
+        the calls of the assistant message before it, or answers one of them twice, is refused, and so are two calls of one
+        message with one id; an assistant message while the calls of the one before it do not all have their result is refused
+        (the first message is not checked).  The normalizer puts each run of results in the order of their calls, which does not
+        change the count.
+    Other versions are refused (3 and 7: mistral_instruct_texts)."""
+    if version not in (11, 13):
+        raise InvalidInput("mistral_instruct_texts_v11 counts instruct versions 11 and 13 (3 and 7: mistral_instruct_texts), "
+                           "not %r" % (version,))
+    return _mistral_texts(messages, tools, version)
+
+
+def _mistral_texts(messages: Sequence[dict], tools: Optional[Sequence[dict]], version: int) -> Tuple[List[str], int]:
+    """mistral_instruct_texts (version 3 or 7) and mistral_instruct_texts_v11 (version 11 or 13), on a version they take"""
     tool_defs = _mistral_tools(tools or ())
     if not messages:
         raise InvalidInput("a conversation for the mistral template has at least one message")
@@ -508,20 +544,23 @@ def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[di
         raise InvalidInput("a conversation of one message for the mistral template is a user or system message")
     if len(roles) > 1 and roles[-1] == "assistant" and not msgs[-1][4]:
         raise InvalidInput("a conversation for the mistral template ends with a user or tool message" +
-                           (" or an assistant message with prefix" if version == 7 else ""))
+                           (" or an assistant message with prefix" if version >= 7 else ""))
     for prev, role in zip(roles, roles[1:]):
         if role not in MISTRAL_NEXT_ROLES[prev]:
             raise InvalidInput("a message of role %r follows one of role %r" % (role, prev))
-    pending = 0                         # tool messages the last tool-calling assistant message still waits for
-    for role, _, calls, _, _ in msgs[1:]:
-        if role == "tool":
-            pending -= 1
-        elif role == "assistant":
-            if pending:
-                raise InvalidInput("an assistant message follows tool calls without exactly one tool message each")
-            pending = len(calls)
-    if version == 7:
-        return _mistral_v7_texts(msgs, tool_defs)
+    if version >= 11:
+        _check_mistral_call_ids(msgs)
+    else:
+        pending = 0                     # tool messages the last tool-calling assistant message still waits for
+        for role, _, calls, _, _ in msgs[1:]:
+            if role == "tool":
+                pending -= 1
+            elif role == "assistant":
+                if pending:
+                    raise InvalidInput("an assistant message follows tool calls without exactly one tool message each")
+                pending = len(calls)
+    if version >= 7:
+        return _mistral_v7_texts(msgs, tool_defs, version)
     system = "\n\n".join(t for t in ("\n\n".join(parts) for role, parts, _, _, _ in msgs if role == "system") if t)
     turns: List[list] = []              # [role, text, calls, result] after merging
     prev = None
@@ -557,8 +596,29 @@ def mistral_instruct_texts(messages: Sequence[dict], tools: Optional[Sequence[di
     return texts, controls
 
 
-def _mistral_v7_texts(msgs: Sequence[tuple], tool_defs: List[dict]) -> Tuple[List[str], int]:
-    """mistral_instruct_texts under version 7, on messages _mistral_message read and mistral_instruct_texts checked"""
+def _check_mistral_call_ids(msgs: Sequence[tuple]) -> None:
+    """MistralRequestValidatorV13's check of tool results against the calls they answer (instruct V11 and V13), on messages
+    _mistral_message read: the first message is not checked"""
+    expected, answered = set(), set()   # the call ids of the last assistant message, the ones its tool messages answered
+    for role, _, calls, result, _ in msgs[1:]:
+        if role == "tool":
+            if result[0] in answered:
+                raise InvalidInput("two tool results answer the call %r" % result[0])
+            if result[0] not in expected:
+                raise InvalidInput("a tool result answers %r, not a call of the assistant message before it" % result[0])
+            answered.add(result[0])
+        elif role == "assistant":
+            if len(answered) != len(expected):
+                raise InvalidInput("an assistant message follows tool calls without a tool result each")
+            expected, answered = set(), set()
+            for c in calls:
+                if c.get("id", "null") in expected:
+                    raise InvalidInput("two tool calls of one assistant message have the id %r" % c.get("id", "null"))
+                expected.add(c.get("id", "null"))
+
+
+def _mistral_v7_texts(msgs: Sequence[tuple], tool_defs: List[dict], version: int) -> Tuple[List[str], int]:
+    """mistral_instruct_texts under version 7, 11 or 13, on messages _mistral_message read and mistral_instruct_texts checked"""
     turns: List[list] = []              # [role, text parts, calls, result] after merging
     prev = None
     for role, parts, calls, result, _ in msgs:
@@ -568,7 +628,8 @@ def _mistral_v7_texts(msgs: Sequence[tuple], tool_defs: List[dict]) -> Tuple[Lis
         else:
             turns.append([role, list(parts), list(calls), result])
         prev = role
-    last_user = max((i for i, t in enumerate(turns) if t[0] == "user"), default=-1)
+    users = [i for i, t in enumerate(turns) if t[0] == "user"]
+    tools_at = (users[0] if version == 13 else users[-1]) if users else -1
     prefix = msgs[-1][4]
     texts, controls = [], 1             # <s>
     for i, (role, parts, calls, result) in enumerate(turns):
@@ -577,7 +638,7 @@ def _mistral_v7_texts(msgs: Sequence[tuple], tool_defs: List[dict]) -> Tuple[Lis
             texts.append(text)
             controls += 2               # [SYSTEM_PROMPT] [/SYSTEM_PROMPT]
         elif role == "user":
-            if i == last_user and tool_defs:
+            if i == tools_at and tool_defs:
                 texts.append(_mistral_json(tool_defs))
                 controls += 2           # [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
             texts.append(text)
@@ -586,11 +647,21 @@ def _mistral_v7_texts(msgs: Sequence[tuple], tool_defs: List[dict]) -> Tuple[Lis
             if not text and not calls:
                 raise InvalidInput("an assistant message without text or tool calls (also once merged)")
             texts.append(text.rstrip(" "))
-            if calls:
+            if calls and version == 7:
                 texts.append(_mistral_json(calls))
                 controls += 1           # [TOOL_CALLS]
+            for c in calls if version >= 11 else ():
+                texts.append(c["name"])
+                if version == 11 and "id" in c:
+                    texts.append(c["id"])
+                    controls += 1       # [CALL_ID]
+                texts.append(_mistral_json(c["arguments"]))
+                controls += 2           # [TOOL_CALLS] [ARGS]
             if not (prefix and i == len(turns) - 1):
                 controls += 1           # </s>
+        elif version == 13:
+            texts.append(_mistral_normalized_content(result[1]))
+            controls += 2               # [TOOL_RESULTS] [/TOOL_RESULTS]
         else:
             call_id, content = result
             texts += [call_id, _mistral_normalized_content(content)]
@@ -1111,7 +1182,8 @@ class LlmGatewayTokenizerService:
         """`Usage.input_tokens` of one chat request as the provider counts it: content AND framing (ChatTemplate).
         messages: [{"role": "user", "name": optional, "content": [{"type": "text", "text": ...}, ...]}, ...]; parts that are
         not text (images ...) are priced elsewhere.  tools: the request's `tools` (schemas/tools/tool.v1), counted by the "mistral"
-        kind only, which also counts tool_call and tool_result parts (mistral_instruct_texts, by the template's instruct version);
+        kind only, which also counts tool_call and tool_result parts (mistral_instruct_texts, or mistral_instruct_texts_v11 for
+        instruct versions 11 and 13);
         the other kinds refuse tools and pass over those parts.  Every stretch of text of the whole request, tool JSON included, goes to the device in ONE batch."""
         import re
         if tools and template.kind != "mistral":
@@ -1154,7 +1226,8 @@ class LlmGatewayTokenizerService:
             feed_framing(template.generation_prompt)
             texts = [t for t in run if t]
         elif template.kind == "mistral":
-            texts, fixed = mistral_instruct_texts(messages, tools, template.instruct_version)
+            texts_of = mistral_instruct_texts_v11 if template.instruct_version in (11, 13) else mistral_instruct_texts
+            texts, fixed = texts_of(messages, tools, template.instruct_version)
         else:
             raise InvalidInput("unknown chat template kind %r" % template.kind)
         texts = [t for t in texts if t]

@@ -18,7 +18,8 @@ The "tekken" vocabulary speaks raw ranks 0..n-1 of the rank file (the stand-in s
 tekken_240718 and Pixtral's tekken_240911 hold the same first 130072 ranks, so both models use the committed 240911 file.
 Mistral's instruct-V7 models (Large 2411, Pixtral Large 2411, Small 2501 and 2503) map to "mistral_tekken" too, as a stand-in:
 their own tekken.json files are not here (MODEL_TOKENIZERS labels them stand_in=True).  A model's chat template sits in its
-MODEL_TOKENIZERS entry, beside its vocabulary, so the gateway never infers it from the model's name.
+MODEL_TOKENIZERS entry, beside its vocabulary, so the gateway never infers it from the model's name.  No model maps to the
+instruct V11 or V13 templates: the repository holds no source for any model's instruct version, so they are used by name.
 """
 import hashlib
 import json

@@ -228,10 +228,10 @@ pub enum ChatTemplate {
     Rendered { bos: String, message_prefix: String, message_suffix: String, generation_prompt: String, special_tokens: Vec<String> },
     /// mistral_common's instruct tokenizer of version `instruct` (Tekken models) on a conversation of text, tool calls and tool
     /// results, with the request's tools (`TokenizerClient::count_chat_tokens_with_tools`); the rules and refusals are those of
-    /// `cfbpe/plugin.py:mistral_instruct_texts`.  V3: system texts join the last user message, runs of one role merge with "\n\n",
-    /// `<s>` + `[INST]` text `[/INST]` per user message (the tools' JSON between `[AVAILABLE_TOOLS]` and `[/AVAILABLE_TOOLS]`
+    /// `cfbpe/plugin.py:mistral_instruct_texts` (V11 and V13: `mistral_instruct_texts_v11`).  V3: system texts join the last user
+    /// message, runs of one role merge with "\n\n", `<s>` + `[INST]` text `[/INST]` per user message (the tools' JSON between `[AVAILABLE_TOOLS]` and `[/AVAILABLE_TOOLS]`
     /// before the last one) + text `</s>` or `[TOOL_CALLS]` calls `</s>` per assistant message + `[TOOL_RESULTS]` result
-    /// `[/TOOL_RESULTS]` per tool message, each text and JSON encoded on its own.  V7: see [`MistralInstruct::V7`]
+    /// `[/TOOL_RESULTS]` per tool message, each text and JSON encoded on its own.  V7, V11 and V13: see [`MistralInstruct`]
     Mistral { instruct: MistralInstruct },
 }
 
@@ -242,6 +242,8 @@ impl ChatTemplate {
             "openai-chatml" => Some(Self::Overhead { tokens_per_message: 3, tokens_per_name: 1, reply_priming: 3 }),
             "mistral-v3" => Some(Self::Mistral { instruct: MistralInstruct::V3 }),
             "mistral-v7" => Some(Self::Mistral { instruct: MistralInstruct::V7 }),
+            "mistral-v11" => Some(Self::Mistral { instruct: MistralInstruct::V11 }),
+            "mistral-v13" => Some(Self::Mistral { instruct: MistralInstruct::V13 }),
             "llama3-instruct" => Some(Self::Rendered {
                 bos: "<|begin_of_text|>".to_owned(),
                 message_prefix: "<|start_header_id|>{role}<|end_header_id|>\n\n".to_owned(),
@@ -265,6 +267,13 @@ pub enum MistralInstruct {
     /// result is `[TOOL_RESULTS]` call id `[TOOL_CONTENT]` content `[/TOOL_RESULTS]` (the content's JSON written again, else as
     /// given, "" as "{}"); a last assistant message with `"prefix": true` has no `</s>`
     V7,
+    /// InstructTokenizerV11: V7, except that each call of an assistant turn is `[TOOL_CALLS]` name, `[CALL_ID]` id (when the id
+    /// is not "null"), `[ARGS]` arguments' JSON; tool results answer the calls of the assistant message before them by id, each
+    /// once (MistralRequestValidatorV13)
+    V11,
+    /// InstructTokenizerV13: V11 without `[CALL_ID]` (a call's id is required, "null" is refused); a tool result is
+    /// `[TOOL_RESULTS]` content `[/TOOL_RESULTS]`; the tools go before the FIRST user message
+    V13,
 }
 
 /// `gts.x.llmgw.core.usage.v1~` (`llm-gateway-sdk/schemas/core/usage.v1.schema.json:8-12`)

@@ -93,7 +93,8 @@ pub struct ChunkResponse {
 }
 
 /// How the provider frames the messages (`llm_gateway_sdk::ChatTemplate`): a template's name (`ChatTemplate::named`:
-/// "openai-chatml", "mistral-v3", "mistral-v7", "llama3-instruct") or the template spelled out; absent: content only.
+/// "openai-chatml", "mistral-v3", "mistral-v7", "mistral-v11", "mistral-v13", "llama3-instruct") or the template spelled out;
+/// absent: content only.
 #[derive(Debug, Deserialize, JsonSchema)]
 #[serde(untagged)]
 pub enum TemplateDto {
@@ -107,7 +108,7 @@ pub enum ChatTemplateDto {
     Overhead { tokens_per_message: u32, tokens_per_name: u32, reply_priming: u32 },
     Rendered { bos: String, message_prefix: String, message_suffix: String, generation_prompt: String, special_tokens: Vec<String> },
     Mistral {
-        /// mistral_common's instruct tokenizer version, 3 or 7; absent: 3
+        /// mistral_common's instruct tokenizer version, 3, 7, 11 or 13; absent: 3
         #[serde(default = "mistral_instruct_default")]
         instruct_version: u8,
     },

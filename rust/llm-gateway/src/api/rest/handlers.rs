@@ -109,7 +109,9 @@ fn chat_template(t: TemplateDto) -> Result<ChatTemplate, TokenizerError> {
             instruct: match instruct_version {
                 3 => MistralInstruct::V3,
                 7 => MistralInstruct::V7,
-                v => return Err(TokenizerError::InvalidInput(format!("the mistral template counts instruct versions 3 and 7, not {v}"))),
+                11 => MistralInstruct::V11,
+                13 => MistralInstruct::V13,
+                v => return Err(TokenizerError::InvalidInput(format!("the mistral template counts instruct versions 3, 7, 11 and 13, not {v}"))),
             },
         },
     })

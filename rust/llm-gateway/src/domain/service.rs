@@ -198,7 +198,7 @@ impl TokenizerService {
     /// role, text parts, tool calls, tool result and prefix flag of one gateway message (Python mirror:
     /// `cfbpe/plugin.py:_mistral_message`); other parts (images ...) are not counted here.  A call is {"name", "arguments", "id"}
     /// as mistral_common prints it (no "id" for "null").  `prefix` (Mistral's chat API: the reply continues this assistant
-    /// message) is read under V7 only.
+    /// message) is read under V7 and later.
     fn mistral_message(m: &Value, instruct: MistralInstruct) -> Result<MistralMessage, TokenizerError> {
         let bad = |msg: &str| TokenizerError::InvalidInput(msg.to_owned());
         let role = m.get("role").and_then(Value::as_str).unwrap_or("");
@@ -210,7 +210,7 @@ impl TokenizerService {
         let texts = Self::text_parts(std::slice::from_ref(m));
         let text = texts.join("\n\n");
         let prefix = match (instruct, m.get("prefix")) {
-            (MistralInstruct::V7, Some(p)) => p.as_bool().filter(|&p| !p || role == "assistant").ok_or_else(|| bad("prefix is a boolean of an assistant message"))?,
+            (MistralInstruct::V7 | MistralInstruct::V11 | MistralInstruct::V13, Some(p)) => p.as_bool().filter(|&p| !p || role == "assistant").ok_or_else(|| bad("prefix is a boolean of an assistant message"))?,
             _ => false,
         };
         let results: Vec<&Value> = parts.iter().filter(|p| of_type(p, "tool_result")).map(|p| p.get("tool_result").unwrap_or(&NULL)).collect();
@@ -225,6 +225,9 @@ impl TokenizerService {
             };
             if id != "null" && !MISTRAL_CALL_ID.is_match(id) {
                 return Err(bad("a tool call id is 9 of a-z, A-Z and 0-9"));
+            }
+            if id == "null" && instruct == MistralInstruct::V13 {
+                return Err(bad("a tool call has an id under instruct V13"));
             }
             if !MISTRAL_NAME.is_match(name) {
                 return Err(bad("a tool call's name is 1 to 64 of a-z, A-Z, 0-9, '_' and '-'"));
@@ -256,9 +259,44 @@ impl TokenizerService {
         Ok(MistralMessage { role: role.to_owned(), parts: texts, calls, result, prefix })
     }
 
-    /// the texts and control tokens of a conversation under V7, on messages `mistral_message` read and the caller checked (Python
-    /// mirror: `cfbpe/plugin.py:_mistral_v7_texts`)
-    fn mistral_v7_texts(msgs: Vec<MistralMessage>, tool_defs: Vec<Value>) -> Result<(Vec<String>, u64), TokenizerError> {
+    /// MistralRequestValidatorV13's check of tool results against the calls they answer (V11 and V13), on messages
+    /// `mistral_message` read: the first message is not checked (Python mirror: `cfbpe/plugin.py:_check_mistral_call_ids`)
+    fn check_mistral_call_ids(msgs: &[MistralMessage]) -> Result<(), TokenizerError> {
+        let bad = |msg: String| TokenizerError::InvalidInput(msg);
+        let (mut expected, mut answered) = (std::collections::HashSet::new(), std::collections::HashSet::new());
+        for m in &msgs[1..] {
+            match m.role.as_str() {
+                "tool" => {
+                    let id = m.result.as_ref().expect("a tool message has its result").0.as_str();
+                    if answered.contains(id) {
+                        return Err(bad(format!("two tool results answer the call {id:?}")));
+                    }
+                    if !expected.contains(id) {
+                        return Err(bad(format!("a tool result answers {id:?}, not a call of the assistant message before it")));
+                    }
+                    answered.insert(id);
+                }
+                "assistant" => {
+                    if answered.len() != expected.len() {
+                        return Err(bad("an assistant message follows tool calls without a tool result each".to_owned()));
+                    }
+                    (expected, answered) = (std::collections::HashSet::new(), std::collections::HashSet::new());
+                    for c in &m.calls {
+                        let id = c.get("id").and_then(Value::as_str).unwrap_or("null");
+                        if !expected.insert(id) {
+                            return Err(bad(format!("two tool calls of one assistant message have the id {id:?}")));
+                        }
+                    }
+                }
+                _ => {}
+            }
+        }
+        Ok(())
+    }
+
+    /// the texts and control tokens of a conversation under V7, V11 or V13, on messages `mistral_message` read and the caller
+    /// checked (Python mirror: `cfbpe/plugin.py:_mistral_v7_texts`)
+    fn mistral_v7_texts(msgs: Vec<MistralMessage>, tool_defs: Vec<Value>, instruct: MistralInstruct) -> Result<(Vec<String>, u64), TokenizerError> {
         let prefix = msgs.last().is_some_and(|m| m.prefix);
         let mut turns: Vec<MistralMessage> = Vec::new();                    // after merging
         let mut prev = String::new();
@@ -273,7 +311,11 @@ impl TokenizerService {
             }
             prev = role;
         }
-        let last_user = turns.iter().rposition(|t| t.role == "user");
+        let tools_at = if instruct == MistralInstruct::V13 {
+            turns.iter().position(|t| t.role == "user")
+        } else {
+            turns.iter().rposition(|t| t.role == "user")
+        };
         let n_turns = turns.len();
         let (mut texts, mut fixed) = (Vec::new(), 1u64);                    // <s>
         let mut tool_defs = Some(tool_defs);
@@ -285,7 +327,7 @@ impl TokenizerService {
                     fixed += 2;                                             // [SYSTEM_PROMPT] [/SYSTEM_PROMPT]
                 }
                 "user" => {
-                    if Some(i) == last_user {
+                    if Some(i) == tools_at {
                         if let Some(defs) = tool_defs.take().filter(|d| !d.is_empty()) {
                             texts.push(mistral_json(&Value::Array(defs)));
                             fixed += 2;                                     // [AVAILABLE_TOOLS] [/AVAILABLE_TOOLS]
@@ -299,9 +341,19 @@ impl TokenizerService {
                         return Err(TokenizerError::InvalidInput("an assistant message without text or tool calls (also once merged)".to_owned()));
                     }
                     texts.push(text.trim_end_matches(' ').to_owned());
-                    if !t.calls.is_empty() {
+                    if instruct == MistralInstruct::V7 && !t.calls.is_empty() {
                         texts.push(mistral_json(&Value::Array(t.calls)));
                         fixed += 1;                                         // [TOOL_CALLS]
+                    } else {
+                        for c in t.calls {
+                            texts.push(c["name"].as_str().expect("a call has a name").to_owned());
+                            if let (MistralInstruct::V11, Some(id)) = (instruct, c.get("id").and_then(Value::as_str)) {
+                                texts.push(id.to_owned());
+                                fixed += 1;                                 // [CALL_ID]
+                            }
+                            texts.push(mistral_json(&c["arguments"]));
+                            fixed += 2;                                     // [TOOL_CALLS] [ARGS]
+                        }
                     }
                     if !(prefix && i == n_turns - 1) {
                         fixed += 1;                                         // </s>
@@ -309,9 +361,14 @@ impl TokenizerService {
                 }
                 _ => {
                     let (id, content) = t.result.expect("a tool message has its result");
-                    texts.push(id);
-                    texts.push(mistral_normalized_content(&content));
-                    fixed += 3;                                             // [TOOL_RESULTS] [TOOL_CONTENT] [/TOOL_RESULTS]
+                    if instruct == MistralInstruct::V13 {
+                        texts.push(mistral_normalized_content(&content));
+                        fixed += 2;                                         // [TOOL_RESULTS] [/TOOL_RESULTS]
+                    } else {
+                        texts.push(id);
+                        texts.push(mistral_normalized_content(&content));
+                        fixed += 3;                                         // [TOOL_RESULTS] [TOOL_CONTENT] [/TOOL_RESULTS]
+                    }
                 }
             }
         }
@@ -476,7 +533,7 @@ impl TokenizerClient for TokenizerService {
                     return Err(bad("a conversation of one message for the mistral template is a user or system message"));
                 }
                 if roles.len() > 1 && roles[roles.len() - 1] == "assistant" && !msgs[msgs.len() - 1].prefix {
-                    return Err(bad(if *instruct == MistralInstruct::V7 {
+                    return Err(bad(if *instruct != MistralInstruct::V3 {
                         "a conversation for the mistral template ends with a user or tool message or an assistant message with prefix"
                     } else {
                         "a conversation for the mistral template ends with a user or tool message"
@@ -487,17 +544,21 @@ impl TokenizerClient for TokenizerService {
                         return Err(TokenizerError::InvalidInput(format!("a message of role {:?} follows one of role {:?}", w[1], w[0])));
                     }
                 }
-                let mut pending = 0i64;                                     // tool messages the last tool-calling assistant message still waits for
-                for m in &msgs[1..] {
-                    match m.role.as_str() {
-                        "tool" => pending -= 1,
-                        "assistant" if pending != 0 => return Err(bad("an assistant message follows tool calls without exactly one tool message each")),
-                        "assistant" => pending = m.calls.len() as i64,
-                        _ => {}
+                if matches!(instruct, MistralInstruct::V11 | MistralInstruct::V13) {
+                    Self::check_mistral_call_ids(&msgs)?;
+                } else {
+                    let mut pending = 0i64;                                 // tool messages the last tool-calling assistant message still waits for
+                    for m in &msgs[1..] {
+                        match m.role.as_str() {
+                            "tool" => pending -= 1,
+                            "assistant" if pending != 0 => return Err(bad("an assistant message follows tool calls without exactly one tool message each")),
+                            "assistant" => pending = m.calls.len() as i64,
+                            _ => {}
+                        }
                     }
                 }
-                if *instruct == MistralInstruct::V7 {
-                    (texts, fixed) = Self::mistral_v7_texts(msgs, tool_defs)?;
+                if *instruct != MistralInstruct::V3 {
+                    (texts, fixed) = Self::mistral_v7_texts(msgs, tool_defs, *instruct)?;
                 } else {
                     // V3: the texts are each message's text parts joined with "\n\n"
                     let system = msgs.iter().filter(|m| m.role == "system").map(|m| m.parts.join("\n\n")).filter(|t| !t.is_empty()).collect::<Vec<_>>().join("\n\n");
